@@ -2,11 +2,11 @@
 """Benchmark of the D-MPNN hot path (BASELINE.json): molecules/sec, forward+backward, of the message-passing encoder +
 aggregation on synthetic molecule batches.
 
-    python bench.py [--config C2|C3|C4|C5] [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--config C2|C3|C4|C5] [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Configurations (BASELINE.json `configs`; C1 is the reference's CPU plumbing case and lives in the tests):
   C2  10 k ~25-atom molecules / GPU, BondMessagePassing h=300 depth=3, bf16 tier, fused depth step   (default, weak scaling)
-  C3  50 k molecules, h=600 depth=6, fp32 tier (3xTF32 tensor-core GEMMs)
+  C3  20 k molecules, h=600 depth=6, fp32 tier (3xTF32 tensor-core GEMMs)
   C4  10 k ~80-atom condensed-reaction graphs (d_v=106, d_e=28), AtomMessagePassing h=300 depth=3, bf16 tier
   C5  1 M molecules, global batch 200 k = 8 micro-batches of 25 k, sharded over the ranks by the loader
       (DistributedSampler semantics), gradient accumulation + ONE all-reduce per step                     (strong scaling)
@@ -24,6 +24,9 @@ Prints ONE JSON line (rank 0):
  cpu_baseline  the oracle port (the reference's own op sequence on torch CPU) on the host cores, bounded sample
 
 `--impl reference` times that CPU implementation on the SAME workload (full batch per step) on the host's cores.
+`--dump-outputs DIR` writes what the last timed step computed (DIR/<name>.npy: loss, aggregated fingerprints, node-level
+output rows, every weight gradient; an array beyond its share of 64 MB as a seeded sample of its rows), so that two builds
+can be compared output for output on identical seeded inputs.
 """
 from __future__ import annotations
 
@@ -44,9 +47,9 @@ sys.path.insert(0, ROOT)
 CONFIGS = {
     "C2": dict(kind="bond", n_mols=10_000, d_h=300, depth=3, precision="bf16", gen="mol", d_v=72, d_e=14, pool=3,
                scaling="weak", desc="10000 synthetic mols/GPU (~25 atoms), BondMessagePassing h=300 depth=3 + MeanAggregation"),
-    "C3": dict(kind="bond", n_mols=50_000, d_h=600, depth=6, precision="fp32", gen="mol", d_v=72, d_e=14, pool=1,
-               scaling="weak", graph=False,      # ~100 GB of activations per step: no room for a graph's private pool beside it
-               desc="50000 synthetic mols/GPU (~25 atoms), BondMessagePassing h=600 depth=6 fp32 + MeanAggregation"),
+    "C3": dict(kind="bond", n_mols=20_000, d_h=600, depth=6, precision="fp32", gen="mol", d_v=72, d_e=14, pool=1,
+               scaling="weak", graph=False,      # ~40 GB of activations per step: no room for a graph's private pool beside it
+               desc="20000 synthetic mols/GPU (~25 atoms), BondMessagePassing h=600 depth=6 fp32 + MeanAggregation"),
     "C4": dict(kind="atom", n_mols=10_000, d_h=300, depth=3, precision="bf16", gen="cgr", d_v=106, d_e=28, pool=2,
                scaling="weak", desc="10000 synthetic condensed reaction graphs/GPU (~80 atoms, d_v=106 d_e=28), "
                                     "AtomMessagePassing h=300 depth=3 + MeanAggregation"),
@@ -55,13 +58,14 @@ CONFIGS = {
                desc="1M synthetic mols (~25 atoms) data-parallel, global batch 200000 = 8 micro-batches of 25000, "
                     "BondMessagePassing h=300 depth=3 + MeanAggregation"),
 }
-FALLBACK_HBM_GBS = 6650.0
-FALLBACK_BF16_TFLOPS = 1400.0
+# NVIDIA's H100 SXM data sheet (700 W): HBM3 bandwidth and dense BF16 tensor rate -- used when no measured peaks are present
+FALLBACK_HBM_GBS = 3350.0
+FALLBACK_BF16_TFLOPS = 989.0
 
 
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    out = {"hbm": FALLBACK_HBM_GBS, "bf16": FALLBACK_BF16_TFLOPS, "src": "fallback"}
+    out = {"hbm": FALLBACK_HBM_GBS, "bf16": FALLBACK_BF16_TFLOPS, "src": "H100 SXM data sheet"}
     if os.path.exists(p):
         try:
             j = json.load(open(p))
@@ -303,7 +307,7 @@ def main_gpu(args):
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=dev)
     lib = _lib.load()
-    assert lib.dmpnn_device_ok() == 1, "bench needs an sm_100 device"
+    assert lib.dmpnn_device_ok() == 1, "bench needs an H100 (compute capability 9.0) device"
 
     n_mols = args.mols or cfg["n_mols"]
     precision = args.precision or cfg["precision"]
@@ -354,12 +358,43 @@ def main_gpu(args):
     V_atoms, E_rows = resident.V.shape[0], resident.E.shape[0]
     n_tiles = resident._meta_host[_lib.META_N_TILES] if resident._meta_host else None
 
+    last = {}                                    # the latest step's outputs (--dump-outputs)
+
     def fwd_bwd(bmg):
         bmg._layout = None                       # the device layout build is part of every step
         H = mp(bmg)
-        loss = agg(H, bmg.batch).float().square().mean()
+        a = agg(H, bmg.batch)
+        loss = a.float().square().mean()
         loss.backward()
+        last.update(H=H.detach(), agg=a.detach(), loss=loss.detach())   # detached: no autograd graph outlives the step
         return loss
+
+    def sampled(X, budget, seed):
+        """(row indices or None, rows): X whole when it fits `budget` bytes as float32 (with 8 bytes per stored row index),
+        else a fixed, seeded sample of its rows that does."""
+        X = X.detach()
+        n = X.shape[0]
+        k = min(n, max(1, budget // (X[0].numel() * 4 + 8)))
+        if k == n:
+            return None, X.float().cpu().numpy()
+        rows = torch.randperm(n, generator=torch.Generator().manual_seed(seed))[:k].sort().values
+        return rows.numpy().astype(np.float64), X[rows.to(X.device)].float().cpu().numpy()
+
+    def snapshot():
+        """What the timed path handed its caller in its last step, as host float32 / float64 arrays, 64 MB at most: the
+        aggregate and the node-level output get 24 MB each, the weight gradients 16 MB between them; an array larger than
+        its share is stored as a seeded sample of its rows (`<name>_rows` holds the row indices)."""
+        out = {"loss": last["loss"].double().cpu().numpy().reshape(1)}
+        grads = [(k, p.grad) for k, p in mp.named_parameters() if p.grad is not None]
+        parts = [("aggregate", last["agg"], 24 << 20), ("H", last["H"], 24 << 20)]
+        parts += [("grad." + k, g, (16 << 20) // len(grads)) for k, g in grads]
+        for i, (name, X, budget) in enumerate(parts):
+            rows, val = sampled(X, budget, 1234 + i)
+            out[name] = val
+            if rows is not None:
+                out[name + "_rows"] = rows
+        assert sum(v.nbytes for v in out.values()) <= 64 << 20
+        return out
 
     def step_resident():
         zero_grads()
@@ -403,6 +438,7 @@ def main_gpu(args):
     with ClockSampler(local) as clocks:
         ms = timed(step_resident, args.steps)
     launches = lib.dmpnn_launch_count() - l0
+    dump = snapshot() if args.dump_outputs and rank == 0 else None
     step_events, engine.STEP_EVENTS = engine.STEP_EVENTS, None
     ms_per_step = ms / args.steps
     value = mols_per_step / (ms_per_step * 1e-3)
@@ -444,6 +480,8 @@ def main_gpu(args):
                 value = mols_per_step / (ms_per_step * 1e-3)
                 launches = gstep.last_launches * args.steps
                 clocks = clocks_g
+                if args.dump_outputs and rank == 0:
+                    dump = snapshot()
                 graph_info = {"used": True, "kernels_per_replay": gstep.last_launches, "graph_launches_per_step": 1}
             if world == 1:
                 for p in params:
@@ -553,19 +591,9 @@ def main_gpu(args):
         dur_ms = statistics.mean(by_tag["fused"])
         alg = 3 * E_rows * h * s + 12 * E_rows + 4 * V_atoms
         ach = alg / (dur_ms * 1e-3) / 1e9
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "fused_step_traffic.json")
-        if os.path.exists(tp):
-            try:
-                tj = json.load(open(tp))
-                if int(tj.get("directed_edges", -1)) == E_rows and tj.get("precision") == precision:
-                    traffic = tj["dram_bytes_per_launch"]
-            except Exception:
-                pass
         roofline = {"bound": "hbm", "achieved": ach, "peak": pk["hbm"], "unit": "GB/s", "frac": ach / pk["hbm"],
-                    "traffic": traffic, "kernel": "k_bond_step_fused: bond depth step t>=2 (message + W_h GEMM + H_0 + tau, one launch)",
+                    "traffic": None, "kernel": "k_bond_step_fused: bond depth step t>=2 (message + W_h GEMM + H_0 + tau, one launch)",
                     "launch_ms": dur_ms, "algorithmic_bytes": alg, "peak_source": pk["src"],
-                    "traffic_source": "profiles/fused_step_traffic.json (ncu --set full of this kernel on this workload)" if traffic else None,
                     "first_step_ms": statistics.mean(by_tag.get("fused_first", [float("nan")]))}
     elif "x3_gemm" in by_tag:
         # fp32 tier: the depth step is bond_message (HBM-bound) + the 3xTF32 W_h GEMM (tensor-bound); the GEMM dominates
@@ -574,10 +602,10 @@ def main_gpu(args):
         ach = flops / (dur_ms * 1e-3) / 1e12
         alg_b = 3 * E_rows * h * 4
         roofline = {"bound": "tensor", "achieved": ach, "peak": pk["bf16"], "unit": "TFLOP/s", "frac": ach / pk["bf16"],
-                    "traffic": None, "kernel": "k_linear_x3: W_h GEMM of the fp32 depth step (3 x tcgen05 kind::tf32 passes per product)",
+                    "traffic": None, "kernel": "k_linear_x3: W_h GEMM of the fp32 depth step (3 tf32 wgmma passes per product)",
                     "launch_ms": dur_ms, "algorithmic_flops": flops, "peak_source": pk["src"],
                     "note": ("algorithmic flops 2*E*h*h; the f32-accurate product costs 3 tf32 MMAs = 6 bf16-equivalents, so the "
-                             "ceiling of this scheme is peak/6; peak = measured dense bf16 (MEASURED_PEAKS.json, sustained)"),
+                             "ceiling of this scheme is peak/6; peak = dense bf16 (see peak_source)"),
                     "frac_of_x3_ceiling": ach / (pk["bf16"] / 6.0),
                     "hbm_bound": {"algorithmic_bytes": alg_b, "achieved_gbs": alg_b / (dur_ms * 1e-3) / 1e9, "peak_gbs": pk["hbm"],
                                   "frac": alg_b / (dur_ms * 1e-3) / 1e9 / pk["hbm"]}}
@@ -608,6 +636,10 @@ def main_gpu(args):
         if world > 1:
             dist.destroy_process_group()
         return
+    if dump is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for k, v in dump.items():
+            np.save(os.path.join(args.dump_outputs, k + ".npy"), v)
 
     # ---- CPU baseline (rank 0, N=1 only; bounded sample) ---------------------------------------
     cpu = None
@@ -666,6 +698,8 @@ def main():
     ap.add_argument("--no-dataset", action="store_true", help="(kept for old command lines; no effect)")
     ap.add_argument("--no-pack", action="store_true", help="keep the sampler's molecule order (no tile packing)")
     ap.add_argument("--no-graph", action="store_true", help="do not run the resident step as a CUDA graph")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     if args.impl == "reference":
         main_reference(args)

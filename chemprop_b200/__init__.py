@@ -1,4 +1,4 @@
-"""chemprop_b200: a Blackwell (sm_100a) engine for chemprop's D-MPNN message-passing hot path,
+"""chemprop_b200: a Hopper (H100, sm_90a) engine for chemprop's D-MPNN message-passing hot path,
 behind chemprop's own module API (`nn.BondMessagePassing`, `nn.AtomMessagePassing`,
 `nn.{Mean,Sum,Norm}Aggregation`, `data.BatchMolGraph`)."""
 from . import data, nn  # noqa: F401

@@ -1,4 +1,4 @@
-"""ctypes binding of libdmpnn_sm100.so (the C ABI declared in include/dmpnn.h).
+"""ctypes binding of libdmpnn_sm90.so (the C ABI declared in include/dmpnn.h).
 
 There is deliberately no fallback: if the shared library is missing or a call fails, the
 product path raises.  (`oracle/` is test infrastructure and is never imported from here.)
@@ -10,7 +10,7 @@ import os
 from pathlib import Path
 
 _PKG = Path(__file__).resolve().parent
-LIB_PATH = Path(os.environ.get("DMPNN_LIB", _PKG / "lib" / "libdmpnn_sm100.so"))
+LIB_PATH = Path(os.environ.get("DMPNN_LIB", _PKG / "lib" / "libdmpnn_sm90.so"))
 
 F32, BF16 = 0, 1
 ACT_NONE, ACT_RELU, ACT_LEAKYRELU, ACT_TANH, ACT_ELU = 0, 1, 2, 3, 4

@@ -1,4 +1,4 @@
-"""Build libdmpnn_sm100.so in-tree with nvcc for sm_100a (no JIT cache: the .so ships with the repo snapshot)."""
+"""Build libdmpnn_sm90.so in-tree with nvcc for sm_90a (H100); build() writes it under chemprop_b200/lib/."""
 from __future__ import annotations
 
 import os
@@ -9,10 +9,10 @@ from pathlib import Path
 
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
-LIB = PKG / "lib" / "libdmpnn_sm100.so"
+LIB = PKG / "lib" / "libdmpnn_sm90.so"
 SOURCES = ["api_misc.cu", "dataset.cu", "layout.cu", "linear.cu", "segment.cu", "step_fused.cu", "step_fused_fwd.cu", "step_fused_bwd.cu", "step_fused_far_fwd.cu", "step_fused_far_bwd.cu", "step_fused_atom_fwd.cu", "step_fused_atom_bwd.cu", "linear_tc.cu", "wgrad_tc.cu", "gemm_x3.cu", "head.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xptxas=-v", "-Xcompiler", "-fPIC",
 ]
 
@@ -96,7 +96,7 @@ def build(force: bool = False, verbose: bool = True) -> Path:
             for line in out.splitlines():
                 if "error" in line or "warning" in line.lower() or "spill" in line and "0 bytes spill" not in line:
                     print(f"[{s}] {line}")
-    cmd = [nvcc, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a"]
     subprocess.run(cmd, check=True)
     return LIB
 

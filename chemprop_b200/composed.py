@@ -1,5 +1,5 @@
 """Composed tier: the reference's own op sequence (chemprop/nn/message_passing/base.py:196-212) with every
-tensor op on the path executed by a kernel of libdmpnn_sm100.so, glued together by torch autograd.
+tensor op on the path executed by a kernel of libdmpnn_sm90.so, glued together by torch autograd.
 
 It serves the configurations the monolithic tiers (engine.BondMPFunction / AtomMPFunction, which fuse tau into
 their kernels) do not cover:

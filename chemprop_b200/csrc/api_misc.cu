@@ -1,4 +1,4 @@
-// Version / error plumbing and the host-side collate of libdmpnn_sm100.so.
+// Version / error plumbing and the host-side collate of libdmpnn_sm90.so.
 #include <stdarg.h>
 #include <atomic>
 #include <string.h>
@@ -32,12 +32,13 @@ const char* dmpnn_last_error(void) { return dmpnn::g_err; }
 int dmpnn_device_ok(void) {
   int dev = -1;
   if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return 0; }
-  int major = 0;
-  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) {
+  int major = 0, minor = 0;
+  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) {
     cudaGetLastError();
     return 0;
   }
-  return major == 10 ? 1 : 0;
+  return (major == 9 && minor == 0) ? 1 : 0;   // sm_90a code runs on compute capability 9.0 only
 }
 
 // Replaces the per-molecule Python loop of BatchMolGraph.__post_init__

@@ -1,4 +1,4 @@
-// Shared helpers for libdmpnn_sm100.so (sm_100a only).
+// Shared helpers for libdmpnn_sm90.so (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -2,7 +2,7 @@
 //
 // Replaces, for pre-featurised data, `[dataset[i] for i in ids]` + collate_batch + the host -> device copy of the
 // batch (chemprop/data/datasets.py:222-244, chemprop/data/collate.py:37-97): the dataset's flat arrays stay in HBM
-// (1 M ~25-atom molecules: 7.2 GB of atom features, 3 GB of bond features, 0.8 GB of local indices -- of 180 GB), a
+// (1 M ~25-atom molecules: 7.2 GB of atom features, 3 GB of bond features, 0.8 GB of local indices -- of the H100's 80 GB), a
 // training step uploads only the ids and the output offsets (24 bytes per molecule) and this kernel copies each
 // selected molecule's rows to its place in the batch, turning molecule-local indices into batch-global ones.
 // Pure HBM streaming: 2 x (4 d_v V + 4 d_e E) + 40 E + 8 V bytes per batch, no reuse, no arithmetic beyond the offsets.
@@ -190,7 +190,14 @@ extern "C" int dmpnn_scale_mask(const void* X, const void* M, void* OUT, int dty
   if (n == 0) return 0;
   int64_t blocks = (n / 4 + 255) / 256;
   if (blocks < 1) blocks = 1;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  static int sm_count = 0;
+  if (!sm_count) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
+    if (sm_count <= 0) sm_count = 132;
+  }
+  if (blocks > (int64_t)sm_count * 16) blocks = (int64_t)sm_count * 16;
   if (dtype == DMPNN_F32) {
     const int vec = dmpnn::vec4_ok<float>(X, 4) && dmpnn::vec4_ok<float>(M, 4) && dmpnn::vec4_ok<float>(OUT, 4);
     k_scale_mask<float><<<(unsigned)blocks, 256, 0, st>>>((const float*)X, (const float*)M, (float*)OUT, n, scale, vec);

@@ -1,30 +1,27 @@
 // fp32-accurate tensor-core GEMMs for the fp32 tier (BASELINE config 3: h = 600, depth 6, fp32): every product is
-// evaluated as THREE tcgen05.mma.kind::tf32 passes on an error-free split of both operands,
+// evaluated as THREE tf32 wgmma passes on an error-free split of both operands,
 //
 //     x = x_hi + x_lo,   x_hi = rna_tf32(x),  x_lo = rna_tf32(x - x_hi)   (x - x_hi is exact in f32)
 //     a . b  ~=  a_lo . b_hi + a_hi . b_lo + a_hi . b_hi                  (the a_lo . b_lo term, 2^-22 relative, is dropped)
 //
-// with f32 accumulation in tensor memory: 2^-21-class relative error per product instead of tf32's 2^-11, i.e. the
+// with f32 accumulation in registers: 2^-21-class relative error per product instead of tf32's 2^-11, i.e. the
 // accuracy of an f32 FMA chain (the reference's ATen sgemm), at tensor-core speed.  SURVEY.md section 7, hard part 2.
 //
 //   dmpnn_linear_x3   C[r, 0:N] = act(A[r, 0:K] . W^T + bias + res[r, 0:N])        A, C, res f32 row-major
 //        replaces chemprop/nn/message_passing/base.py:135-141 (W_h), :180-182 (W_o) and the dX GEMMs of their autograd
 //   dmpnn_wgrad_x3    dW[n, k] (+)= sum_r dY[r, n] X[r, k]                          autograd of the same nn.Linear layers
 //
-// k_linear_x3 -- persistent, one CTA per SM, work item = (256-row pair of tiles, 128-column pass over N):
-//   warp 0       cp.async.bulk producer of the W stages: pre-split, pre-swizzled {W_hi, W_lo} blocks of one 32-wide k slab
-//   warp 1       tcgen05.mma issuer (converged warp, elected lane): per stage 2 tiles x 4 k steps x 3 products, M = 128, N <= 128
-//   warp 2       TMEM allocator: 512 columns = 2 buffers x 2 tiles x 128 accumulator columns (epilogue of item i overlaps item i+1)
-//   warps 4-7    epilogue: tcgen05.ld -> + bias + residual -> act -> f32 rows straight to global memory (64-byte segments)
-//   warps 8-15   A producers, thread = tile row: 128-byte row segment of the slab by LDG.128 (optionally through a row
+// k_linear_x3 -- persistent, one CTA per SM, work item = (128-row tile, 128-column pass over N):
+//   warps 0-3    A producers, thread = tile row: 128-byte row segment of the slab by LDG.128 (optionally through a row
 //                index), split into hi / lo in registers, written as K-major SWIZZLE_128B operand tiles (generic proxy ->
-//                fence.proxy.async); the loads of slab s+1 are in flight while slab s waits for its stage
-// Every W stage (32 KB) serves two A tiles: L2 -> SM operand traffic per flop is half that of a 128-row item, which keeps
-// the kernel on the tensor pipe rather than on L2 bandwidth (the pipe needs ~100 flop / L2 byte at 3 passes of tf32).
+//                fence.proxy.async); thread 0 also lands the pre-split, pre-swizzled {W_hi, W_lo} blocks of the 32-wide
+//                k slab (cp.async.bulk)
+//   warps 4-11   two consumer warpgroups (tile rows [0, 64) / [64, 128)): per stage 4 k steps x 3 products of
+//                wgmma m64n128k8 (tf32), then the epilogue from registers: + bias + residual -> act -> f32 rows to global
 //
-// k_wgrad_x3 -- CTA (n tile of 128, k tile of <= 256, row slot): D[128 x 256] (TMEM) += dY_blk^T . X_blk over 32-row
-// blocks; both operands are MN-major (the contraction runs over rows), written by the producers into the one layout the
-// tensor core transposes 32-bit operands from (SWIZZLE_128B_BASE32B); partial sums per CTA, fixed-order reduce (deterministic).
+// k_wgrad_x3 -- CTA (n tile of 128, k tile of 128, row slot): D[128 x 128] (registers) += dY_blk^T . X_blk over 32-row
+// blocks.  tf32 wgmma reads K-major operands only, so the producers write both operands transposed (rows = n or k,
+// 32 contraction rows per 128-byte line, K-major SWIZZLE_128B); partial sums per CTA, fixed-order reduce (deterministic).
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -55,60 +52,27 @@ __device__ __forceinline__ void split4(const float4 v, uint4& hi, uint4& lo) {
   split1(v.z, hi.z, lo.z);
   split1(v.w, hi.w, lo.w);
 }
-// c = F32, a = b = TF32 (format 2), optional MN-major operands, N >> 3 at [17, 23), M >> 4 at [24, 29)
-__device__ __forceinline__ uint32_t idesc_tf32(int M, int N, bool mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (mn_major ? ((1u << 15) | (1u << 16)) : 0u) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// MN-major tf32 operand.  32-bit operands transposed by the tensor core exist in ONE shared-memory layout only,
-// SWIZZLE_128B_BASE32B (descriptor layout type 1): rows of the contraction index at a 128-byte pitch (32 tf32 along MN),
-// atoms of FOUR rows (512 B) inside which the 32-byte chunk index is XORed with (row & 3) -- Swizzle<2,5,2> on byte
-// addresses; atoms along K `sbo` = 512 B apart, 32-element blocks along MN `lbo` bytes apart.  One k step of the
-// instruction (8 tf32) covers two atoms.
-__device__ __forceinline__ uint64_t desc_mn_sw128_32b(uint32_t saddr, uint32_t lbo) {
-  uint64_t d = (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(512 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)1 << 61;
-  return d;
-}
-// byte offset of 16-byte chunk `c` (0..7) of contraction row `r` inside one 32-element MN block of that layout
-__device__ __forceinline__ uint32_t mn32b_off(int r, int c) {
-  return (uint32_t)(r * 128 + ((((c >> 1) ^ (r & 3)) << 5) | ((c & 1) << 4)));
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // linear
 // ------------------------------------------------------------------------------------------------------------------
 namespace lin {
 constexpr int kTileM = 128;
-constexpr int kPairM = 256;
 constexpr int kNP = 128;                      // output columns per pass
 constexpr int kABytes = kTileM * 128;         // one tile x one 32-wide k slab x one of {hi, lo}: 16 KB
 constexpr int kWBytes = kNP * 128;            // one of {W_hi, W_lo} of a k slab: 16 KB
-constexpr int kOffAhi = 0, kOffAlo = 2 * kABytes, kOffW = 4 * kABytes;
-constexpr int kStageBytes = 4 * kABytes + 2 * kWBytes;   // 96 KB
-constexpr int kStages = 2;
-constexpr int kThreads = 512;
-constexpr int kProducerWarps = 8;
-constexpr int kTmemCols = 512;
+constexpr int kOffAhi = 0, kOffAlo = kABytes, kOffW = 2 * kABytes;
+constexpr int kStageBytes = 2 * kABytes + 2 * kWBytes;   // 64 KB
+constexpr int kStages = 3;
+constexpr int kThreads = 384;
+constexpr int kProducerWarps = 4;
+constexpr int kConsumers = 256;
 constexpr int kOffBar = kStages * kStageBytes;
-constexpr int kOffTmem = kOffBar + 16 * 8;
-constexpr int kSmemBytes = kOffTmem + 16;
+constexpr int kSmemBytes = kOffBar + 8 * 8;
 constexpr int kSmemAlloc = kSmemBytes + 1024;
 static_assert(kStageBytes % 1024 == 0, "SWIZZLE_128B operand tiles need 1024-byte alignment");
 static_assert(kSmemAlloc <= 232448, "exceeds shared memory");
 
-enum { B_FULL = 0, B_EMPTY = 2, B_ACCFULL = 4, B_ACCFREE = 6 };
+enum { B_FULL = 0, B_EMPTY = 3 };
 
 struct Params {
   const float* A;
@@ -121,7 +85,7 @@ struct Params {
   float* C;
   int64_t ldc;
   int64_t R;
-  int K, N, Npad, ldc_pad, nslab, n_pass, n_pairs;
+  int K, N, Npad, ldc_pad, nslab, n_pass, n_tiles;
   int act;
   float act_param;
 };
@@ -131,182 +95,112 @@ __global__ void __launch_bounds__(kThreads, 1) k_linear_x3(Params p) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t sbase = smem_u32(smem);
   const uint32_t sBar = sbase + kOffBar;
-  volatile uint32_t* s_tmem = reinterpret_cast<volatile uint32_t*>(smem + kOffTmem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   auto bar = [&](int i) { return sBar + 8u * (uint32_t)i; };
+  const int n_items = p.n_tiles * p.n_pass;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(bar(B_FULL + i), 1 + kProducerWarps);   // W loader's expect_tx arrive + one arrive per producer warp
-      mbar_init(bar(B_EMPTY + i), 1);                   // tcgen05.commit
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar(B_ACCFULL + i), 1);
-      mbar_init(bar(B_ACCFREE + i), 128);
+      mbar_init(bar(B_EMPTY + i), kConsumers);
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(s_tmem)), kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
-  if (warp == 0) {
-    // ===================== W stages: {W_hi, W_lo} of (pass, slab), contiguous 32 KB in the packed image ==========
+  if (warp < kProducerWarps) {
+    // ===================== A producers (thread = tile row) + W loader (thread 0) =====================
+    const int r = threadIdx.x;
     uint32_t ks = 0;
-    for (int pair = blockIdx.x; pair < p.n_pairs; pair += gridDim.x)
-      for (int ps = 0; ps < p.n_pass; ++ps)
-        for (int s = 0; s < p.nslab; ++s, ++ks) {
-          const uint32_t st = ks % kStages, use = ks / kStages;
-          mbar_wait(bar(B_EMPTY + st), (use & 1) ^ 1);
-          if (elect_one()) {
-            mbar_expect_tx(bar(B_FULL + st), 2 * kWBytes);
-            bulk_load(sbase + st * kStageBytes + kOffW, p.Wpk + ((size_t)ps * p.nslab + s) * (2 * kWBytes), 2 * kWBytes,
-                      bar(B_FULL + st));
-          }
-          __syncwarp();
-        }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    uint32_t ks = 0;
-    int it = 0;
-    for (int pair = blockIdx.x; pair < p.n_pairs; pair += gridDim.x)
-      for (int ps = 0; ps < p.n_pass; ++ps, ++it) {
-        const int np = min(kNP, p.Npad - ps * kNP);
-        const uint32_t idesc = idesc_tf32(kTileM, np, false);
-        const uint32_t buf = (uint32_t)it & 1u;
-        mbar_wait(bar(B_ACCFREE + buf), ((it >> 1) & 1) ^ 1);     // the epilogue drained this buffer two items ago
-        tc_fence_after();
-        for (int s = 0; s < p.nslab; ++s, ++ks) {
-          const uint32_t st = ks % kStages, use = ks / kStages;
-          mbar_wait(bar(B_FULL + st), use & 1);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t stg = sbase + st * kStageBytes;
-            const uint64_t bhi = umma_desc_sw128(stg + kOffW), blo = umma_desc_sw128(stg + kOffW + kWBytes);
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {
-              const uint32_t d = tmem_base + buf * 256u + (uint32_t)t * 128u;
-              const uint64_t ahi = umma_desc_sw128(stg + kOffAhi + t * kABytes), alo = umma_desc_sw128(stg + kOffAlo + t * kABytes);
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) {          // k step = 8 tf32 = 32 B of every operand row
-                const uint64_t o = (uint64_t)(2 * kk);
-                umma_tf32(d, alo + o, bhi + o, idesc, (s > 0 || kk > 0) ? 1u : 0u);
-                umma_tf32(d, ahi + o, blo + o, idesc, 1u);
-                umma_tf32(d, ahi + o, bhi + o, idesc, 1u);
-              }
-            }
-            umma_commit(bar(B_EMPTY + st));
-            if (s == p.nslab - 1) umma_commit(bar(B_ACCFULL + buf));
-          }
-          __syncwarp();
-        }
-      }
-  } else if (warp >= 4 && warp < 8) {
-    // ===================== epilogue: thread = accumulator row (TMEM lane) =====================
-    const int row = (warp & 3) * 32 + lane;
-    const uint32_t tlane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-    int it = 0;
-    for (int pair = blockIdx.x; pair < p.n_pairs; pair += gridDim.x)
-      for (int ps = 0; ps < p.n_pass; ++ps, ++it) {
-        const int np = min(kNP, p.Npad - ps * kNP);
-        const uint32_t buf = (uint32_t)it & 1u;
-        mbar_wait(bar(B_ACCFULL + buf), (it >> 1) & 1);
-        tc_fence_after();
-#pragma unroll 1
-        for (int t = 0; t < 2; ++t) {
-          const int64_t grow = (int64_t)pair * kPairM + t * kTileM + row;
-          const bool rv = grow < p.R;
-          float* crow = p.C + grow * p.ldc;
-          const float* rrow = p.res ? p.res + grow * p.ldres : nullptr;
-#pragma unroll 1
-          for (int j = 0; j < (np >> 4); ++j) {
-            uint32_t v[16];
-            tmem_ld16(tlane + buf * 256u + (uint32_t)t * 128u + (uint32_t)(j * 16), v);
-            const int n0 = ps * kNP + j * 16;
-            float r[16];
-#pragma unroll
-            for (int q = 0; q < 16; ++q) r[q] = 0.f;
-            if (rv && rrow != nullptr) {
-              if (n0 + 16 <= p.N) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float4 x = __ldg(reinterpret_cast<const float4*>(rrow + n0 + 4 * q));
-                  r[4 * q] = x.x; r[4 * q + 1] = x.y; r[4 * q + 2] = x.z; r[4 * q + 3] = x.w;
-                }
-              } else {
-#pragma unroll
-                for (int q = 0; q < 16; ++q) if (n0 + q < p.N) r[q] = __ldg(rrow + n0 + q);
-              }
-            }
-            tmem_wait_ld();
-            if (rv) {
-              float o[16];
-#pragma unroll
-              for (int q = 0; q < 16; ++q) {
-                const int n = n0 + q;
-                float z = __uint_as_float(v[q]) + r[q];
-                if (p.bias != nullptr && n < p.N) z += __ldg(p.bias + n);
-                o[q] = n < p.N ? act_apply(p.act, p.act_param, z) : 0.f;
-              }
-              if (n0 + 16 <= p.ldc_pad) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                  *reinterpret_cast<float4*>(crow + n0 + 4 * q) = make_float4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]);
-              } else {
-#pragma unroll
-                for (int q = 0; q < 16; ++q) if (n0 + q < p.ldc_pad) crow[n0 + q] = o[q];
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        mbar_arrive(bar(B_ACCFREE + buf));
-      }
-  } else if (warp >= 8) {
-    // ===================== A producers: thread = row of the 256-row pair =====================
-    const int r = threadIdx.x - 256;                  // 0..255
-    const int t = r >> 7, rl = r & 127;
-    uint32_t ks = 0;
-    for (int pair = blockIdx.x; pair < p.n_pairs; pair += gridDim.x) {
-      const int64_t grow = (int64_t)pair * kPairM + r;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const int t = item / p.n_pass, ps = item - t * p.n_pass;
+      const int64_t grow = (int64_t)t * kTileM + r;
       const bool rv = grow < p.R;
       const float* arow = nullptr;
       if (rv) arow = p.A + (p.idx ? (int64_t)__ldg(p.idx + grow) : grow) * p.lda;
-      for (int ps = 0; ps < p.n_pass; ++ps)
-        for (int s = 0; s < p.nslab; ++s, ++ks) {
-          // the row segment of this slab: 8 x 16 B, all loads in flight before the stage is waited for
-          float4 x[8];
+      for (int s = 0; s < p.nslab; ++s, ++ks) {
+        // the row segment of this slab: 8 x 16 B, all loads in flight before the stage is waited for
+        float4 x[8];
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const int k0 = s * 32 + c * 4;
-            x[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (rv && k0 < p.K) x[c] = __ldg(reinterpret_cast<const float4*>(arow + k0));   // K % 4 == 0
-          }
-          const uint32_t st = ks % kStages, use = ks / kStages;
-          mbar_wait(bar(B_EMPTY + st), (use & 1) ^ 1);
-          const uint32_t stg = sbase + st * kStageBytes + (uint32_t)t * kABytes;
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            uint4 hi, lo;
-            split4(x[c], hi, lo);
-            const uint32_t off = sw128_off(rl, c);
-            sts128(stg + kOffAhi + off, hi);
-            sts128(stg + kOffAlo + off, lo);
-          }
-          fence_proxy_async();                        // generic-proxy writes -> visible to the tensor core's async proxy
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar(B_FULL + st));
+        for (int c = 0; c < 8; ++c) {
+          const int k0 = s * 32 + c * 4;
+          x[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (rv && k0 < p.K) x[c] = __ldg(reinterpret_cast<const float4*>(arow + k0));   // K % 4 == 0
         }
+        const uint32_t st = ks % kStages, use = ks / kStages;
+        mbar_wait(bar(B_EMPTY + st), (use & 1) ^ 1);
+        const uint32_t stg = sbase + st * kStageBytes;
+        if (threadIdx.x == 0) {
+          mbar_expect_tx(bar(B_FULL + st), 2 * kWBytes);
+          bulk_load(stg + kOffW, p.Wpk + ((size_t)ps * p.nslab + s) * (2 * kWBytes), 2 * kWBytes, bar(B_FULL + st));
+        }
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          uint4 hi, lo;
+          split4(x[c], hi, lo);
+          const uint32_t off = sw128_off(r, c);
+          sts128(stg + kOffAhi + off, hi);
+          sts128(stg + kOffAlo + off, lo);
+        }
+        fence_proxy_async();                        // generic-proxy writes -> visible to the tensor core's async proxy
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar(B_FULL + st));
+      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+  } else {
+    // ===================== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =====================
+    const int wg = (warp - 4) >> 2;
+    const int tt = threadIdx.x - 128 - wg * 128;
+    const int rl = wg * 64 + acc_row0(tt), cl = acc_col0(tt);
+    uint32_t ks = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const int t = item / p.n_pass, ps = item - t * p.n_pass;
+      float acc[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      for (int s = 0; s < p.nslab; ++s, ++ks) {
+        const uint32_t st = ks % kStages, use = ks / kStages;
+        mbar_wait(bar(B_FULL + st), use & 1);
+        const uint32_t stg = sbase + st * kStageBytes;
+        const uint64_t bhi = desc_sw128(stg + kOffW), blo = desc_sw128(stg + kOffW + kWBytes);
+        const uint64_t ahi = desc_sw128(stg + kOffAhi + (uint32_t)wg * 8192u), alo = desc_sw128(stg + kOffAlo + (uint32_t)wg * 8192u);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {            // k step = 8 tf32 = 32 B of every operand row
+          const uint64_t o = (uint64_t)(2 * kk);
+          wgmma_tf32_n128(acc, alo + o, bhi + o, 1u);
+          wgmma_tf32_n128(acc, ahi + o, blo + o, 1u);
+          wgmma_tf32_n128(acc, ahi + o, bhi + o, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence(acc);
+        mbar_arrive(bar(B_EMPTY + st));
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t grow = (int64_t)t * kTileM + rl + 8 * h;
+        if (grow >= p.R) continue;
+        float* crow = p.C + grow * p.ldc;
+        const float* rrow = p.res ? p.res + grow * p.ldres : nullptr;
+#pragma unroll
+        for (int b = 0; b < kNP / 8; ++b) {
+          const int n = ps * kNP + 8 * b + cl;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            if (n + e >= p.ldc_pad) continue;
+            float o = 0.f;
+            if (n + e < p.N) {
+              float z = acc[4 * b + 2 * h + e];
+              if (rrow != nullptr) z += __ldg(rrow + n + e);
+              if (p.bias != nullptr) z += __ldg(p.bias + n + e);
+              o = act_apply(p.act, p.act_param, z);
+            }
+            crow[n + e] = o;
+          }
+        }
+      }
+    }
   }
 }
 
@@ -345,28 +239,25 @@ __global__ void k_pack_weight_x3(const float* __restrict__ W, int64_t ldw, int t
 // ------------------------------------------------------------------------------------------------------------------
 namespace wg {
 constexpr int kRows = 32;                      // contraction rows per stage
-constexpr int kMT = 128, kKT = 256;            // output tile: n x k
-constexpr int kAtomBytes = kRows * 128;        // one 32-column MN block x 32 rows: 4 KB
-constexpr int kABytes = (kMT / 32) * kAtomBytes;     // 16 KB per {hi, lo}
-constexpr int kBBytes = (kKT / 32) * kAtomBytes;     // 32 KB per {hi, lo}
-constexpr int kOffAhi = 0, kOffAlo = kABytes, kOffBhi = 2 * kABytes, kOffBlo = 2 * kABytes + kBBytes;
-constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;   // 96 KB
-constexpr int kStages = 2;
-constexpr int kThreads = 512;
-constexpr int kProducerWarps = 8;
-constexpr int kTmemCols = 256;
+constexpr int kMT = 128, kKT = 128;            // output tile: n x k
+constexpr int kOpBytes = 128 * 128;            // one operand (128 rows of n or k x 32 contraction rows) x one of {hi, lo}
+constexpr int kOffAhi = 0, kOffAlo = kOpBytes, kOffBhi = 2 * kOpBytes, kOffBlo = 3 * kOpBytes;
+constexpr int kStageBytes = 4 * kOpBytes;      // 64 KB
+constexpr int kStages = 3;
+constexpr int kThreads = 384;
+constexpr int kProducerWarps = 4;
+constexpr int kConsumers = 256;
 constexpr int kOffBar = kStages * kStageBytes;
-constexpr int kOffTmem = kOffBar + 8 * 8;
-constexpr int kSmemBytes = kOffTmem + 16;
+constexpr int kSmemBytes = kOffBar + 8 * 8;
 constexpr int kSmemAlloc = kSmemBytes + 1024;
 static_assert(kSmemAlloc <= 232448, "exceeds shared memory");
-enum { B_FULL = 0, B_EMPTY = 2, B_ACCFULL = 4 };
+enum { B_FULL = 0, B_EMPTY = 3 };
 
 struct Params {
   const float* dY;
   const float* X;
   int64_t lddy, ldx, R;
-  float* partial;            // [grid][128][256]
+  float* partial;            // [grid][128][128]
   int N, K, n_mt, n_kt, slots, n_blocks;
 };
 
@@ -375,83 +266,33 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_x3(Params p) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t sbase = smem_u32(smem);
   const uint32_t sBar = sbase + kOffBar;
-  volatile uint32_t* s_tmem = reinterpret_cast<volatile uint32_t*>(smem + kOffTmem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   auto bar = [&](int i) { return sBar + 8u * (uint32_t)i; };
   const int tile = blockIdx.x % (p.n_mt * p.n_kt), slot = blockIdx.x / (p.n_mt * p.n_kt);
   const int mt = tile % p.n_mt, kt = tile / p.n_mt;
   const int n_base = mt * kMT, k_base = kt * kKT;
-  const int kw = min(kKT, (p.K - k_base + 15) / 16 * 16);      // accumulator columns in use (multiple of 16)
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(bar(B_FULL + i), kProducerWarps);
-      mbar_init(bar(B_EMPTY + i), 1);
+      mbar_init(bar(B_EMPTY + i), kConsumers);
     }
-    mbar_init(bar(B_ACCFULL), 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(s_tmem)), kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
-  if (warp == 1) {
-    const uint32_t idesc = idesc_tf32(kMT, kw, true);
+  if (warp < kProducerWarps) {
+    // producers: 32 rows x (128 dY columns + 128 X columns) = 2048 16-byte chunks per stage, 16 per thread.  A warp takes
+    // one 4-column chunk of all 32 rows, so the transposed 4-byte shared-memory stores of a warp fill one 128-byte line
+    // (K-major: line = output row n or k, 32 contraction rows) without bank conflicts.
+    const int tid = threadIdx.x;
     uint32_t ks = 0;
     for (int blk = slot; blk < p.n_blocks; blk += p.slots, ++ks) {
-      const uint32_t st = ks % kStages, use = ks / kStages;
-      mbar_wait(bar(B_FULL + st), use & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t stg = sbase + st * kStageBytes;
+      float4 x[16];
 #pragma unroll
-        for (int kk = 0; kk < kRows / 8; ++kk) {        // k step = 8 contraction rows = one 1024-byte group of every atom
-          const uint64_t ahi = desc_mn_sw128_32b(stg + kOffAhi + kk * 1024, kAtomBytes), alo = desc_mn_sw128_32b(stg + kOffAlo + kk * 1024, kAtomBytes);
-          const uint64_t bhi = desc_mn_sw128_32b(stg + kOffBhi + kk * 1024, kAtomBytes), blo = desc_mn_sw128_32b(stg + kOffBlo + kk * 1024, kAtomBytes);
-          umma_tf32(tmem_base, alo, bhi, idesc, (ks > 0 || kk > 0) ? 1u : 0u);
-          umma_tf32(tmem_base, ahi, blo, idesc, 1u);
-          umma_tf32(tmem_base, ahi, bhi, idesc, 1u);
-        }
-        umma_commit(bar(B_EMPTY + st));
-      }
-      __syncwarp();
-    }
-    if (elect_one()) umma_commit(bar(B_ACCFULL));
-    __syncwarp();
-  } else if (warp >= 4 && warp < 8) {
-    // final drain: thread = output row n (TMEM lane)
-    const int row = (warp & 3) * 32 + lane;
-    const uint32_t tlane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-    float* out = p.partial + ((size_t)blockIdx.x * kMT + row) * kKT;
-    const bool have = slot < p.n_blocks;
-    mbar_wait(bar(B_ACCFULL), 0);
-    tc_fence_after();
-    for (int j = 0; j < (kw >> 4); ++j) {
-      uint32_t v[16];
-      if (have) {
-        tmem_ld16(tlane + (uint32_t)(j * 16), v);
-        tmem_wait_ld();
-      } else {
-#pragma unroll
-        for (int q = 0; q < 16; ++q) v[q] = 0u;
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<uint4*>(out + j * 16 + q * 4) = make_uint4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-    }
-  } else if (warp >= 8) {
-    // producers: 32 rows x (128 dY columns + 256 X columns) = 3072 16-byte chunks per stage, 12 per thread,
-    // consecutive threads on consecutive chunks of a row (coalesced), split into hi / lo, MN-major atom layout
-    const int tid = threadIdx.x - 256;
-    uint32_t ks = 0;
-    for (int blk = slot; blk < p.n_blocks; blk += p.slots, ++ks) {
-      float4 x[12];
-#pragma unroll
-      for (int i = 0; i < 12; ++i) {
-        const int q = tid + 256 * i;
-        const int rr = q / 96, cc = q % 96;
+      for (int i = 0; i < 16; ++i) {
+        const int q = tid + 128 * i;
+        const int rr = q & 31, cc = q >> 5;
         const int64_t grow = (int64_t)blk * kRows + rr;
         x[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (grow < p.R) {
@@ -468,42 +309,71 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_x3(Params p) {
       mbar_wait(bar(B_EMPTY + st), (use & 1) ^ 1);
       const uint32_t stg = sbase + st * kStageBytes;
 #pragma unroll
-      for (int i = 0; i < 12; ++i) {
-        const int q = tid + 256 * i;
-        const int rr = q / 96, cc = q % 96;
+      for (int i = 0; i < 16; ++i) {
+        const int q = tid + 128 * i;
+        const int rr = q & 31, cc = q >> 5;
         uint4 hi, lo;
         split4(x[i], hi, lo);
-        const int cb = cc < 32 ? cc : cc - 32;            // 16-byte chunk along MN inside the operand
-        const uint32_t off = (uint32_t)(cb >> 3) * kAtomBytes + mn32b_off(rr, cb & 7);
-        if (cc < 32) {
-          sts128(stg + kOffAhi + off, hi);
-          sts128(stg + kOffAlo + off, lo);
-        } else {
-          sts128(stg + kOffBhi + off, hi);
-          sts128(stg + kOffBlo + off, lo);
+        const uint32_t hw[4] = {hi.x, hi.y, hi.z, hi.w}, lw[4] = {lo.x, lo.y, lo.z, lo.w};
+        const uint32_t ohi = cc < 32 ? kOffAhi : kOffBhi, olo = cc < 32 ? kOffAlo : kOffBlo;
+        const int m0 = (cc & 31) * 4;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int m = m0 + e;
+          const uint32_t off = (uint32_t)((m >> 3) * 1024 + (m & 7) * 128 + (((rr >> 2) ^ (m & 7)) << 4) + (rr & 3) * 4);
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(stg + ohi + off), "r"(hw[e]) : "memory");
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(stg + olo + off), "r"(lw[e]) : "memory");
         }
       }
       fence_proxy_async();
       __syncwarp();
       if (lane == 0) mbar_arrive(bar(B_FULL + st));
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+  } else {
+    const int wg = (warp - 4) >> 2;
+    const int tt = threadIdx.x - 128 - wg * 128;
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    uint32_t ks = 0;
+    for (int blk = slot; blk < p.n_blocks; blk += p.slots, ++ks) {
+      const uint32_t st = ks % kStages, use = ks / kStages;
+      mbar_wait(bar(B_FULL + st), use & 1);
+      const uint32_t stg = sbase + st * kStageBytes;
+      const uint64_t ahi = desc_sw128(stg + kOffAhi + (uint32_t)wg * 8192u), alo = desc_sw128(stg + kOffAlo + (uint32_t)wg * 8192u);
+      const uint64_t bhi = desc_sw128(stg + kOffBhi), blo = desc_sw128(stg + kOffBlo);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kRows / 8; ++kk) {        // k step = 8 contraction rows = 32 B of every operand line
+        const uint64_t o = (uint64_t)(2 * kk);
+        wgmma_tf32_n128(acc, alo + o, bhi + o, 1u);
+        wgmma_tf32_n128(acc, ahi + o, blo + o, 1u);
+        wgmma_tf32_n128(acc, ahi + o, bhi + o, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(acc);
+      mbar_arrive(bar(B_EMPTY + st));
+    }
+    // drain: zeros when this CTA had no block (acc stays 0)
+    const int rl = wg * 64 + acc_row0(tt), cl = acc_col0(tt);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float* out = p.partial + ((size_t)blockIdx.x * kMT + rl + 8 * h) * kKT;
+#pragma unroll
+      for (int b = 0; b < kKT / 8; ++b)
+        *reinterpret_cast<float2*>(out + 8 * b + cl) = make_float2(acc[4 * b + 2 * h], acc[4 * b + 2 * h + 1]);
+    }
   }
 }
 
-// dW[n, k] (+)= sum_slot partial[(slot * n_tiles + kt * n_mt + mt)][n % 128][k % 256]   (fixed order: deterministic)
+// dW[n, k] (+)= sum_slot partial[(slot * n_tiles + kt * n_mt + mt)][n % kMT][k % kKT]   (fixed order: deterministic)
 __global__ void k_wgrad_x3_reduce(const float* __restrict__ partial, int slots, int n_mt, int n_kt, int N, int K,
                                   float* __restrict__ dW, int64_t lddw, int accumulate) {
   const int n = blockIdx.x;
   const int mt = n >> 7, nl = n & 127;
   for (int k = threadIdx.x; k < K; k += blockDim.x) {
-    const int kt = k >> 8, kl = k & 255;
+    const int kt = k / kKT, kl = k % kKT;
     float s = 0.f;
     for (int sl = 0; sl < slots; ++sl)
       s += partial[((size_t)(sl * n_mt * n_kt + kt * n_mt + mt) * kMT + nl) * kKT + kl];
@@ -521,7 +391,7 @@ static Geom geom(int64_t R, int64_t N, int64_t K) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
-    if (sm_count <= 0) sm_count = 148;
+    if (sm_count <= 0) sm_count = 132;
   }
   Geom g;
   g.n_mt = (int)((N + kMT - 1) / kMT);
@@ -588,7 +458,7 @@ extern "C" int dmpnn_linear_x3(const float* A, int64_t lda, const int32_t* row_i
   p.K = (int)K; p.N = (int)N; p.Npad = g.Npad;
   p.ldc_pad = (int)ldc_pad;
   p.nslab = g.nslab; p.n_pass = g.n_pass;
-  p.n_pairs = (int)((R + kPairM - 1) / kPairM);
+  p.n_tiles = (int)((R + kTileM - 1) / kTileM);
   p.act = act; p.act_param = act_param;
   static int sm_count = 0;
   if (!sm_count) {
@@ -602,7 +472,8 @@ extern "C" int dmpnn_linear_x3(const float* A, int64_t lda, const int32_t* row_i
     DMPNN_CHECK_ARG(e == cudaSuccess, "linear_x3: cannot configure %d B dynamic smem: %s", kSmemAlloc, cudaGetErrorString(e));
     attr_set = true;
   }
-  const int grid = p.n_pairs < sm_count ? p.n_pairs : sm_count;
+  const int items = p.n_tiles * p.n_pass;
+  const int grid = items < sm_count ? items : sm_count;
   k_linear_x3<<<grid, kThreads, kSmemAlloc, st>>>(p);
   DMPNN_CHECK_LAUNCH("linear_x3", 1);
   return 0;

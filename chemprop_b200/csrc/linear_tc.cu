@@ -1,4 +1,4 @@
-// Tensor-core linear layer for the bf16 tier (tcgen05 + TMEM + TMA), the dense GEMMs of the path that
+// Tensor-core linear layer for the bf16 tier (wgmma + TMA), the dense GEMMs of the path that
 // are not the fused depth step:
 //   W_i initialise (chemprop/nn/message_passing/mixins.py:8-9, 22-23)   K = d_v+d_e -> h
 //   W_o finalize   (chemprop/nn/message_passing/base.py:180-182)        K = d_v+h   -> h
@@ -6,13 +6,11 @@
 //
 //   C[r, 0:N] = act( A[r, 0:K] . W^T + bias )        A, C bf16 row-major; W pre-packed bf16
 //
-// Persistent kernel, one CTA per SM, 128-row tiles:
-//   warp 0      TMA producer: per 64-wide k slab one A box (128 rows x 64, SWIZZLE_128B) + the W slab
-//               (pre-packed shared-memory image, cp.async.bulk) into a 3-stage ring
-//   warp 1      tcgen05.mma issuer (converged warp, elected lane): D[128 x Npad] in TMEM (fp32)
-//   warp 2      TMEM allocator
-//   warps 4-11  epilogue, 2 groups x 4 warps: tcgen05.ld -> +bias -> act -> bf16 -> swizzled staging slab
-//               -> TMA store (cp.async.bulk.tensor ... global.shared::cta): no LSU traffic to global
+// Persistent kernel, one CTA per SM, work item = (128-row tile, output columns [152 j, 152 j + 152)):
+//   warp 0      TMA producer: per 64-wide k slab one A box (128 rows x 64, SWIZZLE_128B) + the item's rows of the W slab
+//               (pre-packed shared-memory image, cp.async.bulk) into a 4-stage ring
+//   warps 4-11  two consumer warpgroups, rows [0, 64) and [64, 128) of the tile: wgmma m64n152k16 with the f32
+//               accumulator in registers, then the epilogue from registers: +bias (+residual) -> act -> bf16 -> global
 // HBM bytes per tile: read 128 x K x 2, write 128 x N x 2; W comes from L2.
 #include <cuda.h>
 #include <stdlib.h>
@@ -26,192 +24,128 @@ namespace lintc {
 using namespace dmpnn::tc;
 
 constexpr int kTileM = 128;
+constexpr int kNT = 152;                          // output columns per work item (the wgmma N)
 constexpr int kSlabBytes = kTileM * 128;          // A stage: 128 rows x 64 bf16
 constexpr int kMaxN = 304;
-constexpr int kMaxK = 448;                       // 7 k slabs (CGR dims: d_v + h = 406)
-constexpr int kWSlabBytes = kMaxN * 128;          // W stage: up to 304 rows x 64 bf16 = 38912
-constexpr int kStageBytes = kSlabBytes + kWSlabBytes;   // 55296 (multiple of 1024)
-constexpr int kStages = 3;
-constexpr int kThreads = 384;                     // 4 control warps + 8 epilogue warps
-constexpr int kTmemCols = 512;
+constexpr int kMaxK = 448;                        // 7 k slabs (CGR dims: d_v + h = 406)
+constexpr int kWSlabBytes = kNT * 128;            // W stage: up to 152 rows x 64 bf16 = 19456
+constexpr int kStageBytes = kSlabBytes + kWSlabBytes;   // 35840 (multiple of 1024)
+constexpr int kStages = 4;
+constexpr int kThreads = 384;                     // producer warpgroup + 2 consumer warpgroups
+constexpr int kConsumers = 256;
 
 constexpr int kOffStage = 0;
-constexpr int kOffOut = kStages * kStageBytes;              // 165888
-constexpr int kOffBar = kOffOut + 2 * kSlabBytes;           // 198656
-constexpr int kOffTmem = kOffBar + 16 * 8;
-constexpr int kOffBias = kOffTmem + 16;
+constexpr int kOffBar = kStages * kStageBytes;
+constexpr int kOffBias = kOffBar + 16 * 8;
 constexpr int kSmemBytes = kOffBias + 320 * 4;
 constexpr int kSmemAlloc = kSmemBytes + 1024;
-static_assert(kStageBytes % 1024 == 0 && kOffOut % 1024 == 0, "SWIZZLE_128B buffers need 1024-byte alignment");
+static_assert(kStageBytes % 1024 == 0 && kSlabBytes % 1024 == 0, "SWIZZLE_128B buffers need 1024-byte alignment");
 static_assert(kSmemAlloc <= 232448, "exceeds shared memory");
 
-enum { B_FULL = 0, B_EMPTY = 4, B_ACCFULL = 8, B_ACCFREE = 9 };
+enum { B_FULL = 0, B_EMPTY = 4 };
 
 struct Params {
   const uint8_t* Wpk;
   const float* bias;
   const __nv_bfloat16* res;   // optional residual rows (bf16, row stride ldres), added before the activation
   int64_t ldres;
+  __nv_bfloat16* C;
+  int64_t ldc;
   int64_t R;
-  int K, N, Npad, nslab, ksteps_last, n_tiles;
+  int K, N, Npad, nslab, ksteps_last, n_tiles, n_nt;
   float act_param;
 };
 
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tmap, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tmap)),
-               "r"(src), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
 template <int ACT, bool HAS_BIAS>
 __global__ void __launch_bounds__(kThreads, 1)
-k_linear_tc(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapC, Params p) {
+k_linear_tc(const __grid_constant__ CUtensorMap tmapA, Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t sStage = sbase + kOffStage, sOut = sbase + kOffOut, sBar = sbase + kOffBar;
-  volatile uint32_t* s_tmem = reinterpret_cast<volatile uint32_t*>(smem + kOffTmem);
+  const uint32_t sStage = sbase + kOffStage, sBar = sbase + kOffBar;
   float* s_bias = reinterpret_cast<float*>(smem + kOffBias);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   auto bar = [&](int i) { return sBar + 8u * (uint32_t)i; };
+  const int n_items = p.n_tiles * p.n_nt;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(bar(B_FULL + i), 1);
-      mbar_init(bar(B_EMPTY + i), 1);
+      mbar_init(bar(B_EMPTY + i), kConsumers);
     }
-    mbar_init(bar(B_ACCFULL), 1);
-    mbar_init(bar(B_ACCFREE), 256);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(s_tmem)), kTmemCols);
   for (int i = threadIdx.x; i < 320; i += kThreads) s_bias[i] = (HAS_BIAS && i < p.N) ? p.bias[i] : 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
-  const uint32_t wslab_bytes = (uint32_t)p.Npad * 128u;
 
   if (warp == 0) {
     // ===================== TMA producer =====================
     uint32_t ks = 0;
-    for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const int t = item / p.n_nt, n0 = (item - t * p.n_nt) * kNT;
+      const uint32_t wbytes = (uint32_t)min(kNT, p.Npad - n0) * 128u;
       for (int s = 0; s < p.nslab; ++s, ++ks) {
         const uint32_t st = ks % kStages, use = ks / kStages;
         mbar_wait(bar(B_EMPTY + st), (use & 1) ^ 1);
         if (elect_one()) {
-          mbar_expect_tx(bar(B_FULL + st), kSlabBytes + wslab_bytes);
+          mbar_expect_tx(bar(B_FULL + st), kSlabBytes + wbytes);
           tma_load_2d(sStage + st * kStageBytes, &tmapA, bar(B_FULL + st), s * 64, t * kTileM);
-          bulk_load(sStage + st * kStageBytes + kSlabBytes, p.Wpk + (size_t)s * wslab_bytes, wslab_bytes, bar(B_FULL + st));
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const int n0 = p.Npad <= 256 ? p.Npad : 160;
-    const int n1 = p.Npad - n0;
-    const uint32_t idesc0 = umma_idesc_bf16(kTileM, n0);
-    const uint32_t idesc1 = umma_idesc_bf16(kTileM, n1 > 0 ? n1 : 16);
-    uint32_t ks = 0;
-    int it = 0;
-    for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x, ++it) {
-      mbar_wait(bar(B_ACCFREE), (it & 1) ^ 1);   // the previous tile's accumulator has been drained
-      tc_fence_after();
-      for (int s = 0; s < p.nslab; ++s, ++ks) {
-        const uint32_t st = ks % kStages, use = ks / kStages;
-        mbar_wait(bar(B_FULL + st), use & 1);
-        tc_fence_after();
-        const int nk = (s == p.nslab - 1) ? p.ksteps_last : 4;
-        const uint64_t adesc = umma_desc_sw128(sStage + st * kStageBytes);
-        const uint64_t bdesc0 = umma_desc_sw128(sStage + st * kStageBytes + kSlabBytes);
-        const uint64_t bdesc1 = umma_desc_sw128(sStage + st * kStageBytes + kSlabBytes + (uint32_t)n0 * 128u);
-        if (elect_one()) {
-          for (int kk = 0; kk < nk; ++kk) {
-            const uint32_t acc = (s > 0 || kk > 0) ? 1u : 0u;
-            umma_bf16(tmem_base, adesc + (uint64_t)(2 * kk), bdesc0 + (uint64_t)(2 * kk), idesc0, acc);
-            if (n1 > 0) umma_bf16(tmem_base + (uint32_t)n0, adesc + (uint64_t)(2 * kk), bdesc1 + (uint64_t)(2 * kk), idesc1, acc);
-          }
-          umma_commit(bar(B_EMPTY + st));
-          if (s == p.nslab - 1) umma_commit(bar(B_ACCFULL));
+          bulk_load(sStage + st * kStageBytes + kSlabBytes, p.Wpk + (size_t)s * p.Npad * 128 + (size_t)n0 * 128, wbytes,
+                    bar(B_FULL + st));
         }
         __syncwarp();
       }
     }
   } else if (warp >= 4) {
-    // ===================== epilogue: 2 groups x 4 warps, group g owns output slabs g, g+2, ... =====
-    const int eg = (warp - 4) >> 2;
-    const int et = threadIdx.x - 128 - eg * 128;           // 0..127 in the group == tile row == TMEM lane
-    const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-    const uint32_t obuf = sOut + eg * kSlabBytes;
-    const int nj = p.Npad >> 4;
-    const int nos = (p.Npad + 63) >> 6;                     // 64-column output slabs
-    int it = 0;
-    for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x, ++it) {
-      mbar_wait(bar(B_ACCFULL), it & 1);
-      tc_fence_after();
-      for (int s = eg; s < nos; s += 2) {
-        // the TMA store that last read this staging buffer must have finished reading it
-        if (et == 0) bulk_wait_group_read0();
-        if (eg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
-        else asm volatile("bar.sync 3, 128;" ::: "memory");
-        const int njj = min(4, nj - 4 * s);
-        for (int jj = 0; jj < njj; ++jj) {
-          const int j = 4 * s + jj;
-          uint32_t v[16];
-          tmem_ld16(taddr + j * 16, v);
-          // residual (base.py:138, H_0 + W_h M): the thread's own output row, one 32-byte sector per 16 columns
-          uint4 r0 = make_uint4(0, 0, 0, 0), r1 = make_uint4(0, 0, 0, 0);
-          if (p.res != nullptr) {
-            const int64_t grow = (int64_t)t * kTileM + et;
-            if (grow < p.R) {
-              const uint4* rp = reinterpret_cast<const uint4*>(p.res + grow * p.ldres + j * 16);
-              r0 = __ldg(rp);
-              r1 = __ldg(rp + 1);
-            }
-          }
-          tmem_wait_ld();
-          const uint32_t rw[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-          uint32_t o[8];
+    // ===================== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =====================
+    // W rows past the item's last column may hold stale data of an earlier stage: they only reach accumulator columns
+    // that the epilogue never stores.
+    const int wg = (warp - 4) >> 2;
+    const int tt = threadIdx.x - 128 - wg * 128;
+    const int rl = wg * 64 + acc_row0(tt), cl = acc_col0(tt);
+    uint32_t ks = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const int t = item / p.n_nt, n0 = (item - t * p.n_nt) * kNT;
+      float acc[76];
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            float z0 = __uint_as_float(v[2 * q]) + bf_lo(rw[q]), z1 = __uint_as_float(v[2 * q + 1]) + bf_hi(rw[q]);
-            if constexpr (HAS_BIAS) { z0 += s_bias[j * 16 + 2 * q]; z1 += s_bias[j * 16 + 2 * q + 1]; }
-            if constexpr (ACT == DMPNN_ACT_RELU) o[q] = act_word<ACT>(pack_bf2(z0, z1), 0.f);
-            else o[q] = pack_bf2(act_t<ACT>(p.act_param, z0), act_t<ACT>(p.act_param, z1));
-          }
-          sts128(obuf + sw128_off(et, 2 * jj), make_uint4(o[0], o[1], o[2], o[3]));
-          sts128(obuf + sw128_off(et, 2 * jj + 1), make_uint4(o[4], o[5], o[6], o[7]));
-        }
-        if (s + 2 >= nos) {           // last slab of this group in this tile: accumulator fully read
-          tc_fence_before();
-          mbar_arrive(bar(B_ACCFREE));
-        }
-        fence_proxy_async();          // staging writes -> visible to the TMA store (async proxy)
-        if (eg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
-        else asm volatile("bar.sync 3, 128;" ::: "memory");
-        if (et == 0) {
-          tma_store_2d(&tmapC, obuf, s * 64, t * kTileM);    // clipped at the tensor bounds (rows >= R, cols >= Npad)
-          bulk_commit_group();
-        }
+      for (int i = 0; i < 76; ++i) acc[i] = 0.f;
+      for (int s = 0; s < p.nslab; ++s, ++ks) {
+        const uint32_t st = ks % kStages, use = ks / kStages;
+        mbar_wait(bar(B_FULL + st), use & 1);
+        const int nk = (s == p.nslab - 1) ? p.ksteps_last : 4;
+        const uint64_t adesc = desc_sw128(sStage + st * kStageBytes + (uint32_t)wg * 8192u);
+        const uint64_t bdesc = desc_sw128(sStage + st * kStageBytes + kSlabBytes);
+        wgmma_fence();
+        for (int kk = 0; kk < nk; ++kk) wgmma_bf16_n152(acc, adesc + (uint64_t)(2 * kk), bdesc + (uint64_t)(2 * kk), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence(acc);
+        mbar_arrive(bar(B_EMPTY + st));
       }
-      if (nos <= eg) {                // this group had no slab: it still has to release the accumulator
-        tc_fence_before();
-        mbar_arrive(bar(B_ACCFREE));
+      // epilogue: rows rl, rl + 8 of the tile; columns n0 + 8 b + cl + {0, 1}
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t grow = (int64_t)t * kTileM + rl + 8 * h;
+        if (grow >= p.R) continue;
+        __nv_bfloat16* crow = p.C + grow * p.ldc;
+        const __nv_bfloat16* rrow = p.res != nullptr ? p.res + grow * p.ldres : nullptr;
+#pragma unroll
+        for (int b = 0; b < kNT / 8; ++b) {
+          const int n = n0 + 8 * b + cl;
+          if (n >= p.Npad) continue;
+          float z0 = acc[4 * b + 2 * h], z1 = acc[4 * b + 2 * h + 1];
+          if (rrow != nullptr) {
+            const uint32_t rw = __ldg(reinterpret_cast<const unsigned int*>(rrow + n));
+            z0 += bf_lo(rw); z1 += bf_hi(rw);
+          }
+          if constexpr (HAS_BIAS) { z0 += s_bias[n]; z1 += s_bias[n + 1]; }
+          uint32_t o;
+          if constexpr (ACT == DMPNN_ACT_RELU) o = act_word<ACT>(pack_bf2(z0, z1), 0.f);
+          else o = pack_bf2(act_t<ACT>(p.act_param, z0), act_t<ACT>(p.act_param, z1));
+          *reinterpret_cast<uint32_t*>(crow + n) = o;
+        }
       }
     }
-    if (et == 0) bulk_wait_group0();  // all stores complete before the CTA exits
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
@@ -265,14 +199,14 @@ static bool encode_map(EncodeTiledFn enc, CUtensorMap* tmap, const void* base, i
 }
 
 template <int ACT, bool HAS_BIAS>
-static cudaError_t launch_variant(int grid, cudaStream_t st, const CUtensorMap& mA, const CUtensorMap& mC, const Params& p) {
+static cudaError_t launch_variant(int grid, cudaStream_t st, const CUtensorMap& mA, const Params& p) {
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(k_linear_tc<ACT, HAS_BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemAlloc);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  k_linear_tc<ACT, HAS_BIAS><<<grid, kThreads, kSmemAlloc, st>>>(mA, mC, p);
+  k_linear_tc<ACT, HAS_BIAS><<<grid, kThreads, kSmemAlloc, st>>>(mA, p);
   return cudaSuccess;
 }
 
@@ -316,15 +250,16 @@ extern "C" int dmpnn_linear_tc_bf16(const void* A, int64_t lda, int64_t R, int64
                   "linear_tc: residual needs ldres >= %d, a multiple of 8, 16-byte alignment, and may not alias C", g.Npad);
   EncodeTiledFn enc = get_encode_fn();
   DMPNN_CHECK_ARG(enc != nullptr, "linear_tc: cuTensorMapEncodeTiled not available from the driver");
-  CUtensorMap mA, mC;
+  CUtensorMap mA;
   // A columns beyond K are zero-filled by TMA (the tensor's inner extent is exactly K)
-  DMPNN_CHECK_ARG(encode_map(enc, &mA, A, K, R, lda) && encode_map(enc, &mC, Cout, g.Npad, R, ldc),
-                  "linear_tc: cuTensorMapEncodeTiled failed");
+  DMPNN_CHECK_ARG(encode_map(enc, &mA, A, K, R, lda), "linear_tc: cuTensorMapEncodeTiled failed");
   Params p;
   p.Wpk = (const uint8_t*)Wpk;
   p.bias = bias;
   p.res = (const __nv_bfloat16*)res;
   p.ldres = ldres;
+  p.C = (__nv_bfloat16*)Cout;
+  p.ldc = ldc;
   p.R = R;
   p.K = (int)K;
   p.N = (int)N;
@@ -332,6 +267,7 @@ extern "C" int dmpnn_linear_tc_bf16(const void* A, int64_t lda, int64_t R, int64
   p.nslab = g.nslab;
   p.ksteps_last = (g.Kpad - 64 * (g.nslab - 1)) / 16;
   p.n_tiles = (int)((R + kTileM - 1) / kTileM);
+  p.n_nt = (g.Npad + kNT - 1) / kNT;
   p.act_param = act_param;
   static int sm_count = 0;
   if (!sm_count) {
@@ -339,11 +275,12 @@ extern "C" int dmpnn_linear_tc_bf16(const void* A, int64_t lda, int64_t R, int64
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
   }
-  const int grid = p.n_tiles < sm_count ? p.n_tiles : sm_count;
+  const int items = p.n_tiles * p.n_nt;
+  const int grid = items < sm_count ? items : sm_count;
   cudaError_t e = cudaErrorInvalidValue;
 #define DMPNN_LAUNCH_ACT(A_)                                                                                   \
   case A_:                                                                                                     \
-    e = bias ? launch_variant<A_, true>(grid, st, mA, mC, p) : launch_variant<A_, false>(grid, st, mA, mC, p); \
+    e = bias ? launch_variant<A_, true>(grid, st, mA, p) : launch_variant<A_, false>(grid, st, mA, p); \
     break;
   switch (act) {
     DMPNN_LAUNCH_ACT(DMPNN_ACT_NONE)

@@ -1,4 +1,4 @@
-// Fused Blackwell depth step of BondMessagePassing (bf16 hidden states), one launch per step:
+// Fused Hopper depth step of BondMessagePassing (bf16 hidden states), one launch per step:
 //
 //   H_next[rev(e')] = tau( H_0[rev(e')] + b + W_h . ( sum_{e'' in in(v)} g(H[e'']) - g(H[e']) ) ),  e' in in(v)
 //
@@ -10,19 +10,16 @@
 //               over slab by slab (box s of the next tile is loaded when the message warps have left slab s); L2 prefetch
 //   warp 1      TMA producer: W_h stages (pre-packed smem images, cp.async.bulk): an 80-column output chunk x one
 //               k pass (slabs {0,1,2} | {3,4}), 2-stage ring of 30 KB
-//   warp 2      tcgen05.mma issuer (converged warp, elected lane) + TMEM allocator:
-//               D[128 x hp] (TMEM, fp32) = A (TMEM, bf16) . W_h^T (smem)
-//   warp 3      TMA producer: H_0 slabs -> four staging buffers (two per epilogue group)
-//   warps 4-11  epilogue (2 groups, alternating slab parity per tile): tcgen05.ld -> + H_0[rev] + bias -> tau -> bf16
-//               in the staging slab at row rev(e') -> coalesced copy-out
+//   warp 3      L2 prefetch of the next tile's H_0 rows (and of the backward addends)
+//   warps 4-11  two warpgroups, tile rows [0, 64) / [64, 128): wgmma m64n80k16, D (registers, fp32) = A (smem, bf16)
+//               . W_h^T (smem), chunk by chunk, then the epilogue from registers: + H_0 + bias -> tau -> bf16 -> HBM
 //   warps 12-19 message: thread = row e': sums the sibling rows of e' (same destination atom) out of the
-//               shared-memory tile and writes the bf16 result row into tensor memory (tcgen05.st) = A operand;
+//               shared-memory tile and writes the bf16 result row into the shared-memory A operand tile;
 //               optionally also to HBM (M_out / G_out, one 32-byte sector per thread) for the W_h gradient
-// The row permutation by rev() is applied for free where the epilogue writes row rev(e').
 //
 // The same kernel runs the autograd mirror of the step (MODE_BWD_*, dmpnn_bond_step_bwd_fused_bf16):
 //   dOut = ((S.P) dZ) . W_h [* tau'(Y)]  -- the message warps read the sibling rows through a tile-local rev() table,
-//   W is the packed W_h^T, the epilogue writes row e' itself and multiplies by tau' of the staged Y.
+//   W is the packed W_h^T, the epilogue writes row e' itself and multiplies by tau' of Y.
 //
 // Algorithmic HBM bytes per step: read H_prev + H_0, write H_next = 3*E*h*2 (2*E*h*2 when first_step,
 // H_prev == H_0 comes from L2 the second time); W_h (<=190 KB) is L2-resident.

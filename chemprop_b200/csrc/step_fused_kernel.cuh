@@ -1,6 +1,6 @@
 // The fused depth-step kernel of csrc/step_fused.cu (see there for the description), as a template: its ~70 instantiations
 // (activation x first step x bias x autograd-mirror mode x {windows of oversized molecules} x {dropout in the epilogue}) are
-// compiled in four translation units in parallel (step_fused_{fwd,bwd,far_fwd,far_bwd}.cu).
+// compiled in six translation units in parallel (step_fused_{fwd,bwd,far_fwd,far_bwd,atom_fwd,atom_bwd}.cu).
 #pragma once
 #include <cuda.h>
 #include <stdlib.h>
@@ -14,75 +14,25 @@ namespace fused {
 constexpr int kTileM = 128;
 constexpr int kSlabBytes = kTileM * 128;        // one 64-column K slab of a 128-row tile: 16 KB
 constexpr int kMaxSlabs = 5;                    // hp <= 320
-#ifndef DMPNN_ASLOTS
-#define DMPNN_ASLOTS 5
-#endif
-constexpr int kASlots = DMPNN_ASLOTS;           // shared-memory slots of the raw H tile's 64-column slabs (ring when < kMaxSlabs)
-constexpr int kABufBytes = kASlots * kSlabBytes;
-constexpr int kChunkN = 80;                     // W stage / accumulator chunk = 80 output features (5 x 16)
+constexpr int kABufBytes = kMaxSlabs * kSlabBytes;
+constexpr int kChunkN = 80;                     // W stage / accumulator chunk = 80 output features (the wgmma N)
 constexpr int kMaxChunks = 4;
-// A W stage = an 80-column chunk x up to kWHalfSlabs k slabs; the A tile is handed over in k passes of that many slabs.
-// 3 slabs (passes {0,1,2} | {3,4}, 12 + 7 MMAs per stage, 2 stages of 30 KB) measured 211 us per step at the bench
-// size; 2 slabs (three passes, 3 stages of 20 KB, 8 MMAs per stage) 256 us: the per-stage barrier round trip is not
-// amortised by 8 MMAs.
+// A W stage = an 80-column chunk x up to kWHalfSlabs k slabs; the A operand tile is handed over in k passes of that many
+// slabs ({0,1,2} | {3,4}).
 constexpr int kWHalfSlabs = 3;
 constexpr int kMaxPasses = (kMaxSlabs + kWHalfSlabs - 1) / kWHalfSlabs;   // 2
 constexpr int kWStageBytes = kWHalfSlabs * kChunkN * 128;   // 30 KB
-// Build-time variants (tools/build_variants.sh A/Bs them through tests/native/fused_step_harness):
-//   DMPNN_H0_DIRECT  1: the epilogue reads its H_0 / Y row straight from global memory (one 32-byte sector per thread and
-//                    block, software-pipelined one block ahead; the rows are L2-resident, prefetched a tile ahead by warp 3)
-//                    instead of from TMA-staged slabs -- frees 64 KB of shared memory;
-//   DMPNN_WSTAGES    depth of the W_h stage ring (30 KB each).  The MMA passes are paced by the latency of the W stages
-//                    (182 KB per tile from L2 in 8 stages): 2 stages = 60 KB in flight, 4 stages = 120 KB.
-#ifndef DMPNN_H0_DIRECT
-#define DMPNN_H0_DIRECT 0
-#endif
-#ifndef DMPNN_WSTAGES
-#define DMPNN_WSTAGES (DMPNN_H0_DIRECT ? 4 : 2)
-#endif
-//   DMPNN_MMA_ORDER  order of the (accumulator chunk, k pass) stages in the MMA warp's in-order stream.  The accumulator is
-//                    single-buffered: chunk c of tile k+1 waits for the epilogue of tile k to drain chunk c, and the A tile
-//                    (TMEM) is single-buffered too: the message warps of tile k+2 wait for the last reader of each k half.
-//                    0 = pass-major (first k pass over all chunks, then the second) -- the product.  The LAST chunk's first
-//                        pass (freed when the previous epilogue ENDS) stands in front of the FIRST chunk's second pass, so an
-//                        epilogue starts ~1.5 us after the previous one has ended (profiles/r2_trace_block0.log: period
-//                        5.3 us = 3.8 us epilogue + that hand-over); but the first pass runs under the message phase;
-//                    1 = chunk-major: no hand-over gap, but every k half of A stays busy until the last chunk is done and
-//                        the message warps start late: 214-226 us against 189-195 (profiles/r2_fused_step_variants.log);
-//                    2 = pass-major over all chunks but the last, then the last chunk: 216 us -- the second pass of chunks
-//                        0..n-2 waits for the whole A tile, and the last chunk's first pass (the A half's last reader) queues
-//                        behind it.
-//                    Neither reordering helps while A and the accumulator are single-buffered (TMEM: 304 + 152 of 512
-//                    columns); a deeper W ring (timing-only builds with 3 / 4 stages) changes nothing either.
-#ifndef DMPNN_MMA_ORDER
-#define DMPNN_MMA_ORDER 0
-#endif
-constexpr int kMmaOrder = DMPNN_MMA_ORDER;
-// Timing experiments compiled in only with -DDMPNN_EXPERIMENTS=1 (tools/build_variants.sh; DMPNN_EXP selects at run time; results
-// are wrong by construction): 16384 epilogue skips tcgen05.ld, 32768 epilogue skips its global stores, 65536 message warps
-// skip their shared-memory gathers, 131072 message warps skip tcgen05.st, 262144 the MMA warp issues no MMA (commits only).
+constexpr int kWStages = 2;
+// Timing experiments compiled in only with -DDMPNN_EXPERIMENTS=1 (DMPNN_EXP selects at run time; results are wrong by
+// construction): 32768 epilogue skips its global stores, 65536 message warps skip their shared-memory gathers, 131072
+// message warps skip the A operand stores, 262144 the MMA warpgroups issue no MMA.
 #ifndef DMPNN_EXPERIMENTS
 #define DMPNN_EXPERIMENTS 0
 #endif
 constexpr bool kExp = DMPNN_EXPERIMENTS != 0;
-// stage q of a tile -> (chunk, k pass); the W producer and the MMA warp walk the same sequence
-__device__ __forceinline__ void mma_stage(int q, int nchunks, int npass, int& c, int& half) {
-  if (kMmaOrder == 0) { half = q / nchunks; c = q - half * nchunks; }
-  else if (kMmaOrder == 1) { c = q / npass; half = q - c * npass; }
-  else {
-    const int nb = (nchunks - 1) * npass;
-    if (q < nb) { half = q / (nchunks - 1); c = q - half * (nchunks - 1); }
-    else { c = nchunks - 1; half = q - nb; }
-  }
-}
-constexpr bool kH0Direct = DMPNN_H0_DIRECT != 0;
-constexpr int kWStages = DMPNN_WSTAGES;
-constexpr int kHStages = kH0Direct ? 0 : 4;     // H_0 staging slabs (16 KB each): two per epilogue group
 constexpr int kThreads = 640;
 constexpr int kSWarps = 8;          // message warps (12..19)
-constexpr int kEpiGroups = 2;       // two groups of 4 epilogue warps (4..7, 8..11), alternate slabs
-constexpr int kTmemCols = 512;
-constexpr int kTmemAOff = 320;                // A operand (bf16x2-packed message tile) lives at TMEM columns [320, 472)
+constexpr int kMmaThreads = 256;    // two MMA + epilogue warpgroups (warps 4..7, 8..11)
 constexpr int kMaxHp = 304;
 
 struct Params {
@@ -116,29 +66,27 @@ struct Params {
 
 // shared memory carve-up (after 1024 B alignment)
 constexpr int kOffA = 0;                                     // raw H tile (single buffer, read-only for the SMs)
-constexpr int kOffW = kABufBytes;                            // 81920
-constexpr int kOffH = kOffW + kWStages * kWStageBytes;       // 184320 (1024-aligned)
-constexpr int kOffBar = kOffH + kHStages * kSlabBytes;       // 217088
-constexpr int kNumBars = 40;
-constexpr int kOffTmem = kOffBar + kNumBars * 8;
-constexpr int kOffRowptr = kOffTmem + 16;                    // int32 [2][132]
+constexpr int kOffAop = kABufBytes;                          // A operand tile written by the message warps: 81920
+constexpr int kOffW = kOffAop + kABufBytes;                  // 163840
+constexpr int kOffBar = kOffW + kWStages * kWStageBytes;     // 225280
+constexpr int kNumBars = 24;
+constexpr int kOffRowptr = kOffBar + kNumBars * 8;           // int32 [2][132]
 constexpr int kOffRevl = kOffRowptr + 2 * 132 * 4;           // int16 [2][128]: tile-local rev() (backward mode)
 constexpr int kOffBias = kOffRevl + 2 * 128 * 2;             // float [304]
-constexpr int kNbCap = 1024;                                 // ATOM kernels: staged neighbour entries per tile (else global look-ups)
+constexpr int kNbCap = 512;                                  // ATOM kernels: staged neighbour entries per tile (else global look-ups)
 constexpr int kOffNb = kOffBias + kMaxHp * 4;                // int16 [2][kNbCap]: tile-local neighbour rows of the atom tile
 constexpr int kSmemBytes = kOffNb + 2 * kNbCap * 2;
 constexpr int kSmemAlloc = kSmemBytes + 1024;
-static_assert(kOffH % 1024 == 0, "staging slabs must be 1024-byte aligned for SWIZZLE_128B");
+static_assert(kOffAop % 1024 == 0 && kOffW % 1024 == 0, "operand tiles must be 1024-byte aligned for SWIZZLE_128B");
 static_assert(kSmemAlloc <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
 
 enum {
   B_AFULL = 0, B_AFREE = B_AFULL + kMaxSlabs,        // the H tile is handed over slab by slab (64 columns)
-  B_AREADY = B_AFREE + kMaxSlabs, B_ATFREE = B_AREADY + kMaxPasses, B_ACCFULL = B_ATFREE + kMaxPasses,
-  B_ACCFREE = B_ACCFULL + 4,
-  B_HFULL = B_ACCFREE + 4, B_HFREE = B_HFULL + 4, B_WFULL = B_HFREE + 4, B_WFREE = B_WFULL + kWStages
+  B_AREADY = B_AFREE + kMaxSlabs, B_ATFREE = B_AREADY + kMaxPasses,
+  B_WFULL = B_ATFREE + kMaxPasses, B_WFREE = B_WFULL + kWStages
 };
 static_assert(B_WFREE + kWStages <= kNumBars, "barrier table too small");
-static_assert(kMaxSlabs == 5 && kMaxChunks <= 4 && (kHStages == 4 || kHStages == 0), "barrier numbering assumes these");
+static_assert(kMaxSlabs == 5 && kMaxChunks <= 4, "barrier numbering assumes these");
 
 using namespace dmpnn::tc;
 
@@ -152,7 +100,7 @@ __device__ __forceinline__ void trace_ev(const Params& p, int it, int ev) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// MODE 0: forward step (message of H, epilogue tau(H_0[rev] + bias + acc) written to row rev(e'))
+// MODE 0: forward step (message of H, epilogue tau(H_0 + bias + acc) written to row e')
 // MODE 1: autograd mirror, masked:  A row e' = sum of dZ[rev(x)] over the siblings x of e';  out[e'] = acc * tau'(Y[e'])
 // MODE 2: autograd mirror, plain:   same gather;  out[e'] = acc
 // MODE_BWD_LAST: mask from the PRE-activation (Y = H_0) and up to two row-aligned addends summed into the output:
@@ -173,8 +121,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
   // the address space, so the row-pointer / rev() table look-ups of the message warps are LDS instead of generic LD.E
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t sA = sbase + kOffA, sW = sbase + kOffW, sH = sbase + kOffH, sBar = sbase + kOffBar;
-  volatile uint32_t* s_tmem = reinterpret_cast<volatile uint32_t*>(smem + kOffTmem);
+  const uint32_t sA = sbase + kOffA, sAop = sbase + kOffAop, sW = sbase + kOffW, sBar = sbase + kOffBar;
   int32_t* s_rowptr = reinterpret_cast<int32_t*>(smem + kOffRowptr);
   int16_t* s_revl = reinterpret_cast<int16_t*>(smem + kOffRevl);
   float* s_bias = reinterpret_cast<float*>(smem + kOffBias);
@@ -187,35 +134,20 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
       mbar_init(bar(B_AFULL + i), 1);
       mbar_init(bar(B_AFREE + i), kSWarps * 32);  // every message thread is done reading this slab of the tile
     }
-    for (int i = 0; i < kMaxPasses; ++i) {      // the TMEM A tile is handed over k pass by k pass (slabs {0,1} | {2,3} | {4})
-      mbar_init(bar(B_AREADY + i), kSWarps * 32);   // message threads have written this k half of their row
-      mbar_init(bar(B_ATFREE + i), 1);              // tensor core finished reading this k half
-    }
-    for (int i = 0; i < kHStages; ++i) {
-      mbar_init(bar(B_HFULL + i), 1);
-      mbar_init(bar(B_HFREE + i), 128);
+    for (int i = 0; i < kMaxPasses; ++i) {      // the A operand tile is handed over k pass by k pass (slabs {0,1,2} | {3,4})
+      mbar_init(bar(B_AREADY + i), kSWarps * 32);   // message threads have written this k pass of their row
+      mbar_init(bar(B_ATFREE + i), kMmaThreads);    // both warpgroups' MMAs have finished reading this k pass
     }
     for (int i = 0; i < kWStages; ++i) {
       mbar_init(bar(B_WFULL + i), 1);
-      mbar_init(bar(B_WFREE + i), 1);
-    }
-    for (int i = 0; i < kMaxChunks; ++i) {
-      // an 80-column accumulator chunk is released by every epilogue group that reads part of it
-      int groups = 0;
-      for (int j = 5 * i; j < 5 * i + 5 && j < (p.hp >> 4); ++j) groups |= 1 << ((j >> 2) & 1);
-      mbar_init(bar(B_ACCFULL + i), 1);
-      mbar_init(bar(B_ACCFREE + i), 128 * max(1, __popc(groups)));
+      mbar_init(bar(B_WFREE + i), kMmaThreads);
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(s_tmem)), kTmemCols);
   for (int i = threadIdx.x; i < kMaxHp; i += kThreads) s_bias[i] = (p.bias && i < p.h) ? p.bias[i] : 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
-  const bool alt_groups = p.nslab >= 3 && (p.nslab & 1);   // alternate the epilogue groups' slab parity per tile
   const int n_items = p.n_work_dev ? __ldg(p.n_work_dev) : p.n_tiles;   // work items of this launch (uniform over the grid)
+  const int npass = (p.nslab + kWHalfSlabs - 1) / kWHalfSlabs;
 
   if (warp == 0) {
     // ===================== TMA producer: H_prev tile -> shared memory (single buffer) =====================
@@ -233,7 +165,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
         if (elect_one()) {
           if (s == 0) trace_ev(p, it, 0);
           mbar_expect_tx(bar(B_AFULL + s), kSlabBytes);
-          tma_load_2d(sA + (s % kASlots) * kSlabBytes, &tmapH, bar(B_AFULL + s), s * 64, row0);
+          tma_load_2d(sA + s * kSlabBytes, &tmapH, bar(B_AFULL + s), s * 64, row0);
         }
         __syncwarp();
       }
@@ -243,14 +175,12 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
     }
   } else if (warp == 1) {
     // ===================== TMA producer: W_h stages (pre-packed smem images) =====================
-    // a stage = the W_h rows of one 80-column output chunk for k slabs {0,1,2} or {3,4} (contiguous in the image)
+    // a stage = the W_h rows of one 80-column output chunk for k slabs {0,1,2} or {3,4} (contiguous in the image), in the
+    // MMA warpgroups' order: chunk by chunk, both k passes of a chunk back to back
     uint32_t ws = 0;
-    const int npass = (p.nslab + kWHalfSlabs - 1) / kWHalfSlabs;
     for (int t = blockIdx.x; t < n_items; t += gridDim.x) {
-      {
-        for (int q = 0; q < p.nchunks * npass; ++q, ++ws) {        // stage order = the MMA warp's (mma_stage)
-          int c, half;
-          mma_stage(q, p.nchunks, npass, c, half);
+      for (int c = 0; c < p.nchunks; ++c)
+        for (int half = 0; half < npass; ++half, ++ws) {
           const int s0 = half * kWHalfSlabs;
           const int ns = min(kWHalfSlabs, p.nslab - s0);
           const int nc = min(kChunkN, p.hp - c * kChunkN);
@@ -268,80 +198,21 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
           }
           __syncwarp();
         }
-      }
-    }
-  } else if (warp == 2) {
-    // ===================== MMA issuer (converged warp, one elected lane issues) =====================
-    // D[128 x hp] (TMEM cols 0..) += A (TMEM cols kTmemAOff.., written by the message warps) . W_h^T (smem ring)
-    uint32_t ws = 0;
-    int it = 0;
-    const int npass = (p.nslab + kWHalfSlabs - 1) / kWHalfSlabs;
-    for (int t = blockIdx.x; t < n_items; t += gridDim.x, ++it) {
-      {
-        uint32_t a_waited = 0;                                           // k halves of this tile's A already waited for
-        for (int q = 0; q < p.nchunks * npass; ++q, ++ws) {
-          int c, half;                                                   // half = k pass over one half of the A tile
-          mma_stage(q, p.nchunks, npass, c, half);
-          const int s0 = half * kWHalfSlabs;
-          const int ns = min(kWHalfSlabs, p.nslab - s0);
-          const bool last_pass = s0 + ns >= p.nslab;
-          const bool last_chunk = c == p.nchunks - 1;
-          if (!((a_waited >> half) & 1u)) {
-            a_waited |= 1u << half;
-            mbar_wait(bar(B_AREADY + half), it & 1);                     // the message warps have written this half
-            if (half == 0 && lane == 0) trace_ev(p, it, 3);
-            tc_fence_after();
-          }
-          const int nc = min(kChunkN, p.hp - c * kChunkN);
-          const uint32_t idesc = umma_idesc_bf16(kTileM, nc);
-          const uint32_t d_tmem = tmem_base + (uint32_t)(c * kChunkN);
-          if (s0 == 0) {
-            mbar_wait(bar(B_ACCFREE + c), (it & 1) ^ 1);   // epilogue of the previous tile drained these columns
-            if (c == 0 && lane == 0) trace_ev(p, it, 4);
-          }
-          const uint32_t st = ws % kWStages, usew = ws / kWStages;
-          mbar_wait(bar(B_WFULL + st), usew & 1);
-          tc_fence_after();
-          if (elect_one()) {
-            for (int si = 0; si < ns; ++si) {
-              const int s = s0 + si;
-              const int ks = (s == p.nslab - 1) ? p.ksteps_last : 4;
-              const uint32_t a_tmem = tmem_base + kTmemAOff + (uint32_t)(s * 32);   // 64 bf16 = 32 columns per k slab
-              const uint64_t bdesc = umma_desc_sw128(sW + st * kWStageBytes + (uint32_t)(si * nc * 128));
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk)   // k step = 16 bf16 = 8 TMEM columns of A = 32 B of each W row
-                if (kk < ks && !(kExp && (p.exp_flags & 262144)))
-                  umma_bf16_ts(d_tmem, a_tmem + (uint32_t)(8 * kk), bdesc + (uint64_t)(2 * kk), idesc, (s > 0 || kk > 0) ? 1u : 0u);
-            }
-            umma_commit(bar(B_WFREE + st));
-            if (last_pass) umma_commit(bar(B_ACCFULL + c));
-            // this k half of the A tile may be overwritten once its last reader (the last chunk's pass over it) is done
-            if (last_chunk) umma_commit(bar(B_ATFREE + half));
-          }
-          __syncwarp();
-        }
-      }
-      if (lane == 0) trace_ev(p, it, 5);
     }
   } else if (warp == 3) {
-    // ===================== TMA producer: H_0 slabs -> staging buffers (two per epilogue group) ==========
-    uint32_t cnt[2] = {0u, 0u};   // slabs handed to each group so far
-    int it = 0;
-    // first rows of this tile and of the next, loaded one and two tiles ahead: nothing below waits for a load it just issued
-    int row_c = (int)blockIdx.x < n_items ? __ldg(p.tile_row_ptr + blockIdx.x) : 0;
+    // ===================== L2 prefetch of the epilogue's row streams, one tile ahead ==========
     int row_n = (int)(blockIdx.x + gridDim.x) < n_items ? __ldg(p.tile_row_ptr + blockIdx.x + gridDim.x) : -1;
-    for (int t = blockIdx.x; MODE != MODE_BWD_COPY && t < n_items; t += gridDim.x, ++it) {
-      const int row0 = row_c;
+    for (int t = blockIdx.x; MODE != MODE_BWD_COPY && t < n_items; t += gridDim.x) {
       const int tn = t + gridDim.x;
       const int rown = (tn < n_items && !(p.exp_flags & 2048)) ? row_n : -1;
-      row_c = row_n;
       row_n = (tn + (int)gridDim.x < n_items) ? __ldg(p.tile_row_ptr + tn + gridDim.x) : -1;
       if (rown >= 0 && elect_one())
         for (int s = 0; s < p.nslab; ++s) tma_prefetch_2d(&tmapH0, s * 64, rown);
       __syncwarp();
       if (MODE == MODE_BWD_LAST && p.add0 != nullptr) {
-        // the copy-out of this tile reads the addend rows with plain loads: pull them into L2 now (the rows of a
-        // tile are one contiguous byte range; this warp runs most of a tile ahead of the epilogue)
+        // the epilogue of this tile reads the addend rows with plain loads: pull them into L2 now (the rows of a
+        // tile are one contiguous byte range; this warp runs ahead of the epilogue)
+        const int row0 = __ldg(p.tile_row_ptr + t);
         const int nr = __ldg(p.tile_row_ptr + t + 1) - row0;
         const int64_t lines = ((int64_t)nr * p.ld * 2 + 127) >> 7;
         const char* b0 = reinterpret_cast<const char*>(p.add0 + (int64_t)row0 * p.ld);
@@ -351,176 +222,129 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
           if (b1) asm volatile("prefetch.global.L2 [%0];" ::"l"(b1 + (i << 7)));
         }
       }
-      for (int s = 0; !kH0Direct && s < p.nslab; ++s) {
-        const uint32_t g = (uint32_t)(s + (alt_groups ? it : 0)) & 1u, k = cnt[g]++;   // see the epilogue
-        const uint32_t q = g * 2 + (k & 1), use = k >> 1;
-        mbar_wait(bar(B_HFREE + q), (use & 1) ^ 1);
-        if (elect_one()) {
-          if (s == 0) trace_ev(p, it, 10);
-          mbar_expect_tx(bar(B_HFULL + q), kSlabBytes);
-          tma_load_2d(sH + q * kSlabBytes, &tmapH0, bar(B_HFULL + q), s * 64, row0);
-        }
-        __syncwarp();
-      }
     }
-  } else if (warp < 12) {
-    // ===================== epilogue (2 groups x 4 warps; thread == TMEM lane == GEMM row == OUTPUT row) ==========
-    // The message warps build A row r as the message of edge r itself (they gather through the tile-local rev() table),
-    // so accumulator row r is the update of edge r: it needs H_0 row r -- read from the TMA-staged slab at the thread's own
-    // row, which is bank-conflict free under the 128-byte swizzle -- and produces output row r, written straight from
-    // registers to global memory, one 32-byte sector per thread and 16-column block (STG.256; the four sectors of a
-    // 128-byte line merge in L2).  The staging slab is read-only: no staging writes, no group barrier, no copy-out pass.
-    // Group g owns the 64-column slabs s = g, g+2, ... so the two groups drain the accumulator concurrently.
-    const int eg = (warp - 4) >> 2;
-    const int et = threadIdx.x - 128 - eg * 128;  // 0..127 inside the group
-    const int r = et;                              // TMEM lane (warp & 3 selects the 32-lane quadrant)
-    const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
+  } else if (warp >= 4 && warp < 12) {
+    // ===================== MMA + epilogue: warpgroup wg owns tile rows [64 wg, 64 wg + 64) ==========
+    // D[64 x 80] (registers, fp32) = A (shared memory, written by the message warps) . W_h^T (W stage) per 80-column chunk;
+    // the epilogue of a chunk runs from registers right after its last k pass.  The message warps build A row r as the
+    // message of edge r itself (they gather through the tile-local rev() table), so accumulator row r is the update of
+    // edge r: it needs H_0 row r (global memory; L2-resident, prefetched a tile ahead by warp 3) and produces output row r.
+    // W rows past a chunk's last column may hold the next slab's rows or stale data: they only reach accumulator columns
+    // that the epilogue never stores.
+    const int wg = (warp - 4) >> 2;
+    const int tt = threadIdx.x - 128 - wg * 128;
+    const int rA = wg * 64 + acc_row0(tt), cl = acc_col0(tt);
     const int nj = p.hp >> 4;
-    uint32_t hcnt = 0;                             // slabs this group has consumed
+    uint32_t ws = 0;
     int it = 0;
-    int t = blockIdx.x;
-    int row0 = 0, nrows = 0;
-    if (t < n_items) {
-      row0 = __ldg(p.tile_row_ptr + t);
-      nrows = __ldg(p.tile_row_ptr + t + 1) - row0;
-    }
-    for (; t < n_items; t += gridDim.x, ++it) {
-      // prefetch the next tile's metadata (hides the dependent global loads behind this tile's work)
-      const int tn = t + gridDim.x;
-      int row0n = 0, nrowsn = 0;
-      if (tn < n_items) {
-        row0n = __ldg(p.tile_row_ptr + tn);
-        nrowsn = __ldg(p.tile_row_ptr + tn + 1) - row0n;
-      }
-      const bool rvalid = r < nrows;
-      __nv_bfloat16* orow = p.Hn + (int64_t)(row0 + r) * p.ld;
-      const __nv_bfloat16* yrow = p.H0 + (int64_t)(row0 + r) * p.ld;     // direct mode: this thread's H_0 / Y row
-      int cready = -1;                             // highest accumulator chunk already waited for
-      uint4 n0 = make_uint4(0, 0, 0, 0), n1 = n0;  // direct mode: the NEXT block's H_0 words, in flight one block ahead
-      if (kH0Direct && MODE != MODE_BWD_COPY && rvalid) {
-        const int sf = (eg + (alt_groups ? it : 0)) & 1;
-        if (sf < p.nslab) {
-          const uint4* yp = reinterpret_cast<const uint4*>(yrow + 64 * sf);
-          n0 = __ldg(yp); n1 = __ldg(yp + 1);
+    for (int t = blockIdx.x; t < n_items; t += gridDim.x, ++it) {
+      const int row0 = __ldg(p.tile_row_ptr + t);
+      const int nrows = __ldg(p.tile_row_ptr + t + 1) - row0;
+      uint32_t a_waited = 0;                                             // k passes of this tile's A already waited for
+      for (int c = 0; c < p.nchunks; ++c) {
+        float acc[40];
+#pragma unroll
+        for (int i = 0; i < 40; ++i) acc[i] = 0.f;
+        const int nc = min(kChunkN, p.hp - c * kChunkN);
+        for (int half = 0; half < npass; ++half, ++ws) {
+          const int s0 = half * kWHalfSlabs;
+          const int ns = min(kWHalfSlabs, p.nslab - s0);
+          if (!((a_waited >> half) & 1u)) {
+            a_waited |= 1u << half;
+            mbar_wait(bar(B_AREADY + half), it & 1);                     // the message warps have written this k pass
+            if (half == 0 && tt == 0 && wg == 0) trace_ev(p, it, 3);
+          }
+          const uint32_t st = ws % kWStages, usew = ws / kWStages;
+          mbar_wait(bar(B_WFULL + st), usew & 1);
+          if (!(kExp && (p.exp_flags & 262144))) {
+            wgmma_fence();
+            for (int si = 0; si < ns; ++si) {
+              const int s = s0 + si;
+              const int ks = (s == p.nslab - 1) ? p.ksteps_last : 4;
+              const uint64_t adesc = desc_sw128(sAop + (uint32_t)s * kSlabBytes + (uint32_t)wg * 8192u);
+              const uint64_t bdesc = desc_sw128(sW + st * kWStageBytes + (uint32_t)(si * nc * 128));
+              for (int kk = 0; kk < ks; ++kk)   // k step = 16 bf16 = 32 B of each operand row
+                wgmma_bf16_n80(acc, adesc + (uint64_t)(2 * kk), bdesc + (uint64_t)(2 * kk), 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            acc_fence(acc);
+          }
+          mbar_arrive(bar(B_WFREE + st));
+          // this k pass of the A tile may be overwritten once its last reader (the last chunk's pass over it) is done
+          if (c == p.nchunks - 1) mbar_arrive(bar(B_ATFREE + half));
         }
-      }
-      // group g takes the slabs s with (s + it) % 2 == g when the slab count is odd (5 at h = 300): the group that
-      // got three slabs of this tile gets two of the next, so both drain the accumulator in the same average time.
-      // (Not for 1 slab: a group idle for a whole tile would skip a phase of the parity-tracked ACCFULL barriers.)
-      for (int s = (eg + (alt_groups ? it : 0)) & 1; s < p.nslab; s += kEpiGroups, ++hcnt) {
-        const uint32_t q = (uint32_t)eg * 2 + (hcnt & 1);
-        const uint32_t hbuf = sH + q * kSlabBytes;
-        if (!kH0Direct && MODE != MODE_BWD_COPY) mbar_wait(bar(B_HFULL + q), (hcnt >> 1) & 1);
-        const int njj = (s == p.nslab - 1) ? p.ksteps_last : 4;
-        for (int jj = 0; jj < njj; ++jj) {
-          const int j = 4 * s + jj;
-          const int c = j / 5;
-          if (c > cready) {
-            mbar_wait(bar(B_ACCFULL + c), it & 1);
-            tc_fence_after();
-            if (et == 0 && cready < 0) trace_ev(p, it, 6 + eg);
-            cready = c;
-          }
-          uint32_t v[16];
-          if (kExp && (p.exp_flags & 16384)) {
+        if (c == 0 && tt == 0) trace_ev(p, it, 6 + wg);
+        // ---- epilogue of chunk c: rows rA, rA + 8; columns 80 c + 8 b + cl + {0, 1}
 #pragma unroll
-            for (int qq = 0; qq < 16; ++qq) v[qq] = 0u;
-          } else
-          tmem_ld16(taddr + j * 16, v);
-          uint4 h0 = make_uint4(0, 0, 0, 0), h1 = make_uint4(0, 0, 0, 0);
-          if constexpr (kH0Direct) {
-            h0 = n0; h1 = n1;
-            if (MODE != MODE_BWD_COPY && rvalid) {          // issue the next block's loads before this block's arithmetic
-              int jn2 = -1;
-              if (jj + 1 < njj) jn2 = j + 1;
-              else if (s + kEpiGroups < p.nslab) jn2 = 4 * (s + kEpiGroups);
-              if (jn2 >= 0) {
-                const uint4* yp = reinterpret_cast<const uint4*>(yrow + 16 * jn2);
-                n0 = __ldg(yp); n1 = __ldg(yp + 1);
-              }
-            }
-          } else if (MODE != MODE_BWD_COPY) { h0 = lds128(hbuf + sw128_off(r, 2 * jj)); h1 = lds128(hbuf + sw128_off(r, 2 * jj + 1)); }
-          uint4 a0 = make_uint4(0, 0, 0, 0), a1 = a0, b0 = a0, b1 = a0;
-          if (MODE == MODE_BWD_LAST && p.add0 != nullptr && rvalid) {
-            // dH_0 = (this step's masked gradient) + the earlier steps' dZ rows (L2 hits: prefetched by the staging warp)
-            const uint4* ap = reinterpret_cast<const uint4*>(p.add0 + (int64_t)(row0 + r) * p.ld + j * 16);
-            a0 = __ldg(ap); a1 = __ldg(ap + 1);
-            if (p.add1 != nullptr) {
-              const uint4* bp = reinterpret_cast<const uint4*>(p.add1 + (int64_t)(row0 + r) * p.ld + j * 16);
-              b0 = __ldg(bp); b1 = __ldg(bp + 1);
-            }
-          }
-          uint32_t kb = 0xffffu;
-          if (MODE == MODE_FWD && DROP && rvalid) kb = __ldg(p.drop_bits + (int64_t)(row0 + r) * nj + j);
-          tmem_wait_ld();
-          const uint32_t hw[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-          uint32_t o[8];
+        for (int h = 0; h < 2; ++h) {
+          const int r = rA + 8 * h;
+          if (r >= nrows) continue;
+          const int64_t grow = (int64_t)(row0 + r);
+          __nv_bfloat16* orow = p.Hn + grow * p.ld;
+          const __nv_bfloat16* yrow = p.H0 + grow * p.ld;
 #pragma unroll
-          for (int qq = 0; qq < 8; ++qq) {
+          for (int b = 0; b < kChunkN / 8; ++b) {
+            const int n = c * kChunkN + 8 * b + cl;
+            if (8 * b >= nc) continue;
+            const float v0 = acc[4 * b + 2 * h], v1 = acc[4 * b + 2 * h + 1];
+            uint32_t o;
             if constexpr (MODE == MODE_BWD_COPY) {          // dOut = (S.P)(dZ) . W_h
-              o[qq] = pack_bf2(__uint_as_float(v[2 * qq]), __uint_as_float(v[2 * qq + 1]));
-              continue;
-            } else if constexpr (MODE == MODE_BWD_MASK || MODE == MODE_BWD_LAST) {
-              // ... * tau'(.): from the activation output the row came from, or (LAST) from the pre-activation H_0
-              const float g0 = MODE == MODE_BWD_LAST ? act_grad_from_pre(ACT, p.act_param, bf_lo(hw[qq]))
-                                                     : act_grad_from_out(ACT, p.act_param, bf_lo(hw[qq]));
-              const float g1 = MODE == MODE_BWD_LAST ? act_grad_from_pre(ACT, p.act_param, bf_hi(hw[qq]))
-                                                     : act_grad_from_out(ACT, p.act_param, bf_hi(hw[qq]));
-              float z0 = __uint_as_float(v[2 * qq]) * g0, z1 = __uint_as_float(v[2 * qq + 1]) * g1;
-              if constexpr (MODE == MODE_BWD_LAST) {
-                const uint32_t aw[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-                const uint32_t bw[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-                z0 += bf_lo(aw[qq]) + bf_lo(bw[qq]);
-                z1 += bf_hi(aw[qq]) + bf_hi(bw[qq]);
+              o = pack_bf2(v0, v1);
+            } else {
+              const uint32_t hw = __ldg(reinterpret_cast<const unsigned int*>(yrow + n));
+              if constexpr (MODE == MODE_BWD_MASK || MODE == MODE_BWD_LAST) {
+                // ... * tau'(.): from the activation output the row came from, or (LAST) from the pre-activation H_0
+                const float g0 = MODE == MODE_BWD_LAST ? act_grad_from_pre(ACT, p.act_param, bf_lo(hw))
+                                                       : act_grad_from_out(ACT, p.act_param, bf_lo(hw));
+                const float g1 = MODE == MODE_BWD_LAST ? act_grad_from_pre(ACT, p.act_param, bf_hi(hw))
+                                                       : act_grad_from_out(ACT, p.act_param, bf_hi(hw));
+                float z0 = v0 * g0, z1 = v1 * g1;
+                if (MODE == MODE_BWD_LAST && p.add0 != nullptr) {
+                  // dH_0 = (this step's masked gradient) + the earlier steps' dZ rows (L2 hits: prefetched by warp 3)
+                  const uint32_t aw = __ldg(reinterpret_cast<const unsigned int*>(p.add0 + grow * p.ld + n));
+                  const uint32_t bw = p.add1 != nullptr ? __ldg(reinterpret_cast<const unsigned int*>(p.add1 + grow * p.ld + n)) : 0u;
+                  z0 += bf_lo(aw) + bf_lo(bw);
+                  z1 += bf_hi(aw) + bf_hi(bw);
+                }
+                o = pack_bf2(z0, z1);
+              } else {
+                float z0 = v0 + bf_lo(hw);
+                float z1 = v1 + bf_hi(hw);
+                if constexpr (HAS_BIAS) {
+                  z0 += s_bias[n];
+                  z1 += s_bias[n + 1];
+                }
+                if constexpr (MODE == MODE_FWD && DROP) {
+                  // nn.Dropout of base.py:139 in the epilogue: tau in f32, keep bit, exact f32 scale 1 / (1 - p), one rounding
+                  const uint32_t kb = __ldg(p.drop_bits + grow * nj + (n >> 4));
+                  const int bit = n & 15;
+                  z0 = ((kb >> bit) & 1u) ? act_t<ACT>(p.act_param, z0) * p.drop_scale : 0.f;
+                  z1 = ((kb >> (bit + 1)) & 1u) ? act_t<ACT>(p.act_param, z1) * p.drop_scale : 0.f;
+                  o = pack_bf2(z0, z1);
+                } else if constexpr (ACT == DMPNN_ACT_RELU) {
+                  o = act_word<ACT>(pack_bf2(z0, z1), 0.f);  // max after rounding == rounding after max
+                } else {
+                  o = pack_bf2(act_t<ACT>(p.act_param, z0), act_t<ACT>(p.act_param, z1));
+                }
               }
-              o[qq] = pack_bf2(z0, z1);
-              continue;
             }
-            float z0 = __uint_as_float(v[2 * qq]) + bf_lo(hw[qq]);
-            float z1 = __uint_as_float(v[2 * qq + 1]) + bf_hi(hw[qq]);
-            if constexpr (HAS_BIAS) {
-              z0 += s_bias[j * 16 + 2 * qq];
-              z1 += s_bias[j * 16 + 2 * qq + 1];
-            }
-            if constexpr (MODE == MODE_FWD && DROP) {
-              {
-                // nn.Dropout of base.py:139 in the epilogue: tau in f32, keep bit, exact f32 scale 1 / (1 - p), one rounding
-                z0 = ((kb >> (2 * qq)) & 1u) ? act_t<ACT>(p.act_param, z0) * p.drop_scale : 0.f;
-                z1 = ((kb >> (2 * qq + 1)) & 1u) ? act_t<ACT>(p.act_param, z1) * p.drop_scale : 0.f;
-                o[qq] = pack_bf2(z0, z1);
-                continue;
-              }
-            }
-            if constexpr (ACT == DMPNN_ACT_RELU) o[qq] = act_word<ACT>(pack_bf2(z0, z1), 0.f);  // max after rounding == rounding after max
-            else o[qq] = pack_bf2(act_t<ACT>(p.act_param, z0), act_t<ACT>(p.act_param, z1));
-          }
-          if (rvalid && !(kExp && (p.exp_flags & 32768))) st_global_256(orow + j * 16, o);
-          // release accumulator chunk c once this group has read its last column block of it
-          const int jn = (jj + 1 < njj) ? j + 1 : 4 * (s + kEpiGroups);   // next block this group will read
-          if (jn >= nj || jn / 5 != c) {
-            tc_fence_before();
-            mbar_arrive(bar(B_ACCFREE + c));
+            if (!(kExp && (p.exp_flags & 32768))) *reinterpret_cast<uint32_t*>(orow + n) = o;
           }
         }
-        // this thread has read its H_0 row of the slab: the staging buffer may be refilled
-        if (!kH0Direct && MODE != MODE_BWD_COPY) mbar_arrive(bar(B_HFREE + q));
       }
-      if (et == 0) trace_ev(p, it, 8 + eg);
-      row0 = row0n;
-      nrows = nrowsn;
+      if (tt == 0) trace_ev(p, it, 8 + wg);
     }
-  } else {
-    // ===================== message (warps 12..19): thread == tile row == TMEM lane ==================
+  } else if (warp >= 12) {
+    // ===================== message (warps 12..19): thread == tile row ==================
     // A row e' of the GEMM is M[rev(e')] = sum of the OTHER in-edge states of e's destination atom
     // (mixins.py:11-18).  Each thread reads the <= 3 sibling rows of its row from the TMA-loaded,
     // 128B-swizzled shared-memory tile (read-only), adds them in packed bf16x2 (<= 2 roundings; f32 for
-    // in-degree > 4) and writes its bf16 row straight into tensor memory (tcgen05.st), where the MMA reads
-    // it as its A operand: the gathered operand never returns to shared memory.
-    const int sq = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int shalf = (warp - 12) >> 2;      // two warps per quadrant alternate over the 16-column blocks
+    // in-degree > 4) and writes its bf16 row into the A operand tile (K-major SWIZZLE_128B, the layout wgmma reads).
+    const int sq = warp & 3;                 // 32-row quarter of the tile
+    const int shalf = (warp - 12) >> 2;      // two warps per quarter alternate over the 16-column blocks
     const int r = sq * 32 + lane;            // tile row
     const int tS = threadIdx.x - 384;        // 0..255
-    const uint32_t at_base = tmem_base + kTmemAOff + ((uint32_t)(sq * 32) << 16);
     const int nj = p.hp >> 4;
     constexpr bool kCanEmit = FIRST || MODE != MODE_FWD;   // variants that may also write the gathered operand out
     constexpr bool kNeedRev = !ATOM;   // every bond mode gathers through the tile-local rev() table
@@ -673,16 +497,13 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
       const int npass = (p.nslab + kWHalfSlabs - 1) / kWHalfSlabs;
       int cur_pass = 0;                               // k pass being written; earlier ones are published by this thread
       if (!(p.exp_flags & 8192)) mbar_wait(bar(B_ATFREE + 0), (it & 1) ^ 1);    // tensor core is done with the first k pass of the previous tile
-      tc_fence_after();
       for (int j = shalf; j < nj; j += 2) {
         const int pj = (j >> 2) / kWHalfSlabs;
         if (pj != cur_pass) {                        // crossing into a later k pass: publish the finished ones, wait for the next
-          tmem_wait_st();
-          tc_fence_before();
+          fence_proxy_async();                       // A operand stores -> visible to wgmma (async proxy)
           for (int q = cur_pass; q < pj; ++q) mbar_arrive(bar(B_AREADY + q));
           cur_pass = pj;
           if (!(p.exp_flags & 8192)) mbar_wait(bar(B_ATFREE + pj), (it & 1) ^ 1);   // 8192: timing experiment, as if A were double-buffered
-          tc_fence_after();
         }
         if ((j >> 2) != cur_slab) {                   // entering a new 64-column slab of the H tile
           if (cur_slab >= 0) { mbar_arrive(bar(B_AFREE + cur_slab)); left &= ~(1u << cur_slab); }
@@ -690,7 +511,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
           mbar_wait(bar(B_AFULL + cur_slab), it & 1);
           if (tS == 0 && cur_slab == 0) trace_ev(p, it, 1);
         }
-        const uint32_t sbase = sA + (uint32_t)((j >> 2) % kASlots) * kSlabBytes;
+        const uint32_t sbase = sA + (uint32_t)(j >> 2) * kSlabBytes;
         const int c0 = 2 * (j & 3);
         uint32_t o[8];
         if (nsib <= (ATOM ? 4 : 3)) {
@@ -753,18 +574,21 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
 #pragma unroll
           for (int q = 0; q < 8; ++q) o[q] = pack_bf2(acc[2 * q], acc[2 * q + 1]);
         }
-        if (!(kExp && (p.exp_flags & 131072))) tmem_st8(at_base + (uint32_t)(j * 8), o);
+        if (!(kExp && (p.exp_flags & 131072))) {
+          const uint32_t ab = sAop + (uint32_t)(j >> 2) * kSlabBytes;
+          sts128(ab + sw128_off(r, c0), make_uint4(o[0], o[1], o[2], o[3]));
+          sts128(ab + sw128_off(r, c0 + 1), make_uint4(o[4], o[5], o[6], o[7]));
+        }
         if constexpr (kCanEmit) {
           // forward: A row r is M[r] (mixins.py:11-18); backward: A row r is ((S.P) dZ)[r].  One 32-byte
-          // sector per thread and block (STG.256), consumed by the W_h weight-gradient GEMM.
-          if (gout != nullptr) st_global_256(gout + j * 16, o);
+          // sector per thread and block, consumed by the W_h weight-gradient GEMM.
+          if (gout != nullptr) st_global_2x128(gout + j * 16, o);
         }
       }
       // release the slabs not released inside the loop (the last one visited, and any this thread owned no block of)
       for (int sl = 0; sl < p.nslab; ++sl)
         if (left & (1u << sl)) mbar_arrive(bar(B_AFREE + sl));
-      tmem_wait_st();
-      tc_fence_before();
+      fence_proxy_async();
       for (int q = cur_pass; q < npass; ++q) mbar_arrive(bar(B_AREADY + q));   // every thread arrives once per pass
       if (tS == 0) trace_ev(p, it, 2);
       // publish the next tile's rowptr slice (other buffer; readers of it finished a tile ago)
@@ -781,12 +605,6 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 

@@ -1,9 +1,10 @@
-// Blackwell (sm_100a) PTX wrappers shared by the tensor-core kernels: mbarrier, TMA (tensor + bulk),
-// tcgen05 (alloc / mma / commit / ld / st), UMMA descriptors, packed-bf16 helpers.
+// Hopper (sm_90a) PTX wrappers shared by the tensor-core kernels: mbarrier, TMA (tensor + bulk), wgmma
+// (fence / commit / wait, shared-memory operand descriptors), packed-bf16 helpers.
 #pragma once
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma_ops.cuh"
 
 namespace dmpnn {
 namespace tc {
@@ -45,7 +46,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
   }
 }
-// one lane of a CONVERGED warp; keeps the warp on the uniform datapath (UTCHMMA / UTMALDG operands live
+// one lane of a CONVERGED warp; keeps the warp on the uniform datapath (UTMALDG operands live
 // in uniform registers -- issuing them from a divergent `lane == 0` branch makes ptxas emit a
 // per-lane emulation loop around every instruction)
 __device__ __forceinline__ bool elect_one() {
@@ -59,8 +60,6 @@ __device__ __forceinline__ bool elect_one() {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tmap, uint32_t bar, int c0, int c1) {
   asm volatile(
@@ -80,67 +79,47 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
                "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- warpgroup MMA (wgmma) ----------------------------------------------------------------------
+// wgmma_fence orders the warpgroup's register / shared-memory accesses before the MMAs that follow; commit closes a group
+// of issued MMAs, wait<N> blocks until at most N groups are still in flight (their accumulators are then readable).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an asynchronous MMA
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// K-major, SWIZZLE_128B operand descriptor (rows of 128 B, 8-row groups 1024 B apart)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
+// K-major, SWIZZLE_128B operand descriptor (rows of 128 B, 8-row groups 1024 B apart); advancing the start address by
+// 32 B steps one k16 (bf16) / k8 (tf32) slice along the row
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
   uint64_t d = (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;             // leading byte offset (unused for swizzled K-major) = 16 B
   d |= (uint64_t)(1024 >> 4) << 32;   // stride byte offset: 8 rows x 128 B
-  d |= (uint64_t)1 << 46;             // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;             // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;             // SWIZZLE_128B
   return d;
 }
-__device__ __forceinline__ uint32_t umma_idesc_bf16(int M, int N) {
-  // c=F32 (1<<4), a=BF16 (1<<7), b=BF16 (1<<10), K-major A and B, N>>3 at [17,23), M>>4 at [24,29)
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// MN-major SWIZZLE_128B operand (bf16): rows of the contraction index at 128 B pitch (64 MN elements), 8-row groups
+// 1024 B apart (SBO), 64-element MN blocks `lbo` bytes apart (LBO)
+__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t saddr, uint32_t lbo) {
+  uint64_t d = (uint64_t)((saddr & 0x3FFFF) >> 4);
+  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
 }
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
+// 16-byte global store of 8 bf16 (two per 32-byte sector of a 16-column block)
+__device__ __forceinline__ void st_global_2x128(void* ptr, const uint32_t (&v)[8]) {
+  uint4* q = reinterpret_cast<uint4*>(ptr);
+  q[0] = make_uint4(v[0], v[1], v[2], v[3]);
+  q[1] = make_uint4(v[4], v[5], v[6], v[7]);
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-// one 32-byte sector per thread (STG.256, sm_100+); address must be 32-byte aligned
-__device__ __forceinline__ void st_global_256(void* ptr, const uint32_t (&v)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(v[0]), "r"(v[1]), "r"(v[2]),
-               "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-               "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// A operand from TMEM (lane = row, 2 bf16 per 32-bit column), B from shared memory
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// Accumulator fragment of the calling thread inside its warpgroup (see wgmma_ops.cuh): rows acc_row0 and acc_row0 + 8,
+// columns 8 * b + acc_col0 + {0, 1} of every 8-column block b
+__device__ __forceinline__ int acc_row0(int t) { return ((t >> 5) << 4) + ((t & 31) >> 2); }
+__device__ __forceinline__ int acc_col0(int t) { return (t & 3) << 1; }
 
 __device__ __forceinline__ uint4 lds128(uint32_t a) {
   uint4 v;

@@ -3,16 +3,17 @@
 //
 // The contraction runs over ROWS, so both operands are used "MN-major": a TMA box of 64 rows x 64
 // columns (SWIZZLE_128B) of the row-major dY / X matrices is exactly the canonical MN-major SW128 atom
-// stack (row r = K index at 128-byte pitch, 64 contiguous columns = MN index), no transposes needed.
+// stack (row r = K index at 128-byte pitch, 64 contiguous columns = MN index); the tensor core transposes them.
 //
-//   CTA (mt, slot): output rows n in [128*mt, 128*mt+128), all k; loops over 64-row blocks slot, slot+S, ...
-//     warp 0  TMA producer: 2 dY boxes + ceil(Kpad/64) X boxes per 64-row stage, 3-stage ring
-//     warp 1  tcgen05.mma issuer: D[128 x Kpad] (TMEM, fp32) += dY_blk^T . X_blk   (a_major = b_major = MN)
-//     warp 2  TMEM allocator
-//     warps 4-7  after the last block: TMEM -> f32 partial[cta][128][Kpad] in global memory
+//   CTA (mt, kt, slot): output rows n in [128*mt, 128*mt+128), columns k in [192*kt, 192*kt+192); loops over 64-row
+//   blocks slot, slot+S, ...
+//     warp 0      TMA producer: 2 dY boxes per term + up to 3 X boxes per 64-row stage, 3-stage ring
+//     warps 4-11  two consumer warpgroups (output rows [0, 64) / [64, 128) of the tile): wgmma m64n64k16 with
+//                 transposed operands, D[64 x 192] (registers, fp32) += dY_blk^T . X_blk; after the last block the
+//                 accumulator is written as f32 partial[cta][128][Kpad] to global memory
 //   a second kernel adds the partials of each mt in fixed order (deterministic) into dW.
 // Up to three dY TERMS may share one launch (dW = sum_t dY_t^T X): the X boxes of a stage are loaded once and every term
-// accumulates into the same TMEM tile -- the W_i gradient of the bf16 mirror, whose dH_0 is a sum of per-step terms that
+// accumulates into the same registers -- the W_i gradient of the bf16 mirror, whose dH_0 is a sum of per-step terms that
 // is never formed (engine.bond_backward_tc), reads X_0 once instead of once per term.
 #include <cuda.h>
 #include <stdlib.h>
@@ -27,38 +28,25 @@ using namespace dmpnn::tc;
 
 constexpr int kRowsPerStage = 64;
 constexpr int kBoxBytes = kRowsPerStage * 128;    // 64 rows x 64 bf16 = 8 KB
-constexpr int kMaxXBoxes = 7;                     // K <= 448 (TMEM: 448 of 512 accumulator columns)
-constexpr int kStageBytes = (2 + kMaxXBoxes) * kBoxBytes;   // 72 KB
+constexpr int kMaxXBoxes = 7;                     // K <= 448
+constexpr int kKT = 192;                          // output columns per CTA
+constexpr int kXBoxesPerTile = kKT / 64;
+constexpr int kStageBytes = (2 * 3 + kXBoxesPerTile) * kBoxBytes;   // 72 KB (three terms)
 constexpr int kStages = 3;
-constexpr int kThreads = 256;
-constexpr int kTmemCols = 512;
-constexpr int kOffBar = kStages * kStageBytes;    // 196608
-constexpr int kOffTmem = kOffBar + 8 * 8;
-constexpr int kSmemBytes = kOffTmem + 16;
+constexpr int kThreads = 384;
+constexpr int kConsumers = 256;
+constexpr int kOffBar = kStages * kStageBytes;    // 221184
+constexpr int kSmemBytes = kOffBar + 8 * 8;
 constexpr int kSmemAlloc = kSmemBytes + 1024;
 static_assert(kSmemAlloc <= 232448, "exceeds shared memory");
 
-enum { B_FULL = 0, B_EMPTY = 3, B_ACCFULL = 6 };
+enum { B_FULL = 0, B_EMPTY = 3 };
 
 struct Params {
   float* partial;       // [gridDim.x][128][Kpad]
   int64_t R;
   int N, Kx, Kpad, nxb, n_mt, slots, n_blocks, n_terms;
 };
-
-// MN-major SWIZZLE_128B operand: rows (K index) at 128 B pitch, 8-row groups 1024 B apart (SBO),
-// 64-column MN blocks `lbo` bytes apart (LBO)
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t saddr, uint32_t lbo) {
-  uint64_t d = (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ uint32_t umma_idesc_bf16_mn(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 
 __global__ void __launch_bounds__(kThreads, 1)
 k_wgrad_tc(const __grid_constant__ CUtensorMap tmapY, const __grid_constant__ CUtensorMap tmapY1,
@@ -67,26 +55,23 @@ k_wgrad_tc(const __grid_constant__ CUtensorMap tmapY, const __grid_constant__ CU
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t sbase = smem_u32(smem);
   const uint32_t sBar = sbase + kOffBar;
-  volatile uint32_t* s_tmem = reinterpret_cast<volatile uint32_t*>(smem + kOffTmem);
   const int warp = threadIdx.x >> 5;
   auto bar = [&](int i) { return sBar + 8u * (uint32_t)i; };
   const int mt = blockIdx.x % p.n_mt, slot = blockIdx.x / p.n_mt;
+  const int kt = blockIdx.y;
+  const int kw = min(kKT, p.Kpad - kt * kKT);        // accumulator columns of this CTA (multiple of 16)
+  const int nxb = (kw + 63) / 64;                    // X boxes per stage
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(bar(B_FULL + i), 1);
-      mbar_init(bar(B_EMPTY + i), 1);
+      mbar_init(bar(B_EMPTY + i), kConsumers);
     }
-    mbar_init(bar(B_ACCFULL), 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(s_tmem)), kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
   const int nt = p.n_terms;
-  const uint32_t stage_tx = (uint32_t)(2 * nt + p.nxb) * kBoxBytes;
+  const uint32_t stage_tx = (uint32_t)(2 * nt + nxb) * kBoxBytes;
   const uint32_t x_off = (uint32_t)(2 * nt) * kBoxBytes;      // a stage = [2 boxes per term | X boxes]
 
   if (warp == 0) {
@@ -102,67 +87,52 @@ k_wgrad_tc(const __grid_constant__ CUtensorMap tmapY, const __grid_constant__ CU
           tma_load_2d(base + (2 * t) * kBoxBytes, my, bar(B_FULL + st), mt * 128, blk * kRowsPerStage);
           tma_load_2d(base + (2 * t + 1) * kBoxBytes, my, bar(B_FULL + st), mt * 128 + 64, blk * kRowsPerStage);
         }
-        for (int xb = 0; xb < p.nxb; ++xb)
-          tma_load_2d(base + x_off + xb * kBoxBytes, &tmapX, bar(B_FULL + st), xb * 64, blk * kRowsPerStage);
+        for (int xb = 0; xb < nxb; ++xb)
+          tma_load_2d(base + x_off + xb * kBoxBytes, &tmapX, bar(B_FULL + st), kt * kKT + xb * 64, blk * kRowsPerStage);
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    const int n0 = p.Kpad <= 256 ? p.Kpad : 256;
-    const int n1 = p.Kpad - n0;
-    const uint32_t idesc0 = umma_idesc_bf16_mn(128, n0);
-    const uint32_t idesc1 = umma_idesc_bf16_mn(128, n1 > 0 ? n1 : 16);
+  } else if (warp >= 4) {
+    const int wg = (warp - 4) >> 2;
+    const int tt = threadIdx.x - 128 - wg * 128;
+    float acc[kXBoxesPerTile][32];
+#pragma unroll
+    for (int b = 0; b < kXBoxesPerTile; ++b)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[b][i] = 0.f;
     uint32_t ks = 0;
-    bool any = false;
     for (int blk = slot; blk < p.n_blocks; blk += p.slots, ++ks) {
       const uint32_t st = ks % kStages, use = ks / kStages;
       mbar_wait(bar(B_FULL + st), use & 1);
-      tc_fence_after();
       const uint32_t base = sbase + st * kStageBytes;
-      if (elect_one()) {
-        for (int t = 0; t < nt; ++t)
-          for (int kk = 0; kk < kRowsPerStage / 16; ++kk) {
-            const uint32_t acc = (ks > 0 || kk > 0 || t > 0) ? 1u : 0u;
-            const uint64_t adesc = umma_desc_mn_sw128(base + (2 * t) * kBoxBytes + kk * 2048, kBoxBytes);
-            umma_bf16(tmem_base, adesc, umma_desc_mn_sw128(base + x_off + kk * 2048, kBoxBytes), idesc0, acc);
-            if (n1 > 0)
-              umma_bf16(tmem_base + 256u, adesc, umma_desc_mn_sw128(base + x_off + 4 * kBoxBytes + kk * 2048, kBoxBytes), idesc1, acc);
-          }
-        umma_commit(bar(B_EMPTY + st));
-      }
-      __syncwarp();
-      any = true;
-    }
-    if (elect_one()) umma_commit(bar(B_ACCFULL));
-    __syncwarp();
-    (void)any;
-  } else if (warp >= 4) {
-    // final drain: thread == output row n (TMEM lane), 16 k-columns per tcgen05.ld
-    const int r = (warp & 3) * 32 + (threadIdx.x & 31);
-    const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-    float* out = p.partial + ((size_t)blockIdx.x * 128 + r) * p.Kpad;
-    const bool have = slot < p.n_blocks;   // did this CTA accumulate anything?
-    mbar_wait(bar(B_ACCFULL), 0);
-    tc_fence_after();
-    for (int j = 0; j < p.Kpad / 16; ++j) {
-      uint32_t v[16];
-      if (have) {
-        tmem_ld16(taddr + j * 16, v);
-        tmem_wait_ld();
-      } else {
+      wgmma_fence();
+      for (int t = 0; t < nt; ++t)
 #pragma unroll
-        for (int q = 0; q < 16; ++q) v[q] = 0u;
-      }
+        for (int kk = 0; kk < kRowsPerStage / 16; ++kk) {
+          const uint64_t adesc = desc_mn_sw128(base + (2 * t + wg) * kBoxBytes + kk * 2048, kBoxBytes);
 #pragma unroll
-      for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<uint4*>(out + j * 16 + q * 4) = make_uint4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+          for (int b = 0; b < kXBoxesPerTile; ++b)
+            if (b < nxb) wgmma_bf16_n64_mn(acc[b], adesc, desc_mn_sw128(base + x_off + b * kBoxBytes + kk * 2048, kBoxBytes), 1u);
+        }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int b = 0; b < kXBoxesPerTile; ++b) acc_fence(acc[b]);
+      mbar_arrive(bar(B_EMPTY + st));
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+    // drain: rows 64 wg + acc_row0 (+8), columns 64 b + 8 j + acc_col0 (+1); zeros when this CTA had no block
+    const int rl = wg * 64 + acc_row0(tt), cl = acc_col0(tt);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float* out = p.partial + ((size_t)blockIdx.x * 128 + rl + 8 * h) * p.Kpad + kt * kKT;
+#pragma unroll
+      for (int b = 0; b < kXBoxesPerTile; ++b)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int c = 64 * b + 8 * j + cl;
+          if (c < kw) *reinterpret_cast<float2*>(out + c) = make_float2(acc[b][4 * j + 2 * h], acc[b][4 * j + 2 * h + 1]);
+        }
+    }
   }
 }
 
@@ -222,7 +192,7 @@ static bool encode_map(EncodeTiledFn enc, CUtensorMap* tmap, const void* base, i
 }
 
 struct Geom {
-  int Kpad, nxb, n_mt, slots, grid;
+  int Kpad, nxb, n_mt, n_kt, slots, grid;
 };
 static Geom geom(int64_t N, int64_t Kx) {
   static int sm_count = 0;
@@ -230,13 +200,14 @@ static Geom geom(int64_t N, int64_t Kx) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
-    if (sm_count <= 0) sm_count = 148;
+    if (sm_count <= 0) sm_count = 132;
   }
   Geom g;
   g.Kpad = (int)((Kx + 15) / 16 * 16);
   g.nxb = (g.Kpad + 63) / 64;
   g.n_mt = (int)((N + 127) / 128);
-  g.slots = sm_count / g.n_mt;
+  g.n_kt = (g.Kpad + kKT - 1) / kKT;
+  g.slots = sm_count / (g.n_mt * g.n_kt);
   if (g.slots < 1) g.slots = 1;
   g.grid = g.slots * g.n_mt;
   return g;
@@ -293,7 +264,7 @@ extern "C" int dmpnn_wgrad_tc_multi_bf16(const void* const* dYs, int n_terms, in
       DMPNN_CHECK_ARG(e == cudaSuccess, "wgrad_tc: cannot configure %d B dynamic smem: %s", kSmemAlloc, cudaGetErrorString(e));
       attr_set = true;
     }
-    k_wgrad_tc<<<g.grid, kThreads, kSmemAlloc, st>>>(mY[0], mY[1], mY[2], mX, p);
+    k_wgrad_tc<<<dim3((unsigned)g.grid, (unsigned)g.n_kt), kThreads, kSmemAlloc, st>>>(mY[0], mY[1], mY[2], mX, p);
   } else {
     cudaMemsetAsync(workspace, 0, (size_t)g.grid * 128 * g.Kpad * sizeof(float), st);
   }

@@ -2,7 +2,7 @@
 allocated inside the library) and the autograd functions the nn modules call.
 
 PyTorch here is plumbing only: it owns device memory (caching allocator), streams and the
-autograd graph; every arithmetic step on the path is a kernel of libdmpnn_sm100.so.
+autograd graph; every arithmetic step on the path is a kernel of libdmpnn_sm90.so.
 """
 from __future__ import annotations
 
@@ -83,7 +83,7 @@ def _require_cuda(*ts: Tensor):
     for t in ts:
         if t is not None and not t.is_cuda:
             raise DmpnnError(
-                "chemprop_b200 runs on CUDA (sm_100a) only; got a CPU tensor. There is no CPU fallback: "
+                "chemprop_b200 runs on CUDA (sm_90a) only; got a CPU tensor. There is no CPU fallback: "
                 "move the BatchMolGraph and the module to the GPU."
             )
 
@@ -386,7 +386,7 @@ class MPConfig:
     act_param: float
     undirected: bool
     hidden_dtype: torch.dtype  # torch.float32 (<=1e-5 tier) or torch.bfloat16 (<=1e-2 tier)
-    fused: bool = True         # use the tcgen05 fused depth-step kernel when applicable
+    fused: bool = True         # use the fused wgmma depth-step kernel when applicable
     dropout_p: float = 0.0     # > 0: training-mode dropout on the fused bf16 / ReLU path (dropout_fused_ok)
     mask_fn: object = None     # keep-mask source `f(like) -> {0,1} tensor like `like``; None = torch's bernoulli_
 
@@ -399,7 +399,7 @@ UNDIRECTED_FUSED = os.environ.get("DMPNN_UNDIRECTED_FUSED", "1") != "0"   # DMPN
 
 
 def _fused_step_ok(cfg: MPConfig, lay: Layout, h: int) -> bool:
-    """The fused tcgen05 depth step applies: bf16 tier, h <= 304.  Molecules of any size: those with more than 128 directed
+    """The fused wgmma depth step applies: bf16 tier, h <= 304.  Molecules of any size: those with more than 128 directed
     edges run as 128-row windows of the same kernel (Layout.step_tables).  `undirected=True` (base.py:202-203) runs on it too:
     the reverse-edge average is a prologue pass that produces the step's input (bond_forward)."""
     ok = (cfg.fused and cfg.hidden_dtype == torch.bfloat16 and h <= 304 and lay.E > 0 and (not cfg.undirected or (UNDIRECTED_FUSED and h % 4 == 0))
@@ -1074,7 +1074,7 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
 def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
                      saved: dict, gHv: Tensor, need_bias: tuple[bool, bool, bool]):
     """bf16-tier autograd mirror on the tensor-core kernels (directed bonds).  Differences from the generic
-    mirror: every GEMM is tcgen05; tau' is fused into the backward message kernel; dH_0 is never kept as an f32
+    mirror: every GEMM is on the tensor cores (wgmma); tau' is fused into the backward message kernel; dH_0 is never kept as an f32
     read-modify-write accumulator -- the per-step dZ^t stay in bf16 and are summed once, in f32, at the end."""
     dev = V.device
     h = Wh.shape[0]
@@ -1134,7 +1134,7 @@ def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
     if cfg.depth == 1:
         act_bwd(dMv, H0, nE, hc, act=a, act_param=ap, gidx=lay.dst_row, from_preact=True, dZ=dH0b)
     else:
-        fused_bwd = _fused_step_ok(cfg, lay, h)      # the depth step's mirror on the same fused tcgen05 kernel
+        fused_bwd = _fused_step_ok(cfg, lay, h)      # the depth step's mirror on the same fused wgmma kernel
         if s_drop != 1.0 and not fused_bwd:
             raise DmpnnError("dropout on the monolithic tier needs the fused depth step (see dropout_fused_ok)")
         WhT_pk = None if fused_bwd else pack_weight_tc(Wh, transpose=True)
@@ -1410,7 +1410,7 @@ def atom_forward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tenso
 
 def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
                      saved: dict, gHv: Tensor, need_bias):
-    """Autograd mirror of atom_forward_tc (tcgen05 GEMMs; dH_0 is kept as separate terms, one W_i GEMM each)."""
+    """Autograd mirror of atom_forward_tc (wgmma GEMMs; dH_0 is kept as separate terms, one W_i GEMM each)."""
     dev = V.device
     h = Wi.shape[0]
     hp = pad_hidden(h)

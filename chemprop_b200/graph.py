@@ -2,7 +2,7 @@
 optionally the optimizer -- captured ONCE for a batch signature and replayed with one `cudaGraphLaunch` per step.
 
 Why it is possible: the step is sync-free (layout meta words come from the host, `engine.HOST_META`), every kernel of
-libdmpnn_sm100.so launches on the caller's current stream with plain pointer arguments, the TMA descriptors are passed by value
+libdmpnn_sm90.so launches on the caller's current stream with plain pointer arguments, the TMA descriptors are passed by value
 (`__grid_constant__`), and the library never allocates.  Why it pays: a 10 k-molecule fwd+bwd is ~60 launches of 5-250 us each;
 the host needs ~1 ms of Python + ctypes to issue them, a graph launch needs ~20 us, so the GPU queue never runs dry and the
 host is free for the loader.  (The reference reaches the same point only through `torch.compile(mode="reduce-overhead")`.)

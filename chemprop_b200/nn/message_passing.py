@@ -1,6 +1,6 @@
 """`BondMessagePassing` / `AtomMessagePassing` with the module API of
 chemprop/nn/message_passing/base.py:16-289 (same constructor arguments, `hparams`, parameter names
-W_i / W_h / W_o / W_d, `output_dim`, `forward(bmg, V_d=None)`), executed by the sm_100a engine.
+W_i / W_h / W_o / W_d, `output_dim`, `forward(bmg, V_d=None)`), executed by the sm_90a engine.
 
 Differences a user can see: the module must live on a CUDA device (there is no CPU fallback), and a
 `precision` keyword selects the hidden-state storage type: "fp32" (default; matches the reference
@@ -58,7 +58,7 @@ def engine_activation(tau: nn.Module) -> tuple[int, float]:
     if type(tau) is nn.Identity:
         return _lib.ACT_NONE, 0.0
     raise NotImplementedError(
-        f"activation {type(tau).__name__} is not fused into the sm_100a kernels "
+        f"activation {type(tau).__name__} is not fused into the sm_90a kernels "
         "(fused: ReLU, LeakyReLU, Tanh, ELU; anything else runs on the composed tier)"
     )
 

@@ -1,5 +1,5 @@
 /*
- * dmpnn.h -- C ABI of libdmpnn_sm100.so, the B200 (sm_100a) D-MPNN message-passing engine.
+ * dmpnn.h -- C ABI of libdmpnn_sm90.so, the H100 (sm_90a) D-MPNN message-passing engine.
  *
  * The reference (chemprop v2.3.1) has no FFI on this path: the hot path is ~150 lines of
  * Python dispatching stock ATen ops.  This header is therefore the boundary a maintainer
@@ -66,7 +66,7 @@ enum {
 
 int dmpnn_version(void);
 const char* dmpnn_last_error(void);
-/* 1 if a CUDA device of compute capability 10.x is current, else 0 (never throws). */
+/* 1 if a CUDA device of compute capability 9.0 (H100) is current, else 0 (never throws). */
 int dmpnn_device_ok(void);
 /* Number of kernels this library has launched in this process (bench.py's `gpu_launches`). */
 long long dmpnn_launch_count(void);
@@ -278,7 +278,7 @@ int dmpnn_act_bwd(const void* G, int g_dtype, int64_t ldg, const int32_t* gidx,
                   int64_t R, int64_t C, void* stream);
 
 /* ---------------------------------------------------------------------------------------
- * Fused Blackwell depth step (bf16 hidden states, tcgen05 + TMEM + TMA):
+ * Fused Hopper depth step (bf16 hidden states, wgmma + TMA + mbarrier):
  *   H_next[rev(e')] = tau( H_0[rev(e')] + bias + W_h . ( sum_{in(v)} g(H_prev) - g(H_prev[e']) ) )
  * i.e. message (mixins.py:11-18) + update (base.py:135-141) in ONE launch, one CTA per SM,
  * molecule-aligned 128-row tiles from dmpnn_layout_build.  g = tau when first_step!=0
@@ -289,7 +289,7 @@ int dmpnn_act_bwd(const void* G, int g_dtype, int64_t ldg, const int32_t* gidx,
  * M^1[e] (mixins.py:11-18) that the step consumed, saved for the W_h gradient instead of being recomputed.
  * ------------------------------------------------------------------------------------- */
 /* ---------------------------------------------------------------------------------------
- * Tensor-core linear layers of the bf16 tier (tcgen05 / TMEM / TMA), for the GEMMs outside the fused
+ * Tensor-core linear layers of the bf16 tier (wgmma / TMA), for the GEMMs outside the fused
  * depth step: W_i (mixins.py:8-9, 22-23), W_o (base.py:180-182) and dX = dY.W of their autograd mirror.
  *   dmpnn_concat_bf16     A[r] = bf16([X1[i1(r)] || X2[i2(r)] || 0..])  (torch.cat of mixins.py:9 / base.py:180)
  *   dmpnn_pack_weight_tc  nn.Linear weight (or its transpose: transpose != 0 packs B[n][k] = W[k][n]) ->
@@ -339,7 +339,7 @@ int dmpnn_tiles_build(const int32_t* mol_atom_ptr, const int32_t* mol_row_ptr, i
 /* Atom-granular fused depth step -- AtomMessagePassing (chemprop/nn/message_passing/mixins.py:25-30 + base.py:135-141)
  * restated on atoms (the reference's edge state H[e] depends only on src(e)):
  *   H_next[v] = act( H_0[v] + bias + W . sum_{e in in(v)} g(H_prev[src(e)]) ),   g = act on the first step, identity after,
- * one launch: neighbour gather from the TMA-loaded atom tile + tcgen05 GEMM + epilogue, the kernel of
+ * one launch: neighbour gather from the TMA-loaded atom tile + wgmma GEMM + epilogue, the kernel of
  * dmpnn_bond_step_fused_bf16 with its ATOM gather.  The loop-invariant bond term W_h[:, h:] . sum_in E of the reference's
  * update is folded into H_0 by the caller (engine.atom_forward_fused).  rowptr: dst-sorted CSR over atoms; nbr_row: source
  * atom of every edge row; tile_atom_ptr / tile_edge_ptr: first atom / first edge row of every atom tile (dmpnn_tiles_build
@@ -404,7 +404,7 @@ int dmpnn_work_table_build(const int32_t* tile_row_ptr, const int32_t* tile_atom
 
 /* ---------------------------------------------------------------------------------------
  * fp32-ACCURATE tensor-core GEMMs of the fp32 tier (csrc/gemm_x3.cu): every product is three
- * tcgen05.mma.kind::tf32 passes over an error-free hi / lo split of both operands, f32 accumulation in TMEM --
+ * tf32 wgmma passes over an error-free hi / lo split of both operands, f32 accumulation in registers --
  * the accuracy of an f32 FMA chain (the reference's ATen sgemm on base.py:135-141, 180-182) at tensor-core
  * speed; hidden size up to 4096 (BASELINE config 3: h = 600, depth 6).
  *   dmpnn_pack_weight_x3  nn.Linear weight W (N x K f32, row stride ldw; transpose != 0: B[n][k] = W[k][n]) ->

@@ -362,12 +362,69 @@ def mpnn_head_case() -> dict:
     return d
 
 
+# the configurations tests/test_oracle.py::test_restatement_matches_live_reference compares the restatement with
+LIVE_CASES = [("bond", 3, False, False, "relu"), ("bond", 4, True, True, "elu"), ("atom", 3, True, False, "leakyrelu"),
+              ("atom", 2, False, False, "tanh"), ("bond", 1, False, False, "relu")]
+
+
+def live_reference_case(kind: str, depth: int, bias: bool, undirected: bool, act: str) -> dict:
+    """The reference's module on 40 seeded synthetic molecules (d_h = 96, torch.manual_seed(7) before construction), kept
+    small: a checksum of its initial weights, SHA-256 digests of its collate of the batch, its whole mean aggregate, and seeded
+    samples of its hidden states (128 rows) and of the weight gradients of sum(agg^2) (128 entries each)."""
+    import hashlib
+
+    import_reference()
+    from chemprop.data import BatchMolGraph
+    from chemprop.data.molgraph import MolGraph
+    from chemprop.nn import AtomMessagePassing, BondMessagePassing, MeanAggregation
+
+    from chemprop_b200.data.synthetic import make_molecules
+
+    torch.set_num_threads(1)
+    torch.manual_seed(7)
+    mgs = make_molecules(40, seed=11, shuffle_edges=True)
+    bmg = BatchMolGraph([MolGraph(*m) for m in mgs])
+    cls = BondMessagePassing if kind == "bond" else AtomMessagePassing
+    mp = cls(d_h=96, depth=depth, bias=bias, undirected=undirected, activation=act)
+    out = {"wsum." + k: np.array([v.double().sum().item(), v.double().abs().sum().item()]) for k, v in mp.state_dict().items()}
+    for k in ("V", "E", "edge_index", "rev_edge_index", "batch"):
+        x = getattr(bmg, k).numpy()
+        out["sha256." + k] = np.frombuffer(hashlib.sha256(np.ascontiguousarray(x).tobytes()).digest(), dtype=np.uint8)
+        out["dtype." + k] = np.array(str(x.dtype))
+    H = mp(bmg)
+    a = MeanAggregation()(H, bmg.batch)
+    a.square().sum().backward()
+    rng = np.random.default_rng(3)
+    rows = np.sort(rng.choice(H.shape[0], 128, replace=False)).astype(np.int32)
+    out.update({"H_rows": rows, "H_sample": H.detach().numpy()[rows], "agg_mean": a.detach().numpy()})
+    for k, p in mp.named_parameters():
+        if p.grad is not None:
+            idx = np.sort(rng.choice(p.grad.numel(), min(p.grad.numel(), 128), replace=False)).astype(np.int32)
+            out["gidx." + k] = idx
+            out["grad." + k] = p.grad.numpy().reshape(-1)[idx]
+    return out
+
+
+def seeded_sampler_case() -> dict:
+    """Two epochs of the reference's SeededSampler(203, seed 99) (tests/test_loader.py)."""
+    import_reference()
+    from chemprop.data.samplers import SeededSampler
+
+    ref = SeededSampler(203, 99)
+    return {"order": np.stack([np.fromiter(iter(ref), dtype=np.int64) for _ in range(2)]).astype(np.int16)}
+
+
 def main():
     """`python -m oracle.make_golden [name ...]`: all cases, or only the named ones (a case's seed is its position in
     CASES, so adding cases at the end never changes the committed ones)."""
     os.makedirs(GOLDEN_DIR, exist_ok=True)
     torch.set_num_threads(1)  # deterministic summation order
     only = set(sys.argv[1:])
+    if "live" in only:
+        for i, c in enumerate(LIVE_CASES):
+            np.savez_compressed(os.path.join(GOLDEN_DIR, f"fixture_live_{i}.npz"), **live_reference_case(*c))
+        np.savez_compressed(os.path.join(GOLDEN_DIR, "fixture_seeded_sampler.npz"), **seeded_sampler_case())
+        return
     if "fixture_attentive" in only or not only:
         np.savez_compressed(os.path.join(GOLDEN_DIR, "fixture_attentive.npz"), **attentive_case())
         print("fixture_attentive")

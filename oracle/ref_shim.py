@@ -130,6 +130,16 @@ def import_reference():
         ]:
             if n not in sys.modules:
                 _stub(n)
+        # scaling (sklearn) and uncertainty calibration (scipy, sklearn) are imported by the package but are off the path:
+        # stand-ins only where the real package is not installed
+        import importlib
+
+        for n in ["scipy", "scipy.optimize", "scipy.special", "sklearn", "sklearn.preprocessing", "sklearn.isotonic"]:
+            if n not in sys.modules:
+                try:
+                    importlib.import_module(n)
+                except ImportError:
+                    _stub(n)
         sys.modules["rdkit.Chem.rdchem"].HybridizationType = _Names()
         sys.modules["rdkit.Chem.rdchem"].BondType = _Names()
         for n in ["torchmetrics", "torchmetrics.classification"]:

@@ -1,7 +1,7 @@
 // Hardware check of the two kernels added after the round's GPU budget was spent, WITHOUT Python (starts in ~1 s):
 //   dmpnn_dataset_gather  vs  dmpnn_dataset_gather_host  (bit-exact, all five BatchMolGraph arrays)
 //   dmpnn_scale_mask      vs  a host computation          (f32 and bf16, in place)
-// Build (cross-compiles without a GPU):  see tests/native/Makefile.   Run on the B200 box:  ./tests/native/check_new_kernels
+// Build (cross-compiles without a GPU):  see tests/native/Makefile.   Run on an H100:  ./tests/native/check_new_kernels
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -135,7 +135,7 @@ static int check_scale_mask() {
 }
 
 int main() {
-  if (dmpnn_device_ok() != 1) { printf("no sm_100 device\n"); return 3; }
+  if (dmpnn_device_ok() != 1) { printf("no H100 (sm_90) device\n"); return 3; }
   int rc = 0;
   rc |= check_gather(72, 14);
   rc |= check_gather(106, 28);

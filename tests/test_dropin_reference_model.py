@@ -13,7 +13,7 @@ import torch
 from oracle.ref_shim import reference_available
 from tests import emu
 
-pytestmark = pytest.mark.skipif(not reference_available(), reason="reference tree not reachable (GPU box)")
+pytestmark = pytest.mark.skipif(not reference_available(), reason="needs the unmodified reference package (CHEMPROP_REFERENCE_ROOT)")
 
 
 @pytest.mark.parametrize("kind,agg,act,undirected", [("bond", "mean", "relu", False), ("atom", "sum", "tanh", False),

@@ -1,4 +1,4 @@
-"""GPU tier: the tcgen05 linear kernel (dmpnn_linear_tc_bf16) and its helpers against a plain PyTorch
+"""GPU tier: the wgmma linear kernel (dmpnn_linear_tc_bf16) and its helpers against a plain PyTorch
 fp32 reference of the same op (bf16 operands, fp32 accumulate)."""
 import pytest
 import torch

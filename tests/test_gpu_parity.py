@@ -1,4 +1,4 @@
-"""GPU tier (B200): the CUDA path (through the C ABI) against the golden vectors of the real
+"""GPU tier: the CUDA path (through the C ABI) against the golden vectors of the real
 reference and against oracle/restatement.py on seeded inputs.
 Tolerances (BASELINE.json north_star): indices bit-exact; hidden states <= 1e-5 in the fp32 tier,
 <= 1e-2 in the bf16 tier."""

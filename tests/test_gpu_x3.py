@@ -1,4 +1,4 @@
-"""GPU tier, kernel level: the fp32-accurate tensor-core GEMMs (csrc/gemm_x3.cu, 3 x tcgen05.mma.kind::tf32 on an
+"""GPU tier, kernel level: the fp32-accurate tensor-core GEMMs (csrc/gemm_x3.cu, 3 x tf32 wgmma on an
 error-free hi / lo split) against an f64 reference.  Bound: a few 2^-22 of sum_k |a_k w_k| per output -- the accuracy class
 of an f32 FMA chain (what the reference's ATen sgemm delivers on base.py:135-141), NOT tf32's 2^-11."""
 import pytest

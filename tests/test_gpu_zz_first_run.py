@@ -1,4 +1,4 @@
-"""GPU tier (B200): tests of code that has not yet run on hardware.
+"""GPU tier: the composed tier and the host-side orchestration around the verified kernels.
 
   * the composed tier (chemprop_b200/composed.py) -- PReLU / SELU / user activation modules, dropout > 0 in training,
     AtomMessagePassing(undirected=True) -- through the real kernels, against the golden vectors of the real reference
@@ -10,9 +10,9 @@
   * the mol-atom-bond variants (MABBond / MABAtomMessagePassing), which run on the composed tier, AttentiveAggregation and
     ConstrainerFFN (segment primitives + torch elementwise ops).
 
-(The two NEW kernels these tests reach -- dmpnn_dataset_gather, dmpnn_scale_mask -- did run on a B200 in that round, through
-tests/native/check_new_kernels: bit-exact, profiles/r1_native_check_new_kernels.log.  Everything else here is host-side
-orchestration over kernels the verified tiers already exercise.)
+(The two kernels these tests reach beyond the verified tiers -- dmpnn_dataset_gather, dmpnn_scale_mask -- also have a
+Python-free check in tests/native/check_new_kernels.  Everything else here is host-side orchestration over kernels the
+verified tiers already exercise.)
 
 (Round 2: the module-wide xfail marker of round 1 is gone -- every test here has to pass on hardware.)"""
 import numpy as np
@@ -232,7 +232,7 @@ def test_attentive_aggregation_matches_reference_fixture():
 
 @pytest.mark.parametrize("depth,bias,d_h", [(3, False, 300), (1, True, 64), (4, True, 128)])
 def test_training_dropout_on_the_fused_bf16_path(depth, bias, d_h):
-    """ReLU + dropout in training stays on the fused tcgen05 path; mask for mask against the oracle."""
+    """ReLU + dropout in training stays on the fused tensor-core path; mask for mask against the oracle."""
     from tests.util import fused_dropout_vs_oracle
 
     fused_dropout_vs_oracle("cuda", depth=depth, bias=bias, d_h=d_h, n_mols=400)

@@ -203,11 +203,11 @@ def test_batchmolgraph_pickles_with_its_staging_copy_and_meta_words():
 
 
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):
-    """No silent fallback: without libdmpnn_sm100.so every entry into the engine raises, naming the build command."""
+    """No silent fallback: without libdmpnn_sm90.so every entry into the engine raises, naming the build command."""
     from chemprop_b200 import _lib
 
     monkeypatch.setattr(_lib, "_lib", None)
-    monkeypatch.setattr(_lib, "LIB_PATH", tmp_path / "libdmpnn_sm100.so")
+    monkeypatch.setattr(_lib, "LIB_PATH", tmp_path / "libdmpnn_sm90.so")
     with pytest.raises(DmpnnError, match="chemprop_b200.build.*no CPU / PyTorch fallback"):
         _lib.load()
     with pytest.raises(DmpnnError, match="not found"):

@@ -1,5 +1,6 @@
 """CPU tier: PackedBatchLoader -- the reference's build_dataloader + SeededSampler + DistributedSampler semantics
 (chemprop/data/dataloader.py:24-96, samplers.py:8-27) over the packed data set."""
+import os
 import time
 
 import numpy as np
@@ -8,9 +9,9 @@ import torch
 
 from chemprop_b200.data import BatchMolGraph, PackedBatchLoader, PackedMolGraphDataset, make_molecules
 from chemprop_b200.data.loader import epoch_shard
-from oracle.ref_shim import reference_available
 
 N = 203
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -35,16 +36,12 @@ def test_seeded_order_is_the_references_seeded_sampler(data):
         got = np.concatenate([b.ids for b in loader])
         assert np.array_equal(got, idxs), epoch
     assert len(loader) == 7                                        # 203 = 6 * 32 + 11
-    if reference_available():
-        from oracle.ref_shim import import_reference
-
-        import_reference()
-        from chemprop.data.samplers import SeededSampler
-
-        ref = SeededSampler(N, 99)
-        ours = PackedBatchLoader(ds, batch_size=50, shuffle=True, seed=99, pack_tiles=False)
-        for _ in range(2):
-            assert np.array_equal(np.fromiter(iter(ref), dtype=np.int64), np.concatenate([b.ids for b in ours]))
+    # two epochs of the reference's SeededSampler(203, seed 99), recorded by `oracle/make_golden.py live`
+    ref = np.load(os.path.join(ROOT, "tests", "golden", "fixture_seeded_sampler.npz"))["order"].astype(np.int64)
+    ours = PackedBatchLoader(ds, batch_size=50, shuffle=True, seed=99, pack_tiles=False)
+    assert N == 203
+    for epoch in range(2):
+        assert np.array_equal(ref[epoch], np.concatenate([b.ids for b in ours]))
 
 
 @pytest.mark.parametrize("prefetch,compact", [(2, False), (3, True)])

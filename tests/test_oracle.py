@@ -1,12 +1,11 @@
 """CPU tier: pins oracle/restatement.py against the reference -- (1) every committed golden vector
-(produced by the unmodified reference, oracle/make_golden.py), (2) the live reference when the
-reference tree is reachable (it is not on the GPU box)."""
+(produced by the unmodified reference, oracle/make_golden.py), (2) the reference's module on fresh seeded molecules, as
+recorded in tests/golden/fixture_live_*.npz."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import layout_np, restatement as R
-from oracle.ref_shim import reference_available
 from tests.util import golden_names, load_golden, mab_oracle_forward, oracle_forward
 
 TOL = dict(rtol=1e-5, atol=1e-6)  # same torch ops on the same machine: differences are summation-order only
@@ -136,40 +135,43 @@ def test_layout_restatement_properties():
     assert Lb["max_tile_rows"] > 128 and Lb["n_tiles"] == 3
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference tree not reachable (GPU box)")
 @pytest.mark.parametrize("kind,depth,bias,undirected,act", [
     ("bond", 3, False, False, "relu"), ("bond", 4, True, True, "elu"), ("atom", 3, True, False, "leakyrelu"),
     ("atom", 2, False, False, "tanh"), ("bond", 1, False, False, "relu"),
 ])
 def test_restatement_matches_live_reference(kind, depth, bias, undirected, act):
-    from oracle.ref_shim import import_reference
-
-    import_reference()
-    from chemprop.data import BatchMolGraph
-    from chemprop.data.molgraph import MolGraph
-    from chemprop.nn import AtomMessagePassing, BondMessagePassing, MeanAggregation
+    """The restatement against the reference's own module on fresh seeded molecules, as recorded from the unmodified reference
+    by `oracle/make_golden.py live` (tests/golden/fixture_live_<i>.npz, i = this case's index in LIVE_CASES): same initial
+    weights (checksum), the reference's collate of the batch (SHA-256 digests), its whole mean aggregate, seeded samples of
+    its hidden states and weight gradients."""
+    import hashlib
 
     from chemprop_b200.data.synthetic import make_molecules
+    from chemprop_b200.nn import AtomMessagePassing, BondMessagePassing
+    from oracle.make_golden import LIVE_CASES
 
+    g = load_golden(f"fixture_live_{LIVE_CASES.index((kind, depth, bias, undirected, act))}")
     torch.set_num_threads(1)
     torch.manual_seed(7)
     mgs = make_molecules(40, seed=11, shuffle_edges=True)
-    bmg = BatchMolGraph([MolGraph(*m) for m in mgs])
     cls = BondMessagePassing if kind == "bond" else AtomMessagePassing
-    mp = cls(d_h=96, depth=depth, bias=bias, undirected=undirected, activation=act)
-    H_ref = mp(bmg)
+    mp = cls(d_h=96, depth=depth, bias=bias, undirected=undirected, activation=act)   # the reference's initialisation order
+    for k, v in mp.state_dict().items():
+        np.testing.assert_allclose([v.double().sum().item(), v.double().abs().sum().item()], g["wsum." + k], rtol=1e-12, atol=1e-9)
+    # the restated collate is the reference's, byte for byte
+    col = dict(zip(("V", "E", "edge_index", "rev_edge_index", "batch"), R.collate(mgs)))
+    for k, x in col.items():
+        x = np.ascontiguousarray(np.asarray(x, dtype=str(g["dtype." + k])))
+        assert hashlib.sha256(x.tobytes()).digest() == g["sha256." + k].tobytes(), k
     P = {k: v.detach().clone().requires_grad_(True) for k, v in mp.state_dict().items()}
-    H = R.message_passing_forward(kind, bmg.V, bmg.E, bmg.edge_index, bmg.rev_edge_index, P["W_i.weight"],
+    t = {k: torch.from_numpy(np.asarray(x)) for k, x in col.items()}
+    H = R.message_passing_forward(kind, t["V"], t["E"], t["edge_index"], t["rev_edge_index"], P["W_i.weight"],
                                   P.get("W_i.bias"), P["W_h.weight"], P.get("W_h.bias"), P["W_o.weight"],
                                   P.get("W_o.bias"), depth, act, undirected)
-    torch.testing.assert_close(H, H_ref, **TOL)
-    a_ref = MeanAggregation()(H_ref, bmg.batch)
-    torch.testing.assert_close(R.aggregate(H, bmg.batch, "mean"), a_ref, **TOL)
-    a_ref.square().sum().backward()
-    R.aggregate(H, bmg.batch, "mean").square().sum().backward()
-    for k, p in mp.named_parameters():
-        torch.testing.assert_close(P[k].grad, p.grad, rtol=1e-4, atol=1e-6)
-    # and the reference's collate against the restated one
-    Vn, En, ein, revn, bn = R.collate(mgs)
-    assert np.array_equal(Vn, bmg.V.numpy()) and np.array_equal(ein, bmg.edge_index.numpy())
-    assert np.array_equal(revn, bmg.rev_edge_index.numpy()) and np.array_equal(bn, bmg.batch.numpy())
+    np.testing.assert_allclose(H.detach().numpy()[g["H_rows"]], g["H_sample"], **TOL)
+    a = R.aggregate(H, t["batch"], "mean")
+    np.testing.assert_allclose(a.detach().numpy()[:len(g["agg_mean"])], g["agg_mean"], **TOL)
+    a.square().sum().backward()
+    for k in P:
+        if "gidx." + k in g:
+            np.testing.assert_allclose(P[k].grad.numpy().reshape(-1)[g["gidx." + k]], g["grad." + k], rtol=1e-4, atol=1e-6)

@@ -117,7 +117,10 @@ class RecordingDropout(torch.nn.Dropout):
 
 def dropout_mask_for_mask(kind: str, undirected: bool, act: str, device: str, n_mols: int = 12, d_h: int = 32):
     """Training-mode dropout on the composed tier vs the oracle fed with the very masks the run drew (edge-level masks
-    mapped from the engine's dst-sorted row order back to the caller's edge order through `perm`)."""
+    mapped from the engine's dst-sorted row order back to the caller's edge order through `perm`).  ReLU / PReLU: where a
+    pre-activation lies within the f32 forward's error of zero, the oracle takes the run's side of the kink (z > 0, recorded
+    where the caller's activation module runs), so that rounding cannot flip a derivative between the run and the f64
+    oracle; everywhere else the run's branch must be the oracle's."""
     from chemprop_b200.data import BatchMolGraph, make_molecules
     from chemprop_b200.engine import get_layout
     from chemprop_b200.nn import AtomMessagePassing, BondMessagePassing, MeanAggregation
@@ -134,6 +137,9 @@ def dropout_mask_for_mask(kind: str, undirected: bool, act: str, device: str, n_
     assert mp.uses_composed_tier()
     V_d = torch.randn(bmg.V.shape[0], d_vd)
     P = {k: v.detach().double().requires_grad_(True) for k, v in mp.state_dict().items()}
+    signs = []
+    if act in ("relu", "prelu"):
+        mp.tau.register_forward_pre_hook(lambda _m, args: signs.append((args[0].detach() > 0).cpu()))
     mp = mp.to(device)
     bmg.to(device)
     H = mp(bmg, V_d.to(device))
@@ -148,9 +154,28 @@ def dropout_mask_for_mask(kind: str, undirected: bool, act: str, device: str, n_
         mm[perm] = m
         ref_masks.append(mm.double())
     ref_masks += [m.double() for m in masks[depth - 1:]]
+    tau = act
+    if signs:
+        # activation calls: tau(H_0) and one per depth step on edge rows (internal order), then one after W_o on atoms
+        assert len(signs) == depth + 1
+        ref_signs = []
+        for m in signs[:depth]:
+            mm = torch.empty_like(m)
+            mm[perm] = m
+            ref_signs.append(mm)
+        ref_signs.append(signs[depth])
+        slope = P["tau.weight"] if act == "prelu" else torch.zeros((), dtype=torch.float64)
+
+        def tau(x):
+            # the run's side of the kink is taken only where the f64 pre-activation lies within the f32 forward's error of
+            # zero (the bound H is held to below); everywhere else the run must have decided as the oracle does
+            run = ref_signs.pop(0)
+            near = x.detach().abs() <= 1e-5 * max(1.0, float(x.detach().abs().max()))
+            assert bool(((run == (x.detach() > 0)) | near).all()), "activation branch differs away from the kink"
+            return torch.where(torch.where(near, run, x.detach() > 0), x, x * slope)
     H_ref = R.message_passing_forward(kind, ref.V.double(), ref.E.double(), ref.edge_index, ref.rev_edge_index,
                                       P["W_i.weight"], P["W_i.bias"], P["W_h.weight"], P["W_h.bias"], P["W_o.weight"],
-                                      P["W_o.bias"], depth, act, undirected, V_d.double(), P["W_d.weight"], P["W_d.bias"],
+                                      P["W_o.bias"], depth, tau, undirected, V_d.double(), P["W_d.weight"], P["W_d.bias"],
                                       prelu_weight=P.get("tau.weight"), dropout_masks=ref_masks)
     R.aggregate(H_ref, ref.batch, "mean").square().sum().backward()
     assert (H.detach().double().cpu() - H_ref.detach()).abs().max().item() <= 1e-5

@@ -27,4 +27,4 @@ for first in (False, True):
         ts.append(e0.elapsed_time(e1))
     ms = sorted(ts)[len(ts) // 2]
     byt = (2 if first else 3) * lay.E * h * 2
-    print(f"PACK={os.environ.get('PACK','0')} EXP={os.environ.get('DMPNN_EXP','0')} first={first} E={lay.E} tiles={lay.n_tiles} h={h}: {ms*1e3:.1f} us  {byt/ms/1e6:.0f} GB/s  frac={byt/ms/1e6/6587.7:.3f}")
+    print(f"PACK={os.environ.get('PACK','0')} EXP={os.environ.get('DMPNN_EXP','0')} first={first} E={lay.E} tiles={lay.n_tiles} h={h}: {ms*1e3:.1f} us  {byt/ms/1e6:.0f} GB/s  frac={byt/ms/1e6/3350.0:.3f} of the H100 SXM data sheet's HBM bandwidth")
