@@ -178,7 +178,6 @@ static int launch_step(const char* what, const void* H_prev, const void* H_0, vo
   p.h = (int)h;
   p.hp = hp;
   p.nslab = g.nslab;
-  p.ksteps_last = (hp - 64 * (g.nslab - 1)) / 16;
   p.nchunks = g.nchunks;
   p.act_param = act_param;
   {

@@ -56,7 +56,7 @@ struct Params {
                                  // ATOMS there, `tile_row_ptr` / `tile_atom_ptr` hold the atom / edge offsets of the atom tiles
   const uint16_t* drop_bits;     // nullable (forward): 16 keep bits per (row, 16-column block), dmpnn_dropout_bits
   float drop_scale;              // 1 / (1 - p)
-  int n_tiles, h, hp, nslab, ksteps_last, nchunks;
+  int n_tiles, h, hp, nslab, nchunks;
   float act_param;
   int exp_flags;  // timing experiments only (DMPNN_EXP env var); 0 in production
   unsigned long long* trace;  // optional per-tile phase timestamps of block 0 (dmpnn_set_trace_buffer)
@@ -89,6 +89,19 @@ static_assert(B_WFREE + kWStages <= kNumBars, "barrier table too small");
 static_assert(kMaxSlabs == 5 && kMaxChunks <= 4, "barrier numbering assumes these");
 
 using namespace dmpnn::tc;
+
+// This kernel's bounded wait: the timeout of tc::mbar_wait, without its printf.  A function call anywhere in the kernel makes
+// ptxas serialise every wgmma (C7510), so on a timeout it only traps: a protocol bug still fails loudly (the launch ends in a
+// sticky error that the next synchronising CUDA call reports) instead of hanging the GPU, but it no longer names the block,
+// thread and barrier.  Swapping in tc::mbar_wait, whose printf names them, brings that report back for debugging (at the
+// cost of serialised wgmmas).
+__device__ __forceinline__ void mbar_wait_trap(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > 4000000000LL) asm volatile("trap;");
+  }
+}
 
 constexpr int kTraceEvents = 16;
 __device__ __forceinline__ void trace_ev(const Params& p, int it, int ev) {
@@ -126,7 +139,9 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
   int16_t* s_revl = reinterpret_cast<int16_t*>(smem + kOffRevl);
   float* s_bias = reinterpret_cast<float*>(smem + kOffBias);
   int16_t* s_nb = reinterpret_cast<int16_t*>(smem + kOffNb);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // the role dispatch below branches on `warp`: broadcast from lane 0 so that ptxas sees a warp-uniform value (a role taken
+  // from threadIdx.x directly is a divergent path to the compiler, and it serialises the wgmma instructions inside it)
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   auto bar = [&](int i) { return sBar + 8u * (uint32_t)i; };
 
   if (threadIdx.x == 0) {
@@ -161,7 +176,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
       // slab s of this tile is loaded as soon as the message warps have left slab s of the previous tile: the load
       // of the leading slabs overlaps the gather of the trailing ones (one shared-memory tile, no exposed latency)
       for (int s = 0; s < p.nslab; ++s) {
-        mbar_wait(bar(B_AFREE + s), (it & 1) ^ 1);
+        mbar_wait_trap(bar(B_AFREE + s), (it & 1) ^ 1);
         if (elect_one()) {
           if (s == 0) trace_ev(p, it, 0);
           mbar_expect_tx(bar(B_AFULL + s), kSlabBytes);
@@ -187,7 +202,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
           const uint8_t* src = p.Wpk + (size_t)c * kChunkN * p.nslab * 128 + (size_t)s0 * nc * 128;
           const uint32_t bytes = (uint32_t)(ns * nc * 128);
           const uint32_t st = ws % kWStages, use = ws / kWStages;
-          mbar_wait(bar(B_WFREE + st), (use & 1) ^ 1);
+          mbar_wait_trap(bar(B_WFREE + st), (use & 1) ^ 1);
           if (elect_one()) {
             if (p.exp_flags & 4096) {              // timing experiment: no W stream at all (stale shared memory, wrong results)
               mbar_arrive(bar(B_WFULL + st));
@@ -246,34 +261,64 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
 #pragma unroll
         for (int i = 0; i < 40; ++i) acc[i] = 0.f;
         const int nc = min(kChunkN, p.hp - c * kChunkN);
+        // A W stage (and, in the last chunk, its k pass of the A tile) is released once the wgmma group that read it has
+        // retired: the group of pass k stays in flight while pass k + 1 waits for its operands and issues (wait<1>)
+        auto release = [&](uint32_t st, int half) {
+          mbar_arrive(bar(B_WFREE + st));
+          if (c == p.nchunks - 1) mbar_arrive(bar(B_ATFREE + half));
+        };
+        uint32_t st_prev = 0;
         for (int half = 0; half < npass; ++half, ++ws) {
           const int s0 = half * kWHalfSlabs;
           const int ns = min(kWHalfSlabs, p.nslab - s0);
           if (!((a_waited >> half) & 1u)) {
             a_waited |= 1u << half;
-            mbar_wait(bar(B_AREADY + half), it & 1);                     // the message warps have written this k pass
-            if (half == 0 && tt == 0 && wg == 0) trace_ev(p, it, 3);
+            mbar_wait_trap(bar(B_AREADY + half), it & 1);           // the message warps have written this k pass
+            if (half == 0 && wg == 0 && tt == 0) trace_ev(p, it, 3);
           }
           const uint32_t st = ws % kWStages, usew = ws / kWStages;
-          mbar_wait(bar(B_WFULL + st), usew & 1);
+          mbar_wait_trap(bar(B_WFULL + st), usew & 1);
           if (!(kExp && (p.exp_flags & 262144))) {
-            wgmma_fence();
-            for (int si = 0; si < ns; ++si) {
+#pragma unroll
+            for (int si = 0; si < kWHalfSlabs; ++si) {
+              if (si >= ns) break;
               const int s = s0 + si;
-              const int ks = (s == p.nslab - 1) ? p.ksteps_last : 4;
               const uint64_t adesc = desc_sw128(sAop + (uint32_t)s * kSlabBytes + (uint32_t)wg * 8192u);
               const uint64_t bdesc = desc_sw128(sW + st * kWStageBytes + (uint32_t)(si * nc * 128));
-              for (int kk = 0; kk < ks; ++kk)   // k step = 16 bf16 = 32 B of each operand row
-                wgmma_bf16_n80(acc, adesc + (uint64_t)(2 * kk), bdesc + (uint64_t)(2 * kk), 1u);
+              // k step = 16 bf16 = 32 B of each operand row.  Every slab is four k steps, the last one too: its columns
+              // past hp are zero in the A operand tile (written once by the message warps) and in the packed W_h image, so
+              // they add exact zeros.  A slab is then one straight run of wgmmas behind one fence (a run-time k count would
+              // put a branch between wgmmas, and ptxas inserts a warpgroup.arrive in front of each of them: C7519).
+              wgmma_fence();
+#pragma unroll
+              for (int kk = 0; kk < 4; ++kk) wgmma_bf16_n80(acc, adesc + (uint64_t)(2 * kk), bdesc + (uint64_t)(2 * kk), 1u);
+              wgmma_commit();   // one group per slab: a commit after the slab loop would sit at a join ptxas guards (C7519)
             }
-            wgmma_commit();
-            wgmma_wait<0>();
-            acc_fence(acc);
           }
-          mbar_arrive(bar(B_WFREE + st));
-          // this k pass of the A tile may be overwritten once its last reader (the last chunk's pass over it) is done
-          if (c == p.nchunks - 1) mbar_arrive(bar(B_ATFREE + half));
+          if (half > 0) {   // the previous pass's groups have retired once at most this pass's ns groups are in flight
+            if (ns >= 3) wgmma_wait<3>();
+            else if (ns == 2) wgmma_wait<2>();
+            else wgmma_wait<1>();
+            release(st_prev, half - 1);
+          }
+          st_prev = st;
         }
+        // ---- epilogue operands: requested now, so that their L2 latency overlaps the last wgmma group
+        uint32_t hwv[2][kChunkN / 8];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = rA + 8 * h;
+          const __nv_bfloat16* yrow = p.H0 + (int64_t)(row0 + r) * p.ld;
+#pragma unroll
+          for (int b = 0; b < kChunkN / 8; ++b) {
+            hwv[h][b] = 0u;
+            if (MODE != MODE_BWD_COPY && r < nrows && 8 * b < nc)
+              hwv[h][b] = __ldg(reinterpret_cast<const unsigned int*>(yrow + c * kChunkN + 8 * b + cl));
+          }
+        }
+        wgmma_wait<0>();
+        acc_fence(acc);
+        release(st_prev, npass - 1);
         if (c == 0 && tt == 0) trace_ev(p, it, 6 + wg);
         // ---- epilogue of chunk c: rows rA, rA + 8; columns 80 c + 8 b + cl + {0, 1}
 #pragma unroll
@@ -282,7 +327,6 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
           if (r >= nrows) continue;
           const int64_t grow = (int64_t)(row0 + r);
           __nv_bfloat16* orow = p.Hn + grow * p.ld;
-          const __nv_bfloat16* yrow = p.H0 + grow * p.ld;
 #pragma unroll
           for (int b = 0; b < kChunkN / 8; ++b) {
             const int n = c * kChunkN + 8 * b + cl;
@@ -292,7 +336,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
             if constexpr (MODE == MODE_BWD_COPY) {          // dOut = (S.P)(dZ) . W_h
               o = pack_bf2(v0, v1);
             } else {
-              const uint32_t hw = __ldg(reinterpret_cast<const unsigned int*>(yrow + n));
+              const uint32_t hw = hwv[h][b];
               if constexpr (MODE == MODE_BWD_MASK || MODE == MODE_BWD_LAST) {
                 // ... * tau'(.): from the activation output the row came from, or (LAST) from the pre-activation H_0
                 const float g0 = MODE == MODE_BWD_LAST ? act_grad_from_pre(ACT, p.act_param, bf_lo(hw))
@@ -383,6 +427,13 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
       nx_natoms = __ldg(p.tile_atom_ptr + t1 + 1) - nx_atom0;
       nx_far = FAR && p.work_flag != nullptr && __ldg(p.work_flag + t1) != 0;
       if (nx_far) nx_natoms = 0;
+    }
+    // A operand columns [hp, 64 nslab) -- the last slab's k steps past hp, which the MMAs multiply with the zero columns of the
+    // packed W_h image -- are zeroed once here and never written again (published with the first k pass below)
+    for (int j = nj + shalf; j < p.nslab * 4; j += 2) {
+      const uint32_t ab = sAop + (uint32_t)(j >> 2) * kSlabBytes;
+      sts128(ab + sw128_off(r, 2 * (j & 3)), make_uint4(0, 0, 0, 0));
+      sts128(ab + sw128_off(r, 2 * (j & 3) + 1), make_uint4(0, 0, 0, 0));
     }
     for (; t < n_items; t += gridDim.x, ++it) {
       const int b = it & 1;
@@ -496,19 +547,19 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
       uint32_t left = (1u << p.nslab) - 1u;           // slabs this thread still has to release
       const int npass = (p.nslab + kWHalfSlabs - 1) / kWHalfSlabs;
       int cur_pass = 0;                               // k pass being written; earlier ones are published by this thread
-      if (!(p.exp_flags & 8192)) mbar_wait(bar(B_ATFREE + 0), (it & 1) ^ 1);    // tensor core is done with the first k pass of the previous tile
+      mbar_wait_trap(bar(B_ATFREE + 0), (it & 1) ^ 1);    // tensor core is done with the first k pass of the previous tile
       for (int j = shalf; j < nj; j += 2) {
         const int pj = (j >> 2) / kWHalfSlabs;
         if (pj != cur_pass) {                        // crossing into a later k pass: publish the finished ones, wait for the next
           fence_proxy_async();                       // A operand stores -> visible to wgmma (async proxy)
           for (int q = cur_pass; q < pj; ++q) mbar_arrive(bar(B_AREADY + q));
           cur_pass = pj;
-          if (!(p.exp_flags & 8192)) mbar_wait(bar(B_ATFREE + pj), (it & 1) ^ 1);   // 8192: timing experiment, as if A were double-buffered
+          mbar_wait_trap(bar(B_ATFREE + pj), (it & 1) ^ 1);
         }
         if ((j >> 2) != cur_slab) {                   // entering a new 64-column slab of the H tile
           if (cur_slab >= 0) { mbar_arrive(bar(B_AFREE + cur_slab)); left &= ~(1u << cur_slab); }
           cur_slab = j >> 2;
-          mbar_wait(bar(B_AFULL + cur_slab), it & 1);
+          mbar_wait_trap(bar(B_AFULL + cur_slab), it & 1);
           if (tS == 0 && cur_slab == 0) trace_ev(p, it, 1);
         }
         const uint32_t sbase = sA + (uint32_t)(j >> 2) * kSlabBytes;
