@@ -61,6 +61,8 @@ SIGNATURES = {
     "dmpnn_pack_weight_tc_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
     "dmpnn_pack_weight_tc": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _vp, _vp]),
     "dmpnn_linear_tc_bf16": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i32, _f32, _vp, _i64, _vp]),
+    "dmpnn_linear_tc_rows_bf16": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _i64, _vp, _i32, _f32, _vp, _i64, _i32,
+                                            _vp, _vp, _i64, _vp, _vp, _i32, _i64, _vp]),
     "dmpnn_tiles_workspace_bytes": (C.c_int, [_i64, C.POINTER(_sz)]),
     "dmpnn_tiles_build": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "dmpnn_atom_step_fused_bf16": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _f32,

@@ -12,6 +12,13 @@
 //   warps 4-11  two consumer warpgroups, rows [0, 64) and [64, 128) of the tile: wgmma m64n152k16 with the f32
 //               accumulator in registers, then the epilogue from registers: +bias (+residual) -> act -> bf16 -> global
 // HBM bytes per tile: read 128 x K x 2, write 128 x N x 2; W comes from L2.
+//
+// Epilogue variants (template EPI; the pipeline above is shared by all of them):
+//   kEpiBf16    C = act(acc + bias + res), bf16 store                              (dmpnn_linear_tc_bf16)
+//   kEpiF32     C = act(acc + bias), f32 store of columns [0, N)                   (per-atom / per-edge read-outs)
+//   kEpiMirror  C[out_row[r]] = (acc + res[res_row[r]]) * tau'(Y[out_row[r]]), bf16 store: the gradient of a read-out
+//               that enters a depth loop -- GEMM, row scatter, residual gather and tau' in one pass
+// The last two are reached through dmpnn_linear_tc_rows_bf16.
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -43,6 +50,7 @@ static_assert(kStageBytes % 1024 == 0 && kSlabBytes % 1024 == 0, "SWIZZLE_128B b
 static_assert(kSmemAlloc <= 232448, "exceeds shared memory");
 
 enum { B_FULL = 0, B_EMPTY = 4 };
+enum { kEpiBf16 = 0, kEpiF32 = 1, kEpiMirror = 2 };
 
 struct Params {
   const uint8_t* Wpk;
@@ -54,9 +62,16 @@ struct Params {
   int64_t R;
   int K, N, Npad, nslab, ksteps_last, n_tiles, n_nt;
   float act_param;
+  // kEpiF32 / kEpiMirror only
+  float* Cf;                  // f32 output (kEpiF32)
+  const __nv_bfloat16* Y;     // tau' source rows (kEpiMirror), row stride ldy
+  int64_t ldy;
+  const int32_t* out_row;     // nullable: output / Y row of A row r (identity when null)
+  const int32_t* res_row;     // nullable: residual row of A row r (identity when null)
+  int from_preact;            // Y holds the pre-activation instead of the activation output
 };
 
-template <int ACT, bool HAS_BIAS>
+template <int ACT, bool HAS_BIAS, int EPI = kEpiBf16>
 __global__ void __launch_bounds__(kThreads, 1)
 k_linear_tc(const __grid_constant__ CUtensorMap tmapA, Params p) {
   extern __shared__ uint8_t smem_raw[];
@@ -127,6 +142,52 @@ k_linear_tc(const __grid_constant__ CUtensorMap tmapA, Params p) {
       for (int h = 0; h < 2; ++h) {
         const int64_t grow = (int64_t)t * kTileM + rl + 8 * h;
         if (grow >= p.R) continue;
+        if constexpr (EPI == kEpiF32) {
+          float* crow = p.Cf + grow * p.ldc;
+#pragma unroll
+          for (int b = 0; b < kNT / 8; ++b) {
+            const int n = n0 + 8 * b + cl;
+            if (n >= p.N) continue;
+            float z0 = acc[4 * b + 2 * h], z1 = acc[4 * b + 2 * h + 1];
+            if constexpr (HAS_BIAS) { z0 += s_bias[n]; z1 += s_bias[n + 1]; }
+            z0 = act_t<ACT>(p.act_param, z0);
+            z1 = act_t<ACT>(p.act_param, z1);
+            if (n + 1 < p.N) *reinterpret_cast<float2*>(crow + n) = make_float2(z0, z1);
+            else crow[n] = z0;
+          }
+          continue;
+        }
+        if constexpr (EPI == kEpiMirror) {
+          const int64_t q = p.out_row != nullptr ? (int64_t)__ldg(p.out_row + grow) : grow;
+          const int64_t s = p.res_row != nullptr ? (int64_t)__ldg(p.res_row + grow) : grow;
+          __nv_bfloat16* crow = p.C + q * p.ldc;
+          const __nv_bfloat16* yrow = p.Y + q * p.ldy;
+          const __nv_bfloat16* rrow = p.res != nullptr ? p.res + s * p.ldres : nullptr;
+#pragma unroll
+          for (int b = 0; b < kNT / 8; ++b) {
+            const int n = n0 + 8 * b + cl;
+            if (n >= p.Npad) continue;
+            uint32_t o = 0u;                                      // columns [N, pad16(N)) are written as zeros
+            if (n < p.N) {
+              float z0 = acc[4 * b + 2 * h], z1 = acc[4 * b + 2 * h + 1];
+              if (rrow != nullptr) {
+                const uint32_t rw = __ldg(reinterpret_cast<const unsigned int*>(rrow + n));
+                z0 += bf_lo(rw); z1 += bf_hi(rw);
+              }
+              const uint32_t yw = __ldg(reinterpret_cast<const unsigned int*>(yrow + n));
+              if (p.from_preact) {
+                z0 *= act_grad_from_pre(ACT, p.act_param, bf_lo(yw));
+                z1 *= act_grad_from_pre(ACT, p.act_param, bf_hi(yw));
+              } else {
+                z0 *= act_grad_from_out(ACT, p.act_param, bf_lo(yw));
+                z1 *= act_grad_from_out(ACT, p.act_param, bf_hi(yw));
+              }
+              o = pack_bf2(z0, n + 1 < p.N ? z1 : 0.f);
+            }
+            *reinterpret_cast<uint32_t*>(crow + n) = o;
+          }
+          continue;
+        }
         __nv_bfloat16* crow = p.C + grow * p.ldc;
         const __nv_bfloat16* rrow = p.res != nullptr ? p.res + grow * p.ldres : nullptr;
 #pragma unroll
@@ -198,16 +259,26 @@ static bool encode_map(EncodeTiledFn enc, CUtensorMap* tmap, const void* base, i
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int ACT, bool HAS_BIAS>
+template <int ACT, bool HAS_BIAS, int EPI = kEpiBf16>
 static cudaError_t launch_variant(int grid, cudaStream_t st, const CUtensorMap& mA, const Params& p) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(k_linear_tc<ACT, HAS_BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemAlloc);
+    cudaError_t e = cudaFuncSetAttribute(k_linear_tc<ACT, HAS_BIAS, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemAlloc);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  k_linear_tc<ACT, HAS_BIAS><<<grid, kThreads, kSmemAlloc, st>>>(mA, p);
+  k_linear_tc<ACT, HAS_BIAS, EPI><<<grid, kThreads, kSmemAlloc, st>>>(mA, p);
   return cudaSuccess;
+}
+
+static int sm_count_cached() {
+  static int sm_count = 0;
+  if (!sm_count) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return sm_count;
 }
 
 }  // namespace lintc
@@ -269,14 +340,9 @@ extern "C" int dmpnn_linear_tc_bf16(const void* A, int64_t lda, int64_t R, int64
   p.n_tiles = (int)((R + kTileM - 1) / kTileM);
   p.n_nt = (g.Npad + kNT - 1) / kNT;
   p.act_param = act_param;
-  static int sm_count = 0;
-  if (!sm_count) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
-  }
   const int items = p.n_tiles * p.n_nt;
-  const int grid = items < sm_count ? items : sm_count;
+  const int sms = sm_count_cached();
+  const int grid = items < sms ? items : sms;
   cudaError_t e = cudaErrorInvalidValue;
 #define DMPNN_LAUNCH_ACT(A_)                                                                                   \
   case A_:                                                                                                     \
@@ -292,5 +358,92 @@ extern "C" int dmpnn_linear_tc_bf16(const void* A, int64_t lda, int64_t R, int64
 #undef DMPNN_LAUNCH_ACT
   DMPNN_CHECK_ARG(e == cudaSuccess, "linear_tc: cannot configure %d B dynamic smem: %s", kSmemAlloc, cudaGetErrorString(e));
   DMPNN_CHECK_LAUNCH("linear_tc", 1);
+  return 0;
+}
+
+static bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+extern "C" int dmpnn_linear_tc_rows_bf16(const void* A, int64_t lda, int64_t R, int64_t K, const void* Wpk, int64_t N,
+                                         const float* bias, int act, float act_param, const void* Y, int64_t ldy,
+                                         int from_preact, const int32_t* out_row, const void* res, int64_t ldres,
+                                         const int32_t* res_row, void* Cout, int out_dtype, int64_t ldc, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(R >= 0 && K > 0 && K <= kMaxK && N > 0 && N <= kMaxN, "linear_tc_rows: unsupported sizes K=%lld N=%lld",
+                  (long long)K, (long long)N);
+  DMPNN_CHECK_ARG(act >= DMPNN_ACT_NONE && act <= DMPNN_ACT_ELU, "linear_tc_rows: bad activation %d", act);
+  DMPNN_CHECK_ARG(out_dtype == DMPNN_F32 || out_dtype == DMPNN_BF16, "linear_tc_rows: bad output dtype %d", out_dtype);
+  if (R == 0) return 0;
+  DMPNN_CHECK_ARG(A && Wpk && Cout, "linear_tc_rows: null pointer");
+  PackGeom g = pack_geom(N, K);
+  DMPNN_CHECK_ARG(lda >= K && lda % 8 == 0 && al16(A) && al16(Wpk), "linear_tc_rows: lda must be >= K and a multiple of 8, "
+                  "A and Wpk 16-byte aligned");
+  const bool mirror = Y != nullptr;
+  if (mirror) {
+    DMPNN_CHECK_ARG(bias == nullptr && out_dtype == DMPNN_BF16, "linear_tc_rows: the mirror mode (Y given) takes no bias and "
+                    "stores bf16");
+    DMPNN_CHECK_ARG(ldy >= g.Npad && ldy % 8 == 0 && al16(Y), "linear_tc_rows: Y needs ldy >= %d, a multiple of 8, 16-byte "
+                    "alignment", g.Npad);
+    DMPNN_CHECK_ARG(res == nullptr || (ldres >= g.Npad && ldres % 8 == 0 && al16(res) && res != Cout),
+                    "linear_tc_rows: residual needs ldres >= %d, a multiple of 8, 16-byte alignment, and may not alias C", g.Npad);
+    DMPNN_CHECK_ARG(res != nullptr || res_row == nullptr, "linear_tc_rows: res_row without a residual");
+    DMPNN_CHECK_ARG(Y != Cout && A != Cout, "linear_tc_rows: C may not alias A or Y");
+  } else {
+    DMPNN_CHECK_ARG(out_row == nullptr && res == nullptr && res_row == nullptr && from_preact == 0,
+                    "linear_tc_rows: row maps, residual and from_preact belong to the mirror mode (Y given)");
+  }
+  if (out_dtype == DMPNN_BF16) {
+    DMPNN_CHECK_ARG(ldc >= g.Npad && ldc % 8 == 0 && al16(Cout), "linear_tc_rows: bf16 C needs ldc >= %d, a multiple of 8, "
+                    "16-byte alignment", g.Npad);
+  } else {
+    DMPNN_CHECK_ARG(ldc >= N && ldc % 2 == 0 && (reinterpret_cast<uintptr_t>(Cout) & 7) == 0,
+                    "linear_tc_rows: f32 C needs ldc >= N, even, and 8-byte alignment");
+  }
+  EncodeTiledFn enc = get_encode_fn();
+  DMPNN_CHECK_ARG(enc != nullptr, "linear_tc_rows: cuTensorMapEncodeTiled not available from the driver");
+  CUtensorMap mA;
+  DMPNN_CHECK_ARG(encode_map(enc, &mA, A, K, R, lda), "linear_tc_rows: cuTensorMapEncodeTiled failed");
+  Params p;
+  p.Wpk = (const uint8_t*)Wpk;
+  p.bias = bias;
+  p.res = (const __nv_bfloat16*)res;
+  p.ldres = ldres;
+  p.C = out_dtype == DMPNN_BF16 ? (__nv_bfloat16*)Cout : nullptr;
+  p.Cf = out_dtype == DMPNN_F32 ? (float*)Cout : nullptr;
+  p.ldc = ldc;
+  p.R = R;
+  p.K = (int)K;
+  p.N = (int)N;
+  p.Npad = g.Npad;
+  p.nslab = g.nslab;
+  p.ksteps_last = (g.Kpad - 64 * (g.nslab - 1)) / 16;
+  p.n_tiles = (int)((R + kTileM - 1) / kTileM);
+  p.n_nt = (g.Npad + kNT - 1) / kNT;
+  p.act_param = act_param;
+  p.Y = (const __nv_bfloat16*)Y;
+  p.ldy = ldy;
+  p.out_row = out_row;
+  p.res_row = res_row;
+  p.from_preact = from_preact ? 1 : 0;
+  const int items = p.n_tiles * p.n_nt;
+  const int sms = sm_count_cached();
+  const int grid = items < sms ? items : sms;
+  cudaError_t e = cudaErrorInvalidValue;
+#define DMPNN_LAUNCH_ACT(A_)                                                                                    \
+  case A_:                                                                                                      \
+    if (mirror) e = launch_variant<A_, false, kEpiMirror>(grid, st, mA, p);                                     \
+    else if (out_dtype == DMPNN_F32)                                                                            \
+      e = bias ? launch_variant<A_, true, kEpiF32>(grid, st, mA, p) : launch_variant<A_, false, kEpiF32>(grid, st, mA, p); \
+    else e = bias ? launch_variant<A_, true>(grid, st, mA, p) : launch_variant<A_, false>(grid, st, mA, p);     \
+    break;
+  switch (act) {
+    DMPNN_LAUNCH_ACT(DMPNN_ACT_NONE)
+    DMPNN_LAUNCH_ACT(DMPNN_ACT_RELU)
+    DMPNN_LAUNCH_ACT(DMPNN_ACT_LEAKYRELU)
+    DMPNN_LAUNCH_ACT(DMPNN_ACT_TANH)
+    DMPNN_LAUNCH_ACT(DMPNN_ACT_ELU)
+  }
+#undef DMPNN_LAUNCH_ACT
+  DMPNN_CHECK_ARG(e == cudaSuccess, "linear_tc_rows: cannot configure %d B dynamic smem: %s", kSmemAlloc, cudaGetErrorString(e));
+  DMPNN_CHECK_LAUNCH("linear_tc_rows", 1);
   return 0;
 }

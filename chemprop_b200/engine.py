@@ -115,6 +115,7 @@ class Layout:
     _meta_host: list | None = None
     _work: tuple | None = None
     _atom_work: tuple | None = None
+    _mab: tuple | None = None
 
     def _host(self):
         if self._meta_host is None:
@@ -473,6 +474,22 @@ def linear_tc(A: Tensor, K: int, Wpk: Tensor, N: int, out: Tensor, *, bias: Tens
     _lib.check(rc, "dmpnn_linear_tc_bf16")
 
 
+def linear_tc_rows(A: Tensor, K: int, Wpk: Tensor, N: int, out: Tensor, *, R: int | None = None, bias: Tensor | None = None,
+                   act: int = ACT_NONE, act_param: float = 0.0, Y: Tensor | None = None, from_preact: bool = False,
+                   out_row: Tensor | None = None, res: Tensor | None = None, res_row: Tensor | None = None):
+    """dmpnn_linear_tc_rows_bf16, acc = A[r, :K] . W^T.  Forward mode (Y None): out[r] = act(acc + bias), f32 or bf16 `out`.
+    Mirror mode: out[out_row[r]] = (acc + res[res_row[r]]) * tau'(Y[out_row[r]]) in bf16 (tau' of `act`, from the
+    pre-activation when `from_preact`); a missing map is the identity."""
+    lib = _lib.load()
+    R = A.shape[0] if R is None else R
+    assert A.dtype == torch.bfloat16 and (Y is None or Y.dtype == torch.bfloat16) and (res is None or res.dtype == torch.bfloat16)
+    rc = lib.dmpnn_linear_tc_rows_bf16(A.data_ptr(), _ld(A), R, K, Wpk.data_ptr(), N, _ptr(bias), act, float(act_param),
+                                       _ptr(Y), _ld(Y) if Y is not None else 0, 1 if from_preact else 0, _ptr(out_row),
+                                       _ptr(res), _ld(res) if res is not None else 0, _ptr(res_row),
+                                       out.data_ptr(), _dt(out), _ld(out), _stream())
+    _lib.check(rc, "dmpnn_linear_tc_rows_bf16")
+
+
 def wgrad_tc(dY: Tensor, X: Tensor, R: int, N: int, K: int, dW: Tensor, *, accumulate: bool = False):
     """dW[n, :K] (+)= sum_r dY[r, n] X[r, :K] on the tensor cores (bf16 operands)."""
     lib = _lib.load()
@@ -804,10 +821,11 @@ def atom_step_bwd_fused(dZ: Tensor, Yact: Tensor | None, dOut: Tensor, h: int, W
     _lib.check(rc, "dmpnn_atom_step_bwd_fused_bf16")
 
 
-def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor, bo,
-                 cfg: MPConfig, for_backward: bool = False):
+def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor | None, bo,
+                 cfg: MPConfig, for_backward: bool = False, readout_f32: bool = False):
     """BondMessagePassing.forward up to W_o (chemprop/nn/message_passing/base.py:196-212 with
-    mixins.py:8-18 and base.py:135-141, 180-182).  Returns (H_v, saved-for-backward)."""
+    mixins.py:8-18 and base.py:135-141, 180-182).  Returns (H_v, saved-for-backward).  `Wo` None: the depth loop only
+    (H_v None); `readout_f32` (tensor-core path): the W_o epilogue stores H_v in f32."""
     dev = V.device
     h = Wh.shape[0]
     hp = pad_hidden(h)
@@ -890,7 +908,9 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             Ms.append(M)
         Hs.append(Hn)
         Hprev, first = Hn, False
-    if tc:
+    if Wo is None:
+        XO = Mv = Hv = None
+    elif tc:
         # [V || M_v] assembled once in bf16 (torch.cat of base.py:180), M_v written in place by the segment sum
         hc = (h + 15) // 16 * 16       # zero columns up to pad16(h): 16-byte stores in the segment sum
         ko = (d_v + hc + 1 + 15) // 16 * 16
@@ -904,11 +924,15 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             # the bias gradient (the column sums of dY) as its last column -- no separate column-sum pass over V x h
             ones_col = d_v + hc
             XO[:, ones_col].fill_(1.0)
-        Hvp = torch.empty((max(nV, 1), pad_hidden(h)), dtype=T, device=dev)
-        linear_tc(XO, d_v + h, pack_weight_tc(Wo), h, Hvp, bias=bo, act=a, act_param=ap, R=nV)
-        if cfg.dropout_p > 0:
-            _dropout_(Hvp, cfg)                                                    # base.py:182
-        Hv = Hvp[:nV, :h]
+        if readout_f32:
+            Hv = torch.empty((max(nV, 1), h), dtype=torch.float32, device=dev)[:nV]
+            linear_tc_rows(XO, d_v + h, pack_weight_tc(Wo), h, Hv, R=nV, bias=bo, act=a, act_param=ap)
+        else:
+            Hvp = torch.empty((max(nV, 1), pad_hidden(h)), dtype=T, device=dev)
+            linear_tc(XO, d_v + h, pack_weight_tc(Wo), h, Hvp, bias=bo, act=a, act_param=ap, R=nV)
+            if cfg.dropout_p > 0:
+                _dropout_(Hvp, cfg)                                                    # base.py:182
+            Hv = Hvp[:nV, :h]
     else:
         if cfg.dropout_p > 0:
             raise DmpnnError("dropout on the monolithic tier needs the tensor-core path (see dropout_fused_ok)")
@@ -1072,10 +1096,13 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
 
 
 def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
-                     saved: dict, gHv: Tensor, need_bias: tuple[bool, bool, bool]):
+                     saved: dict, gHv: Tensor | None, need_bias: tuple[bool, bool, bool], entry=None):
     """bf16-tier autograd mirror on the tensor-core kernels (directed bonds).  Differences from the generic
     mirror: every GEMM is on the tensor cores (wgmma); tau' is fused into the backward message kernel; dH_0 is never kept as an f32
-    read-modify-write accumulator -- the per-step dZ^t stay in bf16 and are summed once, in f32, at the end."""
+    read-modify-write accumulator -- the per-step dZ^t stay in bf16 and are summed once, in f32, at the end.
+    `gHv` None: no read-out (dW_o, db_o None).  `entry(dMv, Y, from_preact, out)` (the mol-atom-bond edge head) replaces the
+    pass that starts the loop, out = dM_v[dst(r)] * tau'(Y[r]): it writes out = (its own term + dM_v[dst(r)]) * tau'(Y[r]),
+    dMv None when there is no read-out."""
     dev = V.device
     h = Wh.shape[0]
     hp = pad_hidden(h)
@@ -1092,7 +1119,7 @@ def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
     no_e = nE == 0
     dWi = torch.zeros_like(Wi, dtype=torch.float32) if no_e else torch.empty_like(Wi, dtype=torch.float32)
     dWh = torch.zeros_like(Wh, dtype=torch.float32) if (no_e or cfg.depth == 1) else torch.empty_like(Wh, dtype=torch.float32)
-    dWo = torch.empty_like(Wo, dtype=torch.float32)
+    dWo = torch.empty_like(Wo, dtype=torch.float32) if gHv is not None else None
     wh_acc = [False]                                  # has dW_h been written yet?
 
     def wgrad_h(dYt, Xt):
@@ -1100,9 +1127,7 @@ def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
         wh_acc[0] = True
     dbi = torch.zeros(h, **f32) if need_bias[0] else None
     dbh = torch.zeros(h, **f32) if need_bias[1] else None
-    dbo = torch.zeros(h, **f32) if need_bias[2] else None
-    if gHv.stride(1) != 1:
-        gHv = gHv.contiguous()
+    dbo = torch.zeros(h, **f32) if (need_bias[2] and gHv is not None) else None
     # Training-mode dropout (cfg.dropout_p > 0; ReLU only, dropout_fused_ok): a gradient that crosses a dropout site is
     # multiplied by the keep mask and by s = 1 / (1 - p).  With ReLU the mask is already in tau' of the stored POST-dropout
     # state ([H_post > 0] = mask * [H_pre > 0]), and s, a scalar, folds into the packed weight of the GEMM that produces
@@ -1110,29 +1135,37 @@ def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
     s_drop = 1.0 / (1.0 - cfg.dropout_p) if cfg.dropout_p > 0 else 1.0
     s_v = s_drop                                      # site after W_o (base.py:182)
     s_e = s_drop if cfg.depth > 1 else 1.0            # site on H^{T-1} (base.py:139); H^0 = tau(H_0) has none
-    dY = _empty_hidden(nV, hp, T, dev)
-    act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)      # dY / s_v
-    oc = saved.get("ones_col")
-    if dbo is not None and oc is not None:
-        dWo_ext = torch.empty((h, oc + 1), **f32)            # [dW_o | 0 | db_o]: the ones column of XO (bond_forward)
-        wgrad_tc(dY, saved["XO"], nV, h, oc + 1, dWo_ext)
-        dWo, dbo = dWo_ext[:, : d_v + h], dWo_ext[:, oc]
-    else:
-        wgrad_tc(dY, saved["XO"], nV, h, d_v + h, dWo)
-        if dbo is not None:
-            column_sum(dY, nV, h, dbo)
-    if s_v != 1.0:
-        dWo.mul_(s_v)
-        if dbo is not None:
-            dbo.mul_(s_v)
+    if gHv is not None:
+        if gHv.stride(1) != 1:
+            gHv = gHv.contiguous()
+        dY = _empty_hidden(nV, hp, T, dev)
+        act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)      # dY / s_v
+        oc = saved.get("ones_col")
+        if dbo is not None and oc is not None:
+            dWo_ext = torch.empty((h, oc + 1), **f32)            # [dW_o | 0 | db_o]: the ones column of XO (bond_forward)
+            wgrad_tc(dY, saved["XO"], nV, h, oc + 1, dWo_ext)
+            dWo, dbo = dWo_ext[:, : d_v + h], dWo_ext[:, oc]
+        else:
+            wgrad_tc(dY, saved["XO"], nV, h, d_v + h, dWo)
+            if dbo is not None:
+                column_sum(dY, nV, h, dbo)
+        if s_v != 1.0:
+            dWo.mul_(s_v)
+            if dbo is not None:
+                dbo.mul_(s_v)
     if nE == 0:
         return dWi, dbi, dWh, dbh, dWo, dbo
-    dMv = _empty_hidden(nV, hp, T, dev)
-    Wo_m = Wo[:, d_v:] if s_v * s_e == 1.0 else Wo[:, d_v:] * (s_v * s_e)
-    linear_tc(dY, h, pack_weight_tc(Wo_m, transpose=True), h, dMv, R=nV)
+    dMv = None
+    if gHv is not None:
+        dMv = _empty_hidden(nV, hp, T, dev)
+        Wo_m = Wo[:, d_v:] if s_v * s_e == 1.0 else Wo[:, d_v:] * (s_v * s_e)
+        linear_tc(dY, h, pack_weight_tc(Wo_m, transpose=True), h, dMv, R=nV)
     dH0b = _empty_hidden(nE, hp, T, dev)
     if cfg.depth == 1:
-        act_bwd(dMv, H0, nE, hc, act=a, act_param=ap, gidx=lay.dst_row, from_preact=True, dZ=dH0b)
+        if entry is not None:
+            entry(dMv, H0, True, dH0b)
+        else:
+            act_bwd(dMv, H0, nE, hc, act=a, act_param=ap, gidx=lay.dst_row, from_preact=True, dZ=dH0b)
     else:
         fused_bwd = _fused_step_ok(cfg, lay, h)      # the depth step's mirror on the same fused wgmma kernel
         if s_drop != 1.0 and not fused_bwd:
@@ -1142,7 +1175,10 @@ def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
         # mirror steps whose result arrives at a dropout site (every one but the last, which lands on H^0) carry s
         WhT_pkf_s = WhT_pkf if s_drop == 1.0 else pack_weight_bf16((Wh * s_drop).t().contiguous())
         dZ = _empty_hidden(nE, hp, T, dev)
-        act_bwd(dMv, Hs[-1], nE, hc, act=a, act_param=ap, gidx=lay.dst_row, dZ=dZ)    # dZ^{T-1}
+        if entry is not None:
+            entry(dMv, Hs[-1], False, dZ)
+        else:
+            act_bwd(dMv, Hs[-1], nE, hc, act=a, act_param=ap, gidx=lay.dst_row, dZ=dZ)    # dZ^{T-1}
         dZs, dH_first, fused_sum, dH0_terms = [dZ], None, False, None
         for t in range(cfg.depth - 1, 0, -1):
             first = t == 1
@@ -1359,9 +1395,39 @@ def _atom_tc_ok(cfg: MPConfig, h: int, d_v: int, d_e: int) -> bool:
     return _tc_ok(cfg, h, d_v, h + d_e, d_v + h) and h % 4 == 0
 
 
-def atom_forward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor, bo, cfg: MPConfig):
+def _atom_readout_tc(lay: Layout, V: Tensor, Hprev: Tensor, first: bool, h: int, Wo: Tensor, bo, cfg: MPConfig, rows: int,
+                     with_ones: bool, readout_f32: bool):
+    """H_v = tau(W_o([V || M_v])) of the atom tiers (base.py:180-182, 208-211): returns (H_v, XO, dvp, ones_col).  `with_ones`:
+    a ones column after [V || M_v || 0-pad] delivers db_o with dW_o's GEMM (see bond_forward)."""
+    dev, T, nV = V.device, cfg.hidden_dtype, lay.V
+    a, ap = cfg.act, cfg.act_param
+    d_v = V.shape[1]
+    hc = (h + 15) // 16 * 16
+    dvp = _readout_pad(d_v, h)
+    ones_col = dvp + hc if (with_ones and bo is not None and dvp + hc + 1 <= 448) else None
+    ko = (dvp + hc + 1 + 15) // 16 * 16 if ones_col is not None else (dvp + h + 15) // 16 * 16
+    XO = torch.empty((rows, ko), dtype=T, device=dev)
+    concat_bf16(V, d_v, XO, nV, width=dvp)
+    segment_sum(Hprev, lay.rowptr, nV, h, XO[:, dvp:dvp + h], idx=lay.src_row, act=(a if first else ACT_NONE),
+                act_param=ap, pad_to=(hc if dvp + hc <= ko else h))                           # base.py:208-211
+    if ones_col is not None:
+        XO[:, ones_col].fill_(1.0)
+    Wpk = pack_weight_tc(_wo_padded(Wo, d_v, dvp))
+    if readout_f32:
+        Hv = torch.empty((rows, h), dtype=torch.float32, device=dev)[:nV]
+        linear_tc_rows(XO, dvp + h, Wpk, h, Hv, R=nV, bias=bo, act=a, act_param=ap)
+    else:
+        Hvp = torch.empty((rows, pad_hidden(h)), dtype=T, device=dev)
+        linear_tc(XO, dvp + h, Wpk, h, Hvp, bias=bo, act=a, act_param=ap, R=nV)         # base.py:180-182
+        Hv = Hvp[:nV, :h]
+    return Hv, XO, dvp, ones_col
+
+
+def atom_forward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor, bo, cfg: MPConfig,
+                    readout_f32: bool = False):
     """bf16 tier of atom_forward on the tensor cores: every GEMM is dmpnn_linear_tc_bf16 (the H_0 residual of
-    base.py:138 is added in its epilogue), the neighbour sums write straight into the GEMM's A operand."""
+    base.py:138 is added in its epilogue), the neighbour sums write straight into the GEMM's A operand.  `Wo` None: no
+    read-out; `readout_f32`: H_v stored in f32."""
     dev = V.device
     h = Wi.shape[0]
     hp = pad_hidden(h)
@@ -1396,21 +1462,17 @@ def atom_forward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tenso
         Hs.append(Hn)
         XAs.append(XA)
         Hprev, first = Hn, False
-    dvp = _readout_pad(d_v, h)
-    ko = (dvp + h + 15) // 16 * 16
-    XO = torch.empty((rows, ko), dtype=T, device=dev)
-    concat_bf16(V, d_v, XO, nV, width=dvp)
-    segment_sum(Hprev, lay.rowptr, nV, h, XO[:, dvp:dvp + h], idx=lay.src_row, act=(a if first else ACT_NONE),
-                act_param=ap, pad_to=(hc if dvp + hc <= ko else h))                           # base.py:208-211
-    Hvp = torch.empty((rows, hp), dtype=T, device=dev)
-    linear_tc(XO, dvp + h, pack_weight_tc(_wo_padded(Wo, d_v, dvp)), h, Hvp, bias=bo, act=a, act_param=ap, R=nV)    # base.py:180-182
-    Hv = Hvp[:nV, :h]
+    Hv = XO = dvp = None
+    if Wo is not None:
+        Hv, XO, dvp, _ = _atom_readout_tc(lay, V, Hprev, first, h, Wo, bo, cfg, rows, False, readout_f32)
     return Hv, dict(H0=H0, Hs=Hs, XAs=XAs, XO=XO, Xv=Xv, Hv=Hv, tc=True, dvp=dvp)
 
 
 def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
-                     saved: dict, gHv: Tensor, need_bias):
-    """Autograd mirror of atom_forward_tc (wgmma GEMMs; dH_0 is kept as separate terms, one W_i GEMM each)."""
+                     saved: dict, gHv: Tensor | None, need_bias, entry=None):
+    """Autograd mirror of atom_forward_tc (wgmma GEMMs; dH_0 is kept as separate terms, one W_i GEMM each).  `gHv` None:
+    no read-out.  `entry(dHa, Y, from_preact, out)` (the mol-atom-bond edge head) replaces the first tau' pass
+    out = dHa * tau'(Y): it writes out = (its own term + dHa) * tau'(Y), dHa None when there is no read-out."""
     dev = V.device
     h = Wi.shape[0]
     hp = pad_hidden(h)
@@ -1423,35 +1485,40 @@ def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
     f32 = dict(dtype=torch.float32, device=dev)
     dWi = torch.zeros_like(Wi, dtype=torch.float32)
     dWh = torch.zeros_like(Wh, dtype=torch.float32)
-    dWo = torch.zeros_like(Wo, dtype=torch.float32)
+    dWo = torch.zeros_like(Wo, dtype=torch.float32) if gHv is not None else None
     dbi = torch.zeros(h, **f32) if need_bias[0] else None
     dbh = torch.zeros(h, **f32) if need_bias[1] else None
-    dbo = torch.zeros(h, **f32) if need_bias[2] else None
+    dbo = torch.zeros(h, **f32) if (need_bias[2] and gHv is not None) else None
     if nV == 0:
         return dWi, dbi, dWh, dbh, dWo, dbo
-    if gHv.stride(1) != 1:
-        gHv = gHv.contiguous()
-    dY = _empty_hidden(nV, hp, T, dev)
-    act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)
-    dvp = saved.get("dvp", d_v)
-    if dvp == d_v:
-        wgrad_tc(dY, XO, nV, h, d_v + h, dWo)
-    else:
-        dWo_p = torch.empty((h, dvp + h), dtype=torch.float32, device=dev)
-        wgrad_tc(dY, XO, nV, h, dvp + h, dWo_p)
-        dWo = _wo_unpadded(dWo_p, d_v, dvp)
-    if dbo is not None:
-        column_sum(dY, nV, h, dbo)
-    dMv = _empty_hidden(nV, hp, T, dev)
-    linear_tc(dY, h, pack_weight_tc(Wo[:, d_v:], transpose=True), h, dMv, R=nV)
-    # d(Ha^{T-1})[u] = sum_{e' in in(u)} dM_v[src(e')]   (rev is an involution)
-    dHa = _empty_hidden(nV, hp, T, dev)
-    segment_sum(dMv, lay.rowptr, nV, h, dHa, idx=lay.src_row, pad_to=hc)
+    dHa = None
+    if gHv is not None:
+        if gHv.stride(1) != 1:
+            gHv = gHv.contiguous()
+        dY = _empty_hidden(nV, hp, T, dev)
+        act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)
+        dvp = saved.get("dvp", d_v)
+        if dvp == d_v:
+            wgrad_tc(dY, XO, nV, h, d_v + h, dWo)
+        else:
+            dWo_p = torch.empty((h, dvp + h), dtype=torch.float32, device=dev)
+            wgrad_tc(dY, XO, nV, h, dvp + h, dWo_p)
+            dWo = _wo_unpadded(dWo_p, d_v, dvp)
+        if dbo is not None:
+            column_sum(dY, nV, h, dbo)
+        dMv = _empty_hidden(nV, hp, T, dev)
+        linear_tc(dY, h, pack_weight_tc(Wo[:, d_v:], transpose=True), h, dMv, R=nV)
+        # d(Ha^{T-1})[u] = sum_{e' in in(u)} dM_v[src(e')]   (rev is an involution)
+        dHa = _empty_hidden(nV, hp, T, dev)
+        segment_sum(dMv, lay.rowptr, nV, h, dHa, idx=lay.src_row, pad_to=hc)
     WhT_pk = pack_weight_tc(Wh[:, :h], transpose=True) if cfg.depth > 1 else None
     terms = []
     for t in range(cfg.depth - 1, 0, -1):
         dZ = _empty_hidden(nV, hp, T, dev)
-        act_bwd(dHa, Hs[t - 1], nV, hc, act=a, act_param=ap, dZ=dZ)
+        if entry is not None and t == cfg.depth - 1:
+            entry(dHa, Hs[t - 1], False, dZ)
+        else:
+            act_bwd(dHa, Hs[t - 1], nV, hc, act=a, act_param=ap, dZ=dZ)
         terms.append(dZ)
         wgrad_tc(dZ, XAs[t - 1], nV, h, h + d_e, dWh, accumulate=True)
         if dbh is not None:
@@ -1461,7 +1528,10 @@ def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
         dHa = _empty_hidden(nV, hp, T, dev)
         segment_sum(dN, lay.rowptr, nV, h, dHa, idx=lay.src_row, pad_to=hc)
     dH0l = _empty_hidden(nV, hp, T, dev)
-    act_bwd(dHa, H0, nV, hc, act=a, act_param=ap, from_preact=True, dZ=dH0l)
+    if entry is not None and cfg.depth == 1:
+        entry(dHa, H0, True, dH0l)
+    else:
+        act_bwd(dHa, H0, nV, hc, act=a, act_param=ap, from_preact=True, dZ=dH0l)
     terms.append(dH0l)
     wgrad_tc_multi(terms, Xv, nV, h, d_v, dWi)       # dH_0 = sum_t dZ^t + dHa^0 * tau'(H_0), contracted term by term
     if dbi is not None:
@@ -1470,7 +1540,8 @@ def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
     return dWi, dbi, dWh, dbh, dWo, dbo
 
 
-def atom_forward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor, bo, cfg: MPConfig):
+def atom_forward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor, bo, cfg: MPConfig,
+                       readout_f32: bool = False):
     """bf16 tier of atom_forward with ONE launch per depth step (dmpnn_atom_step_fused_bf16).  The reference's update
     (base.py:135-141) on atoms is tau(H_0 + b_h + W_h . [N^t || SE]) with N^t the neighbour sum of the previous state and SE the
     loop-invariant sum of the incoming bond features: W_h[:, h:] . SE + b_h is added to H_0 ONCE (a K = d_e GEMM with H_0 as
@@ -1513,23 +1584,14 @@ def atom_forward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Te
             atom_step_fused(Hprev, H0p, Hn, h, Whpk, step_bias, lay, a, ap, first, N_out=N1 if first else None)
         Hs.append(Hn)
         Hprev, first = Hn, False
-    dvp = _readout_pad(d_v, h)
-    ones_col = dvp + hc if (bo is not None and dvp + hc + 1 <= 448) else None   # see bond_forward: db_o rides on dW_o's GEMM
-    ko = (dvp + hc + 1 + 15) // 16 * 16 if ones_col is not None else (dvp + h + 15) // 16 * 16
-    XO = torch.empty((rows, ko), dtype=T, device=dev)
-    concat_bf16(V, d_v, XO, nV, width=dvp)
-    segment_sum(Hprev, lay.rowptr, nV, h, XO[:, dvp:dvp + h], idx=lay.src_row, act=ACT_NONE, act_param=ap,
-                pad_to=(hc if dvp + hc <= ko else h))                                         # base.py:208-211
-    if ones_col is not None:
-        XO[:, ones_col].fill_(1.0)
-    Hvp = torch.empty((rows, hp), dtype=T, device=dev)
-    linear_tc(XO, dvp + h, pack_weight_tc(_wo_padded(Wo, d_v, dvp)), h, Hvp, bias=bo, act=a, act_param=ap, R=nV)    # base.py:180-182
-    Hv = Hvp[:nV, :h]
+    Hv = XO = dvp = ones_col = None
+    if Wo is not None:          # db_o rides on dW_o's GEMM (ones column)
+        Hv, XO, dvp, ones_col = _atom_readout_tc(lay, V, Hprev, first, h, Wo, bo, cfg, rows, True, readout_f32)
     return Hv, dict(H0=H0, Hs=Hs, N1=N1, SEb=SEb, XO=XO, Xv=Xv, Hv=Hv, tc=True, fused=True, dvp=dvp, ones_col=ones_col)
 
 
 def atom_backward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
-                        saved: dict, gHv: Tensor, need_bias):
+                        saved: dict, gHv: Tensor | None, need_bias, entry=None):
     """Autograd mirror of atom_forward_fused.  With A the (symmetric) atom adjacency, N^t = A H^{t-1}:
     dH^{t-1} = ((A dZ^t) . W_h[:, :h]) * tau'(H^{t-1}) -- the mirror mode of the fused kernel, whose gathered operand
     G^t = A dZ^t is also the left factor of the step's weight gradient (dZ^T . N^t = G^T . H^{t-1}); t = 1 uses the N^1 the
@@ -1546,33 +1608,47 @@ def atom_backward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tenso
     f32 = dict(dtype=torch.float32, device=dev)
     dWi = torch.empty_like(Wi, dtype=torch.float32)
     dWh = torch.empty_like(Wh, dtype=torch.float32)
-    dWo = torch.empty_like(Wo, dtype=torch.float32)
+    dWo = torch.empty_like(Wo, dtype=torch.float32) if gHv is not None else None
     dbi = torch.zeros(h, **f32) if need_bias[0] else None
     dbh = torch.zeros(h, **f32) if need_bias[1] else None
-    dbo = torch.zeros(h, **f32) if need_bias[2] else None
-    if gHv.stride(1) != 1:
-        gHv = gHv.contiguous()
-    dY = _empty_hidden(nV, hp, T, dev)
-    act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)
-    dvp = saved.get("dvp", d_v)
-    oc = saved.get("ones_col")
-    if dbo is not None and oc is not None:
-        dWo_p = torch.empty((h, oc + 1), dtype=torch.float32, device=dev)      # [dW_o (padded) | 0 | db_o]
-        wgrad_tc(dY, XO, nV, h, oc + 1, dWo_p)
-        dWo, dbo = _wo_unpadded(dWo_p[:, :dvp + h], d_v, dvp), dWo_p[:, oc]
-    else:
-        if dvp == d_v:
-            wgrad_tc(dY, XO, nV, h, d_v + h, dWo)
+    dbo = torch.zeros(h, **f32) if (need_bias[2] and gHv is not None) else None
+    if gHv is not None:
+        if gHv.stride(1) != 1:
+            gHv = gHv.contiguous()
+        dY = _empty_hidden(nV, hp, T, dev)
+        act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)
+        dvp = saved.get("dvp", d_v)
+        oc = saved.get("ones_col")
+        if dbo is not None and oc is not None:
+            dWo_p = torch.empty((h, oc + 1), dtype=torch.float32, device=dev)      # [dW_o (padded) | 0 | db_o]
+            wgrad_tc(dY, XO, nV, h, oc + 1, dWo_p)
+            dWo, dbo = _wo_unpadded(dWo_p[:, :dvp + h], d_v, dvp), dWo_p[:, oc]
         else:
-            dWo_p = torch.empty((h, dvp + h), dtype=torch.float32, device=dev)
-            wgrad_tc(dY, XO, nV, h, dvp + h, dWo_p)
-            dWo = _wo_unpadded(dWo_p, d_v, dvp)
-        if dbo is not None:
-            column_sum(dY, nV, h, dbo)
+            if dvp == d_v:
+                wgrad_tc(dY, XO, nV, h, d_v + h, dWo)
+            else:
+                dWo_p = torch.empty((h, dvp + h), dtype=torch.float32, device=dev)
+                wgrad_tc(dY, XO, nV, h, dvp + h, dWo_p)
+                dWo = _wo_unpadded(dWo_p, d_v, dvp)
+            if dbo is not None:
+                column_sum(dY, nV, h, dbo)
     # dZ^{T-1} = (A (dY . W_o[:, d_v:])) * tau'(H^{T-1}) = ((A dY) . W_o[:, d_v:]) * tau'(H^{T-1}): the read-out GEMM, the
     # neighbour gather of its result and the tau' pass are ONE mirror launch of the fused kernel on dY (three launches before)
-    dZ = _empty_hidden(nV, hp, T, dev)
-    atom_step_bwd_fused(dY, Hs[-1], dZ, h, pack_weight_bf16(Wo[:, d_v:].t().contiguous()), lay, a, ap)
+    if entry is None:
+        dZ = _empty_hidden(nV, hp, T, dev)
+        atom_step_bwd_fused(dY, Hs[-1], dZ, h, pack_weight_bf16(Wo[:, d_v:].t().contiguous()), lay, a, ap)
+    else:
+        # zero-filled: the entry writes columns up to pad16(h), the next mirror step's TMA boxes read up to the 64-column edge
+        dZ = _hidden(nV, hp, T, dev)
+        # `entry(dHa, Y, from_preact, out)` (mol-atom-bond edge head): the read-out's term unmasked, as in atom_backward_tc
+        # (dM_v = dY . W_o[:, d_v:], then its neighbour sum); the entry adds its own term and applies tau'
+        dHa = None
+        if gHv is not None:
+            dMv = _empty_hidden(nV, hp, T, dev)
+            linear_tc(dY, h, pack_weight_tc(Wo[:, d_v:], transpose=True), h, dMv, R=nV)
+            dHa = _empty_hidden(nV, hp, T, dev)
+            segment_sum(dMv, lay.rowptr, nV, h, dHa, idx=lay.src_row, pad_to=hc)
+        entry(dHa, Hs[-1], False, dZ)
     WhT = pack_weight_bf16(Wh[:, :h].t().contiguous())
     dWhN = dWh[:, :h]
     terms, wrote = [dZ], False
@@ -1645,6 +1721,159 @@ class AtomMPFunction(torch.autograd.Function):
         cast = lambda g, d: None if g is None else g.to(d)
         return (None, None, cast(dWi, d0), cast(dbi, d0), cast(dWh, d1), cast(dbh, d1), cast(dWo, d2),
                 cast(dbo, d2), None, None)
+
+
+# ----------------------------------------------------------------------------------------------
+# mol-atom-bond message passing on the bf16 tier (chemprop/nn/message_passing/mol_atom_bond.py): the depth loop and the
+# W_vo read-out of Bond / AtomMPFunction, plus the per-edge head H_e = tau(W_eo([E || H^{T-1}])) in the caller's edge order
+# ----------------------------------------------------------------------------------------------
+def mab_bf16_limits(kind: str, h: int, d_v: int, d_e: int) -> str | None:
+    """None when every GEMM of the bf16 mol-atom-bond path fits the tensor-core kernels (the limits of _tc_ok / _atom_tc_ok
+    plus K = d_e + d_h for W_eo), else the reason it does not."""
+    Ks = (d_v + d_e, d_v + h, d_e + h) if kind == "bond" else (d_v, h + d_e, d_v + h, d_e + h)
+    if h > 304:
+        return f"d_h = {h} > 304"
+    if h % 4 != 0:
+        return f"d_h = {h} not a multiple of 4"
+    if d_e == 0:
+        return "d_e = 0"
+    if any(k > 448 for k in Ks):
+        return f"GEMM inner dimensions {Ks} above 448"
+    if not _fused_available():
+        return "tensor-core kernels unavailable"
+    return None
+
+
+def mab_tables(lay: Layout):
+    """(dst atom of caller edge e, src atom of caller edge e, caller edge of the reverse of dst-sorted row r) as int32, built
+    once per batch: the residual map of the bond kind's mirror, the gather of the atom kind's edge operand, and the
+    out-edge table of the atom kind's backward segment sum."""
+    if lay._mab is None:
+        ip = lay.inv_perm.long()
+        lay._mab = (lay.dst_row.index_select(0, ip), lay.src_row.index_select(0, ip),
+                    lay.perm.index_select(0, lay.rev_row.long()))
+    return lay._mab
+
+
+class MABMPFunction(torch.autograd.Function):
+    """(H_v, H_e) of MABBond / MABAtomMessagePassing on the bf16 tier, both f32; an absent read-out (W_vo or W_eo None)
+    gives an empty tensor in its place.
+
+    Forward: the depth loop of bond_forward / atom_forward_fused (atom_forward_tc where the fused atom step does not apply),
+    the W_vo read-out with an f32 store, and the edge head: X_e[e] = [E[e] || H^{T-1}(e)] assembled once in caller order
+    (H^{T-1}(e) = H[inv_perm[e]] for bonds, H_a[src(e)] for atoms), then one tensor-core GEMM with bias, tau and the f32
+    store in its epilogue.  Backward: dY_e = g_e * tau'(H_e); dW_eo, db_eo from X_e; the gradient dY_e . W_eo[:, d_e:]
+    enters the depth loop's mirror at its first tau' (the `entry` of bond_backward_tc / the atom backward functions) through
+    the mirror mode of dmpnn_linear_tc_rows_bf16; the rest of the mirror is unchanged."""
+
+    @staticmethod
+    def forward(ctx, V, E, Wi, bi, Wh, bh, Wvo, bvo, Weo, beo, lay, cfg, kind):
+        _require_cuda(V, E, Wi, Wh)
+        _refuse_feature_grads(ctx)
+        V = V.contiguous().float()
+        E = E.contiguous().float()
+        f = lambda w: None if w is None else w.detach().contiguous().float()  # noqa: E731
+        Wi_, bi_, Wh_, bh_, Wvo_, bvo_, Weo_, beo_ = (f(w) for w in (Wi, bi, Wh, bh, Wvo, bvo, Weo, beo))
+        h = Wh_.shape[0]
+        d_v, d_e = V.shape[1], E.shape[1]
+        nE, nV = lay.E, lay.V
+        dev, T = V.device, cfg.hidden_dtype
+        a, ap = cfg.act, cfg.act_param
+        if kind == "bond":
+            Hv, saved = bond_forward(lay, V, E, Wi_, bi_, Wh_, bh_, Wvo_, bvo_, cfg, for_backward=any(ctx.needs_input_grad),
+                                     readout_f32=True)
+            src_idx = lay.inv_perm
+            if Weo_ is not None and nE > 0:
+                mab_tables(lay)            # built here, on the forward's stream, for the backward's residual map
+        else:
+            fwd = atom_forward_fused if _atom_fused_ok(cfg, lay, h, d_v, d_e) else atom_forward_tc
+            Hv, saved = fwd(lay, V, E, Wi_, bi_, Wh_, bh_, Wvo_, bvo_, cfg, readout_f32=True)
+            src_idx = mab_tables(lay)[1] if nE > 0 else None
+        He = Xe = None
+        if Weo_ is not None:
+            He = torch.empty((max(nE, 1), h), dtype=torch.float32, device=dev)[:nE]
+            if nE > 0:
+                Hfin = saved["Hs"][-1] if saved["Hs"] else None
+                if Hfin is None:
+                    # depth 1: H^0 = tau(H_0) is applied on load by every consumer and never stored -- the edge head needs the
+                    # activated rows, so the W_i GEMM runs once more with tau in its epilogue
+                    rows = nE if kind == "bond" else nV
+                    Hfin = _empty_hidden(rows, pad_hidden(h), T, dev)
+                    X, K = (saved["X0"], d_v + d_e) if kind == "bond" else (saved["Xv"], d_v)
+                    linear_tc(X, K, pack_weight_tc(Wi_), h, Hfin, bias=bi_, act=a, act_param=ap, R=rows)
+                Xe = torch.empty((nE, (d_e + h + 15) // 16 * 16), dtype=T, device=dev)
+                concat_bf16(E, d_e, Xe, nE, X2=Hfin, K2=h, idx2=src_idx)
+                linear_tc_rows(Xe, d_e + h, pack_weight_tc(Weo_), h, He, R=nE, bias=beo_, act=a, act_param=ap)
+        if Hv is not None:
+            saved["Hv"] = Hv.detach()          # see BondMPFunction.forward: no reference cycle through the output
+        ctx.lay, ctx.cfg, ctx.saved, ctx.kind = lay, cfg, saved, kind
+        ctx.VE = (V, E)
+        ctx.W = (Wi_, Wh_, Wvo_, Weo_)
+        ctx.edge = (Xe, None if He is None else He.detach())
+        ctx.has_bias = (bi is not None, bh is not None, bvo is not None, beo is not None)
+        ctx.wdtypes = tuple(None if w is None else w.dtype for w in (Wi, Wh, Wvo, Weo))
+        empty = torch.empty((0, h), dtype=torch.float32, device=dev)
+        return (Hv if Hv is not None else empty), (He if He is not None else empty)
+
+    @staticmethod
+    def backward(ctx, gHv, gHe):
+        V, E = ctx.VE
+        Wi, Wh, Wvo, Weo = ctx.W
+        Xe, He = ctx.edge
+        lay, cfg, kind = ctx.lay, ctx.cfg, ctx.kind
+        dev, T = V.device, cfg.hidden_dtype
+        h = Wh.shape[0]
+        hp, hc = pad_hidden(h), (h + 15) // 16 * 16
+        d_e = E.shape[1]
+        nE, nV = lay.E, lay.V
+        a, ap = cfg.act, cfg.act_param
+        f32 = dict(dtype=torch.float32, device=dev)
+        entry = None
+        dWeo = dbeo = None
+        if Weo is not None:
+            dWeo = torch.zeros_like(Weo)
+            dbeo = torch.zeros(h, **f32) if ctx.has_bias[3] else None
+            if nE > 0:
+                if gHe.stride(1) != 1:
+                    gHe = gHe.contiguous()
+                dYe = _hidden(nE, hp, T, dev)          # zero padding: the out-edge segment sum reads 16-column vectors
+                act_bwd(gHe, He, nE, h, act=a, act_param=ap, dZ=dYe)                  # dY_e = g_e * tau'(H_e), caller order
+                wgrad_tc(dYe, Xe, nE, h, d_e + h, dWeo)
+                if dbeo is not None:
+                    column_sum(dYe, nE, h, dbeo)
+                WeoT = pack_weight_tc(Weo[:, d_e:], transpose=True)
+                if kind == "bond":
+                    # dZ^{T-1}[inv_perm[e]] = ((dY_e . W_eo[:, d_e:])[e] + dM_v[dst(e)]) * tau'(H^{T-1}[inv_perm[e]])
+                    dst_e = mab_tables(lay)[0]
+
+                    def entry(dMv, Y, from_preact, out):
+                        linear_tc_rows(dYe, h, WeoT, h, out, R=nE, act=a, act_param=ap, Y=Y, from_preact=from_preact,
+                                       out_row=lay.inv_perm, res=dMv, res_row=dst_e if dMv is not None else None)
+                else:
+                    # atom v receives sum_{src(e)=v} dY_e[e] . W_eo[:, d_e:] = (sum_{src(e)=v} dY_e[e]) . W_eo[:, d_e:]: the
+                    # sum over v's out-edges first (segment sum over the in-edges r of v, read through perm[rev[r]]), then a
+                    # V-row GEMM whose epilogue adds the read-out's term and applies tau'
+                    Se = _empty_hidden(nV, hp, T, dev)
+                    segment_sum(dYe, lay.rowptr, nV, h, Se, idx=mab_tables(lay)[2], pad_to=hc)
+
+                    def entry(dHa, Y, from_preact, out):
+                        linear_tc_rows(Se, h, WeoT, h, out, R=nV, act=a, act_param=ap, Y=Y, from_preact=from_preact, res=dHa)
+        gv = gHv if Wvo is not None else None
+        nb = ctx.has_bias[:3]
+        if gv is None and entry is None:
+            # nothing reaches the depth loop (edge-only module on a batch without edges)
+            z = lambda w, b: (torch.zeros_like(w), torch.zeros(w.shape[0], **f32) if b else None)  # noqa: E731
+            (dWi, dbi), (dWh, dbh) = z(Wi, nb[0]), z(Wh, nb[1])
+            dWvo = dbvo = None
+        elif kind == "bond":
+            dWi, dbi, dWh, dbh, dWvo, dbvo = bond_backward_tc(lay, V, E, Wi, Wh, Wvo, cfg, ctx.saved, gv, nb, entry=entry)
+        else:
+            bwd = atom_backward_fused if ctx.saved.get("fused") else atom_backward_tc
+            dWi, dbi, dWh, dbh, dWvo, dbvo = bwd(lay, V, E, Wi, Wh, Wvo, cfg, ctx.saved, gv, nb, entry=entry)
+        d0, d1, d2, d3 = ctx.wdtypes
+        cast = lambda g, d: None if (g is None or d is None) else g.to(d)  # noqa: E731
+        return (None, None, cast(dWi, d0), cast(dbi, d0), cast(dWh, d1), cast(dbh, d1), cast(dWvo, d2), cast(dbvo, d2),
+                cast(dWeo, d3), cast(dbeo, d3), None, None, None)
 
 
 # ----------------------------------------------------------------------------------------------

@@ -310,6 +310,21 @@ int dmpnn_pack_weight_tc(const float* W, int64_t ldw, int64_t N, int64_t K, int 
 int dmpnn_linear_tc_bf16(const void* A, int64_t lda, int64_t R, int64_t K, const void* Wpk, int64_t N,
                          const float* bias, const void* res, int64_t ldres, int act, float act_param,
                          void* C, int64_t ldc, void* stream);
+/* The same kernel with the epilogues of the per-atom / per-edge read-outs (mol-atom-bond message passing), acc = A[r, 0:K] . B^T:
+ *   forward mode (Y == NULL):  C[r, 0:N] = act(acc + bias), stored as out_dtype.  DMPNN_F32: columns [0, N) only,
+ *                              ldc >= N and even, C 8-byte aligned; DMPNN_BF16: as dmpnn_linear_tc_bf16 (ldc >= pad16(N)).
+ *                              out_row, res, res_row must be NULL and from_preact 0.
+ *   mirror mode (Y != NULL):   with q = out_row[r] and s = res_row[r] (identity where the map is NULL),
+ *                              C[q, 0:N] = (acc + res[s, 0:N]) * tau'(Y[q, 0:N]), bf16, columns [N, pad16(N)) zeroed;
+ *                              tau' of `act` evaluated from the activation output Y, or from the pre-activation when
+ *                              from_preact != 0.  res nullable.  Y, res, C bf16 with ld >= pad16(N), ld % 8 == 0, 16-byte
+ *                              aligned; bias must be NULL; C may not alias A, Y or res.  out_row must not repeat a row
+ *                              (rows of C not named by it are left as they are); res_row may.
+ * A and Wpk as for dmpnn_linear_tc_bf16; K <= 448, N <= 304. */
+int dmpnn_linear_tc_rows_bf16(const void* A, int64_t lda, int64_t R, int64_t K, const void* Wpk, int64_t N,
+                              const float* bias, int act, float act_param, const void* Y, int64_t ldy, int from_preact,
+                              const int32_t* out_row, const void* res, int64_t ldres, const int32_t* res_row,
+                              void* C, int out_dtype, int64_t ldc, void* stream);
 
 /* Autograd mirror of one depth step on the same fused kernel (gather-by-rev mode):
  *   dOut[e] = ( sum_{e'' : src(e'') = dst(e)} dM[e''] - dM[rev(e)] ) * tau'(Yact[e]),   dM = dZ . W_h
@@ -346,7 +361,10 @@ int dmpnn_tiles_build(const int32_t* mol_atom_ptr, const int32_t* mol_row_ptr, i
  * with atom_limit = 128) and *n_tiles_dev tiles (device scalar; n_tiles_max only sizes the checks).  Every molecule must
  * have <= 128 atoms.  N_out (first step only): the gathered operand, for the W_h gradient.  The mirror:
  *   dOut[v] = ( (sum_{e in in(v)} dZ[src(e)]) . W ) * act'(Yact[v])      (the adjacency is symmetric)
- * with the modes of dmpnn_bond_step_bwd_fused_bf16 (Yact null: no mask; y_is_preact + addends: the last step). */
+ * with the modes of dmpnn_bond_step_bwd_fused_bf16 (Yact null: no mask; y_is_preact + addends: the last step).
+ * KNOWN ISSUE: the unmasked mode (Yact null) of this ATOM entry point gave NaN gradients on condensed-reaction batches
+ * (~80-atom molecules, h = 300) on the H100, cause not found; no caller in this library uses it -- do not rely on it.
+ * The masked modes, and the unmasked mode of dmpnn_bond_step_bwd_fused_bf16, are exercised by the test-suite. */
 int dmpnn_atom_step_fused_bf16(const void* H_prev, const void* H_0, void* H_next, int64_t ld, int64_t n_rows_alloc, int64_t h,
                                const void* Wpk, const float* bias, const int32_t* rowptr, const int32_t* nbr_row,
                                const int32_t* tile_atom_ptr, const int32_t* tile_edge_ptr, const int32_t* n_tiles_dev,
