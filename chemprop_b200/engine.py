@@ -1617,6 +1617,10 @@ def atom_backward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tenso
             gHv = gHv.contiguous()
         dY = _empty_hidden(nV, hp, T, dev)
         act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)
+        if hc > h:
+            # act_bwd writes h columns; the fused mirror below reads dY up to pad16(h), where a NaN left by the allocator
+            # would reach every output column through the zero rows of the packed weight (0 * NaN = NaN)
+            dY[:, h:hc].zero_()
         dvp = saved.get("dvp", d_v)
         oc = saved.get("ones_col")
         if dbo is not None and oc is not None:

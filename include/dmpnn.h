@@ -287,6 +287,9 @@ int dmpnn_act_bwd(const void* G, int g_dtype, int64_t ldg, const int32_t* gidx,
  * <= 128 rows, DMPNN_FLAG_REV_INVOLUTION.  Returns <0 (and does nothing) otherwise.
  * M_out (nullable; first_step only; bf16, same ld, 32-byte aligned, ld % 16 == 0): also stores the message
  * M^1[e] (mixins.py:11-18) that the step consumed, saved for the W_h gradient instead of being recomputed.
+ * Precondition: columns [h, pad16(h)) of every hidden input (H_prev, H_0) are zero (finite).  The kernel reads them (its TMA
+ * boxes span pad16(h) columns, the epilogue reads H_0 words there) and multiplies them by the zero rows of the packed weight:
+ * a NaN or Inf there makes the whole output row NaN.  Columns [h, pad16(h)) of H_next are written as tau(H_0 there), i.e. zero.
  * ------------------------------------------------------------------------------------- */
 /* ---------------------------------------------------------------------------------------
  * Tensor-core linear layers of the bf16 tier (wgmma / TMA), for the GEMMs outside the fused
@@ -335,7 +338,8 @@ int dmpnn_linear_tc_rows_bf16(const void* A, int64_t lda, int64_t R, int64_t K, 
  * before the single rounding, so that step writes dH_0 = dZ^{T-1} + .. + dZ^1 + dH^0 * tau'(H_0) directly.
  * G_out (nullable, bf16, same ld, 32-byte aligned, ld % 16 == 0): also writes the gathered operand G = (S.P) dZ, so
  * that the W_h gradient of this step is the plain GEMM dW_h += G^T . H^{t-1} (dZ^T . M^t == ((S.P) dZ)^T . H^{t-1}).
- * Same size / layout requirements as dmpnn_bond_step_fused_bf16. */
+ * Same size / layout requirements as dmpnn_bond_step_fused_bf16, and the same precondition: columns [h, pad16(h)) of every
+ * hidden input (dZ, Yact, add0, add1) are zero (finite).  Columns [h, pad16(h)) of dOut are written as zeros. */
 int dmpnn_bond_step_bwd_fused_bf16(const void* dZ, const void* Yact, void* dOut, int64_t ld, int64_t n_rows_alloc,
                                    int64_t h, const void* WpkT, const int32_t* rowptr, const int32_t* rev_row,
                                    const int32_t* tile_row_ptr, const int32_t* tile_atom_ptr, int64_t n_tiles,
@@ -362,9 +366,11 @@ int dmpnn_tiles_build(const int32_t* mol_atom_ptr, const int32_t* mol_row_ptr, i
  * have <= 128 atoms.  N_out (first step only): the gathered operand, for the W_h gradient.  The mirror:
  *   dOut[v] = ( (sum_{e in in(v)} dZ[src(e)]) . W ) * act'(Yact[v])      (the adjacency is symmetric)
  * with the modes of dmpnn_bond_step_bwd_fused_bf16 (Yact null: no mask; y_is_preact + addends: the last step).
- * KNOWN ISSUE: the unmasked mode (Yact null) of this ATOM entry point gave NaN gradients on condensed-reaction batches
- * (~80-atom molecules, h = 300) on the H100, cause not found; no caller in this library uses it -- do not rely on it.
- * The masked modes, and the unmasked mode of dmpnn_bond_step_bwd_fused_bf16, are exercised by the test-suite. */
+ * Both entry points have the precondition of dmpnn_bond_step_fused_bf16: columns [h, pad16(h)) of every hidden input
+ * (H_prev, H_0; dZ, Yact, add0, add1) are zero (finite), else whole output rows come out NaN.
+ * The unmasked mode (Yact null) once gave NaN gradients on condensed-reaction batches (~80-atom molecules, h = 300), not at
+ * h = 64.  That is this precondition broken: on 40 such graphs at h = 300 it gives no NaN with zero padding and a NaN in
+ * every row with NaN in columns [300, 304); h = 64 has no padding column.  All modes are tested (DESIGN.md section 9). */
 int dmpnn_atom_step_fused_bf16(const void* H_prev, const void* H_0, void* H_next, int64_t ld, int64_t n_rows_alloc, int64_t h,
                                const void* Wpk, const float* bias, const int32_t* rowptr, const int32_t* nbr_row,
                                const int32_t* tile_atom_ptr, const int32_t* tile_edge_ptr, const int32_t* n_tiles_dev,

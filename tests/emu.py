@@ -347,7 +347,7 @@ def _sibling_sum_packed(f, lay, through_rev):
         x = x + (x >= r).long()
         ok = (k < d - 1) & (d <= 4)
         x = torch.where(ok, x, r)
-        vals.append(rd[x] * ok.unsqueeze(1).to(f.dtype))
+        vals.append(torch.where(ok.unsqueeze(1), rd[x], 0.0))      # an absent slot is +0, its row is not read
     small = _bf(_bf(vals[0] + vals[1]) + vals[2])
     big = d > 4
     if bool(big.any()):
@@ -356,43 +356,59 @@ def _sibling_sum_packed(f, lay, through_rev):
     return small
 
 
+def _pad16(h):
+    return (h + 15) // 16 * 16
+
+
+def _mma(A, Wpk, h):
+    """A[:, :pad16(h)] . B^T with B = Wpk [h x h] zero-padded to pad16(h) x pad16(h) (k_pack_weight), as the kernel's MMA sees
+    it: columns [0, h) are A[:, :h] . Wpk^T and columns [h, pad16(h)) zero, except that a NaN or Inf anywhere in a row of A
+    makes the whole result row NaN (0 * NaN = 0 * Inf = NaN)."""
+    out = torch.zeros((A.shape[0], _pad16(h)))
+    out[:, :h] = A[:, :h] @ Wpk.t()
+    out[~torch.isfinite(A).all(1)] = float("nan")
+    return out
+
+
+# The fused-step emulations below read the columns the kernel reads: input rows [0, pad16(h)) (its TMA boxes span pad16(h)
+# columns; the FAR windows' global gathers read the same 16-column blocks) and the epilogue's H_0 / Y / addend words in
+# [h, pad16(h)), and they produce the output's padding columns the way each mode does: FWD tau(H_0 + 0), MASK 0 * tau'(Y),
+# LAST 0 * tau'(H_0) + addends, COPY 0 -- all zero when the inputs' padding is, NaN rows when it is not.
 def bond_step_fused(H_prev, H0, H_next, h, Wpk, bias, lay, act, act_param, first_step, M_out=None, drop_bits=None,
                     drop_scale=1.0):
     """H_next[e] = tau(H_0[e] + b + W_h . M[e]),  M = message of g(H_prev), g = tau on the first step (include/dmpnn.h)."""
-    f = _act(H_prev.float()[: lay.E, :h], act if first_step else ACT_NONE, act_param)
+    hp = _pad16(h)
+    f = _act(H_prev.float()[: lay.E, :hp], act if first_step else ACT_NONE, act_param)
     if first_step:
         f = _bf(f)                                    # act_word: tau applied to the bf16 word, result a bf16 word
     A = _sibling_sum_packed(f, lay, through_rev=False)     # A row r is the message of edge rev(r)
-    M = torch.zeros((lay.E, h))
+    M = torch.zeros((lay.E, hp))
     M[lay.rev_row.long()] = A
-    Z = M @ Wpk.t() + H0[: lay.E, :h].float()
+    Z = _mma(M, Wpk, h) + H0[: lay.E, :hp].float()
     if bias is not None:
-        Z = Z + bias.float()
+        Z[:, :h] = Z[:, :h] + bias.float()          # the kernel's bias is zero past h
     Y = _act(Z, act, act_param)
     if drop_bits is not None:           # keep ? tau(z) * scale : 0 in f32, one rounding (the kernel's epilogue)
-        nj = (h + 15) // 16
+        nj = hp // 16
         keep = ((drop_bits[: lay.E].to(torch.int32).unsqueeze(-1) >> torch.arange(16, dtype=torch.int32)) & 1).reshape(lay.E, nj * 16)
-        Y = Y * keep[:, :h].float() * drop_scale
-    H_next[: lay.E, :h] = Y.to(H_next.dtype)
-    H_next[: lay.E, h:(h + 15) // 16 * 16] = 0
+        Y = Y * keep.float() * drop_scale
+    H_next[: lay.E, :hp] = Y.to(H_next.dtype)
     if M_out is not None:
-        M_out[: lay.E, :h] = M.to(M_out.dtype)
-        M_out[: lay.E, h:(h + 15) // 16 * 16] = 0
+        M_out[: lay.E, :hp] = M.to(M_out.dtype)
 
 
 def bond_step_bwd_fused(dZ, Yact, dOut, h, WpkT, lay, act, act_param, G_out=None, y_is_preact=False, addends=()):
     """dOut = ((S.P) dZ) . W_h [* tau'(Yact)] [+ addends];  G_out = (S.P) dZ   (WpkT holds B = W_h^T of A . B^T)."""
-    G = _sibling_sum_packed(dZ.float()[: lay.E, :h], lay, through_rev=True)
-    D = G @ WpkT.t()
+    hp = _pad16(h)
+    G = _sibling_sum_packed(dZ.float()[: lay.E, :hp], lay, through_rev=True)
+    D = _mma(G, WpkT, h)
     if Yact is not None:
-        D = D * _dact(Yact[: lay.E, :h].float(), act, act_param, y_is_preact)
+        D = D * _dact(Yact[: lay.E, :hp].float(), act, act_param, y_is_preact)
     for a in addends:
-        D = D + a[: lay.E, :h].float()
-    dOut[: lay.E, :h] = D.to(dOut.dtype)
-    dOut[: lay.E, h:(h + 15) // 16 * 16] = 0
+        D = D + a[: lay.E, :hp].float()
+    dOut[: lay.E, :hp] = D.to(dOut.dtype)
     if G_out is not None:
-        G_out[: lay.E, :h] = G.to(G_out.dtype)
-        G_out[: lay.E, h:(h + 15) // 16 * 16] = 0
+        G_out[: lay.E, :hp] = G.to(G_out.dtype)
 
 
 def atom_tables(lay):
@@ -413,7 +429,7 @@ def _neighbour_sum_packed(f, lay):
     for k in range(4):
         ok = (k < d) & (d <= 4)
         x = torch.where(ok, src[torch.clamp(g0 + k, max=max(lay.E - 1, 0))], r)
-        vals.append(f[x] * ok.unsqueeze(1).to(f.dtype))
+        vals.append(torch.where(ok.unsqueeze(1), f[x], 0.0))
     small = _bf(_bf(_bf(vals[0] + vals[1]) + vals[2]) + vals[3])
     big = d > 4
     if bool(big.any()):
@@ -424,33 +440,29 @@ def _neighbour_sum_packed(f, lay):
 
 def atom_step_fused(H_prev, H0, H_next, h, Wpk, bias, lay, act, act_param, first_step, N_out=None):
     """H_next[v] = tau(H0[v] + b + W . N[v]),  N = neighbour sum of g(H_prev), g = tau on the first step (include/dmpnn.h)."""
-    V = lay.V
-    f = _act(H_prev.float()[:V, :h], act if first_step else ACT_NONE, act_param)
+    V, hp = lay.V, _pad16(h)
+    f = _act(H_prev.float()[:V, :hp], act if first_step else ACT_NONE, act_param)
     if first_step:
         f = _bf(f)
     N = _neighbour_sum_packed(f, lay)
-    Z = N @ Wpk.t() + H0[:V, :h].float()
+    Z = _mma(N, Wpk, h) + H0[:V, :hp].float()
     if bias is not None:
-        Z = Z + bias.float()
-    H_next[:V, :h] = _act(Z, act, act_param).to(H_next.dtype)
-    H_next[:V, h:(h + 15) // 16 * 16] = 0
+        Z[:, :h] = Z[:, :h] + bias.float()
+    H_next[:V, :hp] = _act(Z, act, act_param).to(H_next.dtype)
     if N_out is not None:
-        N_out[:V, :h] = N.to(N_out.dtype)
-        N_out[:V, h:(h + 15) // 16 * 16] = 0
+        N_out[:V, :hp] = N.to(N_out.dtype)
 
 
 def atom_step_bwd_fused(dZ, Yact, dOut, h, WpkT, lay, act, act_param, G_out=None, y_is_preact=False):
     """dOut = (A dZ) . W [* tau'(Yact)];  G_out = A dZ   (WpkT holds B = W^T of A . B^T)."""
-    V = lay.V
-    G = _neighbour_sum_packed(dZ.float()[:V, :h], lay)
-    D = G @ WpkT.t()
+    V, hp = lay.V, _pad16(h)
+    G = _neighbour_sum_packed(dZ.float()[:V, :hp], lay)
+    D = _mma(G, WpkT, h)
     if Yact is not None:
-        D = D * _dact(Yact[:V, :h].float(), act, act_param, y_is_preact)
-    dOut[:V, :h] = D.to(dOut.dtype)
-    dOut[:V, h:(h + 15) // 16 * 16] = 0
+        D = D * _dact(Yact[:V, :hp].float(), act, act_param, y_is_preact)
+    dOut[:V, :hp] = D.to(dOut.dtype)
     if G_out is not None:
-        G_out[:V, :h] = G.to(G_out.dtype)
-        G_out[:V, h:(h + 15) // 16 * 16] = 0
+        G_out[:V, :hp] = G.to(G_out.dtype)
 
 
 def bond_message_bwd_masked(dM, Yact, lay, Ccols, out, *, act, act_param=0.0):
