@@ -7,10 +7,10 @@
 //
 // Persistent, warp-specialised, one CTA per SM, molecule-aligned tiles of <=128 dst-sorted edge rows:
 //   warp 0      TMA producer: H tile (5 boxes of 128 rows x 64 cols, SWIZZLE_128B) -> one shared-memory tile, handed
-//               over slab by slab (box s of the next tile is loaded when the message warps have left slab s); L2 prefetch
+//               over slab by slab (box s of the next tile is loaded when the message warps have left slab s)
 //   warp 1      TMA producer: W_h stages (pre-packed smem images, cp.async.bulk): an 80-column output chunk x one
 //               k pass (slabs {0,1,2} | {3,4}), 2-stage ring of 30 KB
-//   warp 3      L2 prefetch of the next tile's H_0 rows (and of the backward addends)
+//   warp 3      L2 prefetch of the backward addends (MODE_BWD_LAST)
 //   warps 4-11  two warpgroups, tile rows [0, 64) / [64, 128): wgmma m64n80k16, D (registers, fp32) = A (smem, bf16)
 //               . W_h^T (smem), chunk by chunk, then the epilogue from registers: + H_0 + bias -> tau -> bf16 -> HBM
 //   warps 12-19 message: thread = row e': sums the sibling rows of e' (same destination atom) out of the
@@ -148,10 +148,8 @@ static int launch_step(const char* what, const void* H_prev, const void* H_0, vo
   if (n_tiles == 0) return 0;
   EncodeTiledFn enc = get_encode_fn();
   DMPNN_CHECK_ARG(enc != nullptr, "%s: cuTensorMapEncodeTiled not available from the driver", what);
-  CUtensorMap mH, mH0;
-  DMPNN_CHECK_ARG(encode_rows_map(enc, &mH, H_prev, hp, n_rows_alloc, ld) &&
-                      encode_rows_map(enc, &mH0, H_0 ? H_0 : H_prev, hp, n_rows_alloc, ld),
-                  "%s: cuTensorMapEncodeTiled failed", what);
+  CUtensorMap mH;
+  DMPNN_CHECK_ARG(encode_rows_map(enc, &mH, H_prev, hp, n_rows_alloc, ld), "%s: cuTensorMapEncodeTiled failed", what);
 
   PackGeom g = pack_geom(h, h);
   Params p;
@@ -202,13 +200,13 @@ static int launch_step(const char* what, const void* H_prev, const void* H_0, vo
   const bool far = work_flag != nullptr;
   cudaError_t e;
   if (atom)
-    e = mode == MODE_FWD ? dispatch_fwd<false, true>(act, first_step != 0, bias != nullptr, false, grid, st, mH, mH0, p)
-                         : dispatch_bwd<false, true>(mode, act, grid, st, mH, mH0, p);
+    e = mode == MODE_FWD ? dispatch_fwd<false, true>(act, first_step != 0, bias != nullptr, false, grid, st, mH, p)
+                         : dispatch_bwd<false, true>(mode, act, grid, st, mH, p);
   else if (mode == MODE_FWD)
-    e = far ? dispatch_fwd<true>(act, first_step != 0, bias != nullptr, drop_bits != nullptr, grid, st, mH, mH0, p)
-            : dispatch_fwd<false>(act, first_step != 0, bias != nullptr, drop_bits != nullptr, grid, st, mH, mH0, p);
+    e = far ? dispatch_fwd<true>(act, first_step != 0, bias != nullptr, drop_bits != nullptr, grid, st, mH, p)
+            : dispatch_fwd<false>(act, first_step != 0, bias != nullptr, drop_bits != nullptr, grid, st, mH, p);
   else
-    e = far ? dispatch_bwd<true>(mode, act, grid, st, mH, mH0, p) : dispatch_bwd<false>(mode, act, grid, st, mH, mH0, p);
+    e = far ? dispatch_bwd<true>(mode, act, grid, st, mH, p) : dispatch_bwd<false>(mode, act, grid, st, mH, p);
   DMPNN_CHECK_ARG(!(drop_bits != nullptr && act != DMPNN_ACT_RELU), "%s: dropout in the epilogue is built for ReLU only", what);
   DMPNN_CHECK_ARG(e == cudaSuccess, "%s: cannot configure %d B dynamic smem: %s", what, kSmemAlloc, cudaGetErrorString(e));
   DMPNN_CHECK_LAUNCH(what, 1);

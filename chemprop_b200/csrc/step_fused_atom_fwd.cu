@@ -4,6 +4,6 @@
 
 namespace dmpnn {
 namespace fused {
-template cudaError_t dispatch_fwd<false, true>(int, bool, bool, bool, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&, const Params&);
+template cudaError_t dispatch_fwd<false, true>(int, bool, bool, bool, int, cudaStream_t, const CUtensorMap&, const Params&);
 }  // namespace fused
 }  // namespace dmpnn

@@ -3,6 +3,6 @@
 
 namespace dmpnn {
 namespace fused {
-template cudaError_t dispatch_bwd<true>(int, int, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&, const Params&);
+template cudaError_t dispatch_bwd<true>(int, int, int, cudaStream_t, const CUtensorMap&, const Params&);
 }  // namespace fused
 }  // namespace dmpnn

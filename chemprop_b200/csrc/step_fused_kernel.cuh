@@ -128,7 +128,7 @@ enum { MODE_FWD = 0, MODE_BWD_MASK = 1, MODE_BWD_COPY = 2, MODE_BWD_LAST = 3 };
 // is two directed edges), so the autograd mirror is the same gather applied to dZ.  Everything after the gather is shared.
 template <int ACT, bool FIRST, bool HAS_BIAS, int MODE, bool FAR, bool DROP, bool ATOM = false>
 __global__ void __launch_bounds__(kThreads, 1)
-k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_constant__ CUtensorMap tmapH0, Params p) {
+k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, Params p) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment as an OFFSET from the shared-memory symbol (not through a uintptr_t round trip): the compiler keeps
   // the address space, so the row-pointer / rev() table look-ups of the message warps are LDS instead of generic LD.E
@@ -166,13 +166,15 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
 
   if (warp == 0) {
     // ===================== TMA producer: H_prev tile -> shared memory (single buffer) =====================
+    // No L2 prefetch of the next tile's rows (nor of its H_0 rows in warp 3): both made the step slower on an H100 at
+    // h = 300 (DESIGN.md 7).  The H_0 prefetch had no barrier to pace it, so it ran through all of a CTA's tiles at the
+    // start of the launch, far more rows than L2 holds.
     int it = 0;
     int row_carry = (int)blockIdx.x < n_items ? __ldg(p.tile_row_ptr + blockIdx.x) : 0;   // the next tile's first row, loaded a tile ahead
     for (int t = blockIdx.x; t < n_items; t += gridDim.x, ++it) {
       const int row0 = row_carry;
       const int t2 = t + gridDim.x;
-      const int row2 = (t2 < n_items && !(p.exp_flags & 2048)) ? __ldg(p.tile_row_ptr + t2) : -1;
-      if (t2 < n_items) row_carry = (p.exp_flags & 2048) ? __ldg(p.tile_row_ptr + t2) : row2;
+      if (t2 < n_items) row_carry = __ldg(p.tile_row_ptr + t2);
       // slab s of this tile is loaded as soon as the message warps have left slab s of the previous tile: the load
       // of the leading slabs overlaps the gather of the trailing ones (one shared-memory tile, no exposed latency)
       for (int s = 0; s < p.nslab; ++s) {
@@ -184,9 +186,6 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
         }
         __syncwarp();
       }
-      if (row2 >= 0 && elect_one())
-        for (int s = 0; s < p.nslab; ++s) tma_prefetch_2d(&tmapH, s * 64, row2);   // next tile -> L2
-      __syncwarp();
     }
   } else if (warp == 1) {
     // ===================== TMA producer: W_h stages (pre-packed smem images) =====================
@@ -215,18 +214,12 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
         }
     }
   } else if (warp == 3) {
-    // ===================== L2 prefetch of the epilogue's row streams, one tile ahead ==========
-    int row_n = (int)(blockIdx.x + gridDim.x) < n_items ? __ldg(p.tile_row_ptr + blockIdx.x + gridDim.x) : -1;
-    for (int t = blockIdx.x; MODE != MODE_BWD_COPY && t < n_items; t += gridDim.x) {
-      const int tn = t + gridDim.x;
-      const int rown = (tn < n_items && !(p.exp_flags & 2048)) ? row_n : -1;
-      row_n = (tn + (int)gridDim.x < n_items) ? __ldg(p.tile_row_ptr + tn + gridDim.x) : -1;
-      if (rown >= 0 && elect_one())
-        for (int s = 0; s < p.nslab; ++s) tma_prefetch_2d(&tmapH0, s * 64, rown);
-      __syncwarp();
-      if (MODE == MODE_BWD_LAST && p.add0 != nullptr) {
+    // ===================== L2 prefetch of the backward addends (MODE_BWD_LAST) ==========
+    for (int t = blockIdx.x; MODE == MODE_BWD_LAST && t < n_items; t += gridDim.x) {
+      if (p.add0 != nullptr) {
         // the epilogue of this tile reads the addend rows with plain loads: pull them into L2 now (the rows of a
-        // tile are one contiguous byte range; this warp runs ahead of the epilogue)
+        // tile are one contiguous byte range).  Nothing paces this warp: it runs ahead of the epilogue by as many tiles
+        // as it gets to
         const int row0 = __ldg(p.tile_row_ptr + t);
         const int nr = __ldg(p.tile_row_ptr + t + 1) - row0;
         const int64_t lines = ((int64_t)nr * p.ld * 2 + 127) >> 7;
@@ -243,7 +236,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
     // D[64 x 80] (registers, fp32) = A (shared memory, written by the message warps) . W_h^T (W stage) per 80-column chunk;
     // the epilogue of a chunk runs from registers right after its last k pass.  The message warps build A row r as the
     // message of edge r itself (they gather through the tile-local rev() table), so accumulator row r is the update of
-    // edge r: it needs H_0 row r (global memory; L2-resident, prefetched a tile ahead by warp 3) and produces output row r.
+    // edge r: it needs H_0 row r (global memory, requested before the chunk's last wgmma group is waited for) and produces output row r.
     // W rows past a chunk's last column may hold the next slab's rows or stale data: they only reach accumulator columns
     // that the epilogue never stores.
     const int wg = (warp - 4) >> 2;
@@ -660,7 +653,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, const __grid_consta
 
 
 template <int ACT, bool FIRST, bool HAS_BIAS, int MODE, bool FAR, bool DROP, bool ATOM = false>
-static cudaError_t launch_variant(int grid, cudaStream_t st, const CUtensorMap& mH, const CUtensorMap& mH0, const Params& p) {
+static cudaError_t launch_variant(int grid, cudaStream_t st, const CUtensorMap& mH, const Params& p) {
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(k_bond_step_fused<ACT, FIRST, HAS_BIAS, MODE, FAR, DROP, ATOM>,
@@ -668,19 +661,18 @@ static cudaError_t launch_variant(int grid, cudaStream_t st, const CUtensorMap& 
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  k_bond_step_fused<ACT, FIRST, HAS_BIAS, MODE, FAR, DROP, ATOM><<<grid, kThreads, kSmemAlloc, st>>>(mH, mH0, p);
+  k_bond_step_fused<ACT, FIRST, HAS_BIAS, MODE, FAR, DROP, ATOM><<<grid, kThreads, kSmemAlloc, st>>>(mH, p);
   return cudaSuccess;
 }
 
 // forward step: every fused activation x first x bias; dropout (keep bits) is a ReLU-only feature (engine.dropout_fused_ok)
 template <bool FAR, bool ATOM = false>
-cudaError_t dispatch_fwd(int act, bool first, bool bias, bool drop, int grid, cudaStream_t st, const CUtensorMap& mH,
-                         const CUtensorMap& mH0, const Params& p) {
+cudaError_t dispatch_fwd(int act, bool first, bool bias, bool drop, int grid, cudaStream_t st, const CUtensorMap& mH, const Params& p) {
 #define DMPNN_FB(A, D)                                                                                              \
-  (first ? (bias ? launch_variant<A, true, true, MODE_FWD, FAR, D, ATOM>(grid, st, mH, mH0, p)                             \
-                 : launch_variant<A, true, false, MODE_FWD, FAR, D, ATOM>(grid, st, mH, mH0, p))                            \
-         : (bias ? launch_variant<A, false, true, MODE_FWD, FAR, D, ATOM>(grid, st, mH, mH0, p)                            \
-                 : launch_variant<A, false, false, MODE_FWD, FAR, D, ATOM>(grid, st, mH, mH0, p)))
+  (first ? (bias ? launch_variant<A, true, true, MODE_FWD, FAR, D, ATOM>(grid, st, mH, p)                             \
+                 : launch_variant<A, true, false, MODE_FWD, FAR, D, ATOM>(grid, st, mH, p))                            \
+         : (bias ? launch_variant<A, false, true, MODE_FWD, FAR, D, ATOM>(grid, st, mH, p)                            \
+                 : launch_variant<A, false, false, MODE_FWD, FAR, D, ATOM>(grid, st, mH, p)))
   if (drop) {
     if constexpr (ATOM) return cudaErrorInvalidValue;
     else return act == DMPNN_ACT_RELU ? DMPNN_FB(DMPNN_ACT_RELU, true) : cudaErrorInvalidValue;
@@ -697,12 +689,12 @@ cudaError_t dispatch_fwd(int act, bool first, bool bias, bool drop, int grid, cu
 }
 
 template <bool FAR, bool ATOM = false>
-cudaError_t dispatch_bwd(int mode, int act, int grid, cudaStream_t st, const CUtensorMap& mH, const CUtensorMap& mH0,
+cudaError_t dispatch_bwd(int mode, int act, int grid, cudaStream_t st, const CUtensorMap& mH,
                          const Params& p) {
-  if (mode == MODE_BWD_COPY) return launch_variant<DMPNN_ACT_NONE, false, false, MODE_BWD_COPY, FAR, false, ATOM>(grid, st, mH, mH0, p);
+  if (mode == MODE_BWD_COPY) return launch_variant<DMPNN_ACT_NONE, false, false, MODE_BWD_COPY, FAR, false, ATOM>(grid, st, mH, p);
 #define DMPNN_BM(A)                                                                                         \
-  (mode == MODE_BWD_LAST ? launch_variant<A, false, false, MODE_BWD_LAST, FAR, false, ATOM>(grid, st, mH, mH0, p)   \
-                         : launch_variant<A, false, false, MODE_BWD_MASK, FAR, false, ATOM>(grid, st, mH, mH0, p))
+  (mode == MODE_BWD_LAST ? launch_variant<A, false, false, MODE_BWD_LAST, FAR, false, ATOM>(grid, st, mH, p)   \
+                         : launch_variant<A, false, false, MODE_BWD_MASK, FAR, false, ATOM>(grid, st, mH, p))
   switch (act) {
     case DMPNN_ACT_NONE: return DMPNN_BM(DMPNN_ACT_NONE);
     case DMPNN_ACT_RELU: return DMPNN_BM(DMPNN_ACT_RELU);
@@ -715,12 +707,12 @@ cudaError_t dispatch_bwd(int mode, int act, int grid, cudaStream_t st, const CUt
 }
 
 // explicit instantiations live in step_fused_{fwd,bwd,far_fwd,far_bwd,atom_fwd,atom_bwd}.cu
-extern template cudaError_t dispatch_fwd<false, true>(int, bool, bool, bool, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&, const Params&);
-extern template cudaError_t dispatch_bwd<false, true>(int, int, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&, const Params&);
-extern template cudaError_t dispatch_fwd<false>(int, bool, bool, bool, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&, const Params&);
-extern template cudaError_t dispatch_fwd<true>(int, bool, bool, bool, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&, const Params&);
-extern template cudaError_t dispatch_bwd<false>(int, int, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&, const Params&);
-extern template cudaError_t dispatch_bwd<true>(int, int, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&, const Params&);
+extern template cudaError_t dispatch_fwd<false, true>(int, bool, bool, bool, int, cudaStream_t, const CUtensorMap&, const Params&);
+extern template cudaError_t dispatch_bwd<false, true>(int, int, int, cudaStream_t, const CUtensorMap&, const Params&);
+extern template cudaError_t dispatch_fwd<false>(int, bool, bool, bool, int, cudaStream_t, const CUtensorMap&, const Params&);
+extern template cudaError_t dispatch_fwd<true>(int, bool, bool, bool, int, cudaStream_t, const CUtensorMap&, const Params&);
+extern template cudaError_t dispatch_bwd<false>(int, int, int, cudaStream_t, const CUtensorMap&, const Params&);
+extern template cudaError_t dispatch_bwd<true>(int, int, int, cudaStream_t, const CUtensorMap&, const Params&);
 
 }  // namespace fused
 }  // namespace dmpnn
