@@ -69,6 +69,7 @@ struct Params {
   const int32_t* out_row;     // nullable: output / Y row of A row r (identity when null)
   const int32_t* res_row;     // nullable: residual row of A row r (identity when null)
   int from_preact;            // Y holds the pre-activation instead of the activation output
+  int f32_v4;                 // kEpiF32: Cf and ldc keep every row 16-byte aligned (whole runs as float4 stores)
 };
 
 template <int ACT, bool HAS_BIAS, int EPI = kEpiBf16>
@@ -137,73 +138,96 @@ k_linear_tc(const __grid_constant__ CUtensorMap tmapA, Params p) {
         acc_fence(acc);
         mbar_arrive(bar(B_EMPTY + st));
       }
-      // epilogue: rows rl, rl + 8 of the tile; columns n0 + 8 b + cl + {0, 1}
+      // epilogue: rows rl, rl + 8 of the tile.  The packed W image permutes the columns of every work item (tc::acc_out_col):
+      // per 32-column group G, this thread's accumulator blocks 4 G, 4 G + 1, ... hold the run of output columns
+      // n0 + acc_out_col(32 G + cl, nc) + [0, run): 8 in a full group, 4 in a 16-column tail, 2 in an 8-column tail
+      // (acc_run_cols).  A 16-column tail followed by an 8-column one (nc = 152 = 4 * 32 + 16 + 8, nc = 56 = 32 + 16 + 8) adds
+      // a second run of 2 from block 4 G + 2.  Word w of a run (columns n, n + 1) comes from accumulator block b0 + w.
+      const int nc = min(kNT, p.Npad - n0);   // columns of this item: all < Npad
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int64_t grow = (int64_t)t * kTileM + rl + 8 * h;
         if (grow >= p.R) continue;
+        __nv_bfloat16* crow = nullptr;
+        float* cfrow = nullptr;
+        const __nv_bfloat16* yrow = nullptr;
+        const __nv_bfloat16* rrow = nullptr;
         if constexpr (EPI == kEpiF32) {
-          float* crow = p.Cf + grow * p.ldc;
-#pragma unroll
-          for (int b = 0; b < kNT / 8; ++b) {
-            const int n = n0 + 8 * b + cl;
-            if (n >= p.N) continue;
-            float z0 = acc[4 * b + 2 * h], z1 = acc[4 * b + 2 * h + 1];
-            if constexpr (HAS_BIAS) { z0 += s_bias[n]; z1 += s_bias[n + 1]; }
-            z0 = act_t<ACT>(p.act_param, z0);
-            z1 = act_t<ACT>(p.act_param, z1);
-            if (n + 1 < p.N) *reinterpret_cast<float2*>(crow + n) = make_float2(z0, z1);
-            else crow[n] = z0;
-          }
-          continue;
-        }
-        if constexpr (EPI == kEpiMirror) {
+          cfrow = p.Cf + grow * p.ldc;
+        } else if constexpr (EPI == kEpiMirror) {
           const int64_t q = p.out_row != nullptr ? (int64_t)__ldg(p.out_row + grow) : grow;
           const int64_t s = p.res_row != nullptr ? (int64_t)__ldg(p.res_row + grow) : grow;
-          __nv_bfloat16* crow = p.C + q * p.ldc;
-          const __nv_bfloat16* yrow = p.Y + q * p.ldy;
-          const __nv_bfloat16* rrow = p.res != nullptr ? p.res + s * p.ldres : nullptr;
-#pragma unroll
-          for (int b = 0; b < kNT / 8; ++b) {
-            const int n = n0 + 8 * b + cl;
-            if (n >= p.Npad) continue;
-            uint32_t o = 0u;                                      // columns [N, pad16(N)) are written as zeros
-            if (n < p.N) {
-              float z0 = acc[4 * b + 2 * h], z1 = acc[4 * b + 2 * h + 1];
-              if (rrow != nullptr) {
-                const uint32_t rw = __ldg(reinterpret_cast<const unsigned int*>(rrow + n));
-                z0 += bf_lo(rw); z1 += bf_hi(rw);
-              }
-              const uint32_t yw = __ldg(reinterpret_cast<const unsigned int*>(yrow + n));
-              if (p.from_preact) {
-                z0 *= act_grad_from_pre(ACT, p.act_param, bf_lo(yw));
-                z1 *= act_grad_from_pre(ACT, p.act_param, bf_hi(yw));
-              } else {
-                z0 *= act_grad_from_out(ACT, p.act_param, bf_lo(yw));
-                z1 *= act_grad_from_out(ACT, p.act_param, bf_hi(yw));
-              }
-              o = pack_bf2(z0, n + 1 < p.N ? z1 : 0.f);
-            }
-            *reinterpret_cast<uint32_t*>(crow + n) = o;
-          }
-          continue;
+          crow = p.C + q * p.ldc;
+          yrow = p.Y + q * p.ldy;
+          rrow = p.res != nullptr ? p.res + s * p.ldres : nullptr;
+        } else {
+          crow = p.C + grow * p.ldc;
+          rrow = p.res != nullptr ? p.res + grow * p.ldres : nullptr;
         }
-        __nv_bfloat16* crow = p.C + grow * p.ldc;
-        const __nv_bfloat16* rrow = p.res != nullptr ? p.res + grow * p.ldres : nullptr;
 #pragma unroll
-        for (int b = 0; b < kNT / 8; ++b) {
-          const int n = n0 + 8 * b + cl;
-          if (n >= p.Npad) continue;
-          float z0 = acc[4 * b + 2 * h], z1 = acc[4 * b + 2 * h + 1];
-          if (rrow != nullptr) {
-            const uint32_t rw = __ldg(reinterpret_cast<const unsigned int*>(rrow + n));
-            z0 += bf_lo(rw); z1 += bf_hi(rw);
+        for (int G = 0; G < (kNT + 31) / 32; ++G) {
+          const int run0 = acc_run_cols(32 * G + cl, nc);
+#pragma unroll
+          for (int part = 0; part < 2; ++part) {
+            const int b0 = 4 * G + 2 * part;     // first accumulator block of the run
+            if (b0 >= kNT / 8) break;
+            const int j = 32 * G + 16 * part + cl;
+            const int run = part == 0 ? run0 : (run0 == 4 ? acc_run_cols(j, nc) : 0);
+            if (run == 0) continue;
+            const int nw = run >> 1;             // bf16x2 words of the run
+            const int n = n0 + acc_out_col(j, nc);
+            uint32_t rw[4] = {0u, 0u, 0u, 0u}, yw[4] = {0u, 0u, 0u, 0u}, o[4] = {0u, 0u, 0u, 0u};
+            float zf[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            if (EPI != kEpiF32 && rrow != nullptr) ld_run(rrow + n, nw, rw);
+            if (EPI == kEpiMirror && n < p.N) ld_run(yrow + n, nw, yw);
+#pragma unroll
+            for (int w = 0; w < 4; ++w) {
+              const int b = b0 + w;
+              if (b >= kNT / 8 || w >= nw) break;
+              const int nn = n + 2 * w;
+              float z0 = acc[4 * b + 2 * h], z1 = acc[4 * b + 2 * h + 1];
+              if constexpr (EPI == kEpiF32) {
+                if constexpr (HAS_BIAS) { z0 += s_bias[nn]; z1 += s_bias[nn + 1]; }
+                zf[2 * w] = act_t<ACT>(p.act_param, z0);
+                zf[2 * w + 1] = act_t<ACT>(p.act_param, z1);
+              } else if constexpr (EPI == kEpiMirror) {
+                if (nn < p.N) {                    // columns [N, pad16(N)) are written as zeros
+                  if (rrow != nullptr) { z0 += bf_lo(rw[w]); z1 += bf_hi(rw[w]); }
+                  if (p.from_preact) {
+                    z0 *= act_grad_from_pre(ACT, p.act_param, bf_lo(yw[w]));
+                    z1 *= act_grad_from_pre(ACT, p.act_param, bf_hi(yw[w]));
+                  } else {
+                    z0 *= act_grad_from_out(ACT, p.act_param, bf_lo(yw[w]));
+                    z1 *= act_grad_from_out(ACT, p.act_param, bf_hi(yw[w]));
+                  }
+                  o[w] = pack_bf2(z0, nn + 1 < p.N ? z1 : 0.f);
+                }
+              } else {
+                if (rrow != nullptr) { z0 += bf_lo(rw[w]); z1 += bf_hi(rw[w]); }
+                if constexpr (HAS_BIAS) { z0 += s_bias[nn]; z1 += s_bias[nn + 1]; }
+                if constexpr (ACT == DMPNN_ACT_RELU) o[w] = act_word<ACT>(pack_bf2(z0, z1), 0.f);
+                else o[w] = pack_bf2(act_t<ACT>(p.act_param, z0), act_t<ACT>(p.act_param, z1));
+              }
+            }
+            if constexpr (EPI == kEpiF32) {
+              // f32 columns [0, N) only: whole 16-byte stores where the run lies below N and the rows are 16-byte aligned
+              if (p.f32_v4 && n + run <= p.N && nw >= 2) {
+                float4* dst = reinterpret_cast<float4*>(cfrow + n);
+                dst[0] = make_float4(zf[0], zf[1], zf[2], zf[3]);
+                if (nw == 4) dst[1] = make_float4(zf[4], zf[5], zf[6], zf[7]);
+              } else {
+#pragma unroll
+                for (int w = 0; w < 4; ++w) {
+                  const int nn = n + 2 * w;
+                  if (w >= nw || nn >= p.N) break;
+                  if (nn + 1 < p.N) *reinterpret_cast<float2*>(cfrow + nn) = make_float2(zf[2 * w], zf[2 * w + 1]);
+                  else cfrow[nn] = zf[2 * w];
+                }
+              }
+            } else {
+              st_run(crow + n, nw, o);
+            }
           }
-          if constexpr (HAS_BIAS) { z0 += s_bias[n]; z1 += s_bias[n + 1]; }
-          uint32_t o;
-          if constexpr (ACT == DMPNN_ACT_RELU) o = act_word<ACT>(pack_bf2(z0, z1), 0.f);
-          else o = pack_bf2(act_t<ACT>(p.act_param, z0), act_t<ACT>(p.act_param, z1));
-          *reinterpret_cast<uint32_t*>(crow + n) = o;
         }
       }
     }
@@ -222,13 +246,16 @@ __host__ __device__ inline PackGeom pack_geom(int64_t N, int64_t K) {
   g.nslab = (g.Kpad + 63) / 64;
   return g;
 }
-// B[n][k] = transpose ? W[k][n] : W[n][k]   (W row-major with row stride ldw)
+// B[n][k] = transpose ? W[k][n] : W[n][k]   (W row-major with row stride ldw).  Inside each 152-row work item, image row
+// 152 i + j holds B row 152 i + acc_out_col(j, nc_i) (tc_common.cuh), so that the epilogue's fragments are column runs.
 __global__ void k_pack_weight_tc(const float* __restrict__ W, int64_t ldw, int transpose, PackGeom g,
                                  __nv_bfloat16* __restrict__ out) {
-  const int n = blockIdx.x;  // 0 .. Npad-1
+  const int r = blockIdx.x;  // image row, 0 .. Npad-1
+  const int n0 = r / kNT * kNT;
+  const int n = n0 + acc_out_col(r - n0, min(kNT, g.Npad - n0));   // the B row (output column) it holds; zero at n >= N
   for (int k = threadIdx.x; k < g.nslab * 64; k += blockDim.x) {
     const int s = k >> 6, kl = k & 63;
-    const size_t off = (size_t)s * g.Npad * 128 + (size_t)(n >> 3) * 1024 + (n & 7) * 128 + (((kl >> 3) ^ (n & 7)) << 4) + (kl & 7) * 2;
+    const size_t off = (size_t)s * g.Npad * 128 + (size_t)(r >> 3) * 1024 + (r & 7) * 128 + (((kl >> 3) ^ (r & 7)) << 4) + (kl & 7) * 2;
     float v = 0.f;
     if (n < g.N && k < g.K) v = transpose ? W[(int64_t)k * ldw + n] : W[(int64_t)n * ldw + k];
     out[off >> 1] = __float2bfloat16_rn(v);
@@ -340,6 +367,10 @@ extern "C" int dmpnn_linear_tc_bf16(const void* A, int64_t lda, int64_t R, int64
   p.n_tiles = (int)((R + kTileM - 1) / kTileM);
   p.n_nt = (g.Npad + kNT - 1) / kNT;
   p.act_param = act_param;
+  p.Cf = nullptr;
+  p.Y = nullptr;
+  p.out_row = p.res_row = nullptr;
+  p.from_preact = p.f32_v4 = 0;
   const int items = p.n_tiles * p.n_nt;
   const int sms = sm_count_cached();
   const int grid = items < sms ? items : sms;
@@ -424,6 +455,7 @@ extern "C" int dmpnn_linear_tc_rows_bf16(const void* A, int64_t lda, int64_t R, 
   p.out_row = out_row;
   p.res_row = res_row;
   p.from_preact = from_preact ? 1 : 0;
+  p.f32_v4 = out_dtype == DMPNN_F32 && (reinterpret_cast<uintptr_t>(Cout) & 15) == 0 && ldc % 4 == 0;
   const int items = p.n_tiles * p.n_nt;
   const int sms = sm_count_cached();
   const int grid = items < sms ? items : sms;

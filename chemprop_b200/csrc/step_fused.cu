@@ -30,7 +30,8 @@ namespace fused {
 
 // ---- weight packing: W (f32, N x K) -> bf16 stage images in consumption order ----------------
 // image = for each 80-row output chunk c, for each 64-wide k slab s: a (rows_c x 128 B) block in the
-// K-major SWIZZLE_128B layout the tensor core reads; one cp.async.bulk per block lands it in smem.
+// K-major SWIZZLE_128B layout the tensor core reads; one cp.async.bulk per block lands it in smem.  Inside a chunk, image
+// row j holds W row 80 c + acc_out_col(j, rows_c) (tc_common.cuh), so that the epilogue's fragments are column runs.
 struct PackGeom {
   int N, K, hpN, hpK, nslab, nchunks;
 };
@@ -45,10 +46,10 @@ __host__ __device__ inline PackGeom pack_geom(int64_t N, int64_t K) {
 }
 
 __global__ void k_pack_weight(const float* __restrict__ W, int64_t ldw, PackGeom g, __nv_bfloat16* __restrict__ out) {
-  const int n = blockIdx.x;                        // 0 .. hpN-1
-  const int c = n / kChunkN;
-  const int nl = n - c * kChunkN;
+  const int c = blockIdx.x / kChunkN;              // image row blockIdx.x (0 .. hpN-1) = row nl of chunk c
+  const int nl = blockIdx.x - c * kChunkN;
   const int rows = min(kChunkN, g.hpN - c * kChunkN);
+  const int n = c * kChunkN + tc::acc_out_col(nl, rows);   // the W row (output column) it holds; zero at n >= N
   for (int k = threadIdx.x; k < g.nslab * 64; k += blockDim.x) {
     const int s = k >> 6, kl = k & 63;
     const size_t blk = (size_t)c * kChunkN * g.nslab * 128 + (size_t)s * rows * 128;

@@ -296,24 +296,42 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, Params p) {
           }
           st_prev = st;
         }
-        // ---- epilogue operands: requested now, so that their L2 latency overlaps the last wgmma group
+        // ---- epilogue operands: requested now, so that their L2 latency overlaps the last wgmma group.  The packed W_h image
+        // permutes the columns of every chunk (tc::acc_out_col): in each 32-column group G this thread's accumulator blocks
+        // 4 G .. 4 G + 3 hold the 8 contiguous output columns from acc_out_col(32 G + cl, nc) on, in a 16-column tail its
+        // blocks 4 G, 4 G + 1 hold 4 (acc_run_cols).  So each row and group is one 16-byte (tail: 8-byte) load and store, and
+        // hwv[h][b] is the operand word of accumulator block b, as before.
+        constexpr int kGroups = (kChunkN + 31) / 32;   // two 32-column groups and a 16-column tail
         uint32_t hwv[2][kChunkN / 8];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int r = rA + 8 * h;
-          const __nv_bfloat16* yrow = p.H0 + (int64_t)(row0 + r) * p.ld;
+          const __nv_bfloat16* yrow = p.H0 + (int64_t)(row0 + r) * p.ld + c * kChunkN;
 #pragma unroll
-          for (int b = 0; b < kChunkN / 8; ++b) {
-            hwv[h][b] = 0u;
-            if (MODE != MODE_BWD_COPY && r < nrows && 8 * b < nc)
-              hwv[h][b] = __ldg(reinterpret_cast<const unsigned int*>(yrow + c * kChunkN + 8 * b + cl));
+          for (int G = 0; G < kGroups; ++G) {
+            const int run = acc_run_cols(32 * G + cl, nc);
+            uint4 v = make_uint4(0u, 0u, 0u, 0u);
+            if (MODE != MODE_BWD_COPY && r < nrows) {
+              const __nv_bfloat16* src = yrow + acc_out_col(32 * G + cl, nc);
+              if (32 * G + 32 <= kChunkN && run == 8) {
+                v = __ldg(reinterpret_cast<const uint4*>(src));
+              } else if (run == 4) {
+                const uint2 u = __ldg(reinterpret_cast<const uint2*>(src));
+                v.x = u.x; v.y = u.y;
+              }
+            }
+            const uint32_t vw[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int w = 0; w < 4; ++w)
+              if (4 * G + w < kChunkN / 8) hwv[h][4 * G + w] = vw[w];
           }
         }
         wgmma_wait<0>();
         acc_fence(acc);
         release(st_prev, npass - 1);
         if (c == 0 && tt == 0) trace_ev(p, it, 6 + wg);
-        // ---- epilogue of chunk c: rows rA, rA + 8; columns 80 c + 8 b + cl + {0, 1}
+        // ---- epilogue of chunk c: rows rA, rA + 8; per group G the run of columns 80 c + acc_out_col(32 G + cl, nc) + [0, run),
+        // word w of which (columns n, n + 1) comes from accumulator block 4 G + w
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int r = rA + 8 * h;
@@ -321,52 +339,70 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, Params p) {
           const int64_t grow = (int64_t)(row0 + r);
           __nv_bfloat16* orow = p.Hn + grow * p.ld;
 #pragma unroll
-          for (int b = 0; b < kChunkN / 8; ++b) {
-            const int n = c * kChunkN + 8 * b + cl;
-            if (8 * b >= nc) continue;
-            const float v0 = acc[4 * b + 2 * h], v1 = acc[4 * b + 2 * h + 1];
-            uint32_t o;
-            if constexpr (MODE == MODE_BWD_COPY) {          // dOut = (S.P)(dZ) . W_h
-              o = pack_bf2(v0, v1);
-            } else {
-              const uint32_t hw = hwv[h][b];
-              if constexpr (MODE == MODE_BWD_MASK || MODE == MODE_BWD_LAST) {
-                // ... * tau'(.): from the activation output the row came from, or (LAST) from the pre-activation H_0
-                const float g0 = MODE == MODE_BWD_LAST ? act_grad_from_pre(ACT, p.act_param, bf_lo(hw))
-                                                       : act_grad_from_out(ACT, p.act_param, bf_lo(hw));
-                const float g1 = MODE == MODE_BWD_LAST ? act_grad_from_pre(ACT, p.act_param, bf_hi(hw))
-                                                       : act_grad_from_out(ACT, p.act_param, bf_hi(hw));
-                float z0 = v0 * g0, z1 = v1 * g1;
-                if (MODE == MODE_BWD_LAST && p.add0 != nullptr) {
-                  // dH_0 = (this step's masked gradient) + the earlier steps' dZ rows (L2 hits: prefetched by warp 3)
-                  const uint32_t aw = __ldg(reinterpret_cast<const unsigned int*>(p.add0 + grow * p.ld + n));
-                  const uint32_t bw = p.add1 != nullptr ? __ldg(reinterpret_cast<const unsigned int*>(p.add1 + grow * p.ld + n)) : 0u;
-                  z0 += bf_lo(aw) + bf_lo(bw);
-                  z1 += bf_hi(aw) + bf_hi(bw);
-                }
-                o = pack_bf2(z0, z1);
+          for (int G = 0; G < kGroups; ++G) {
+            const int run = acc_run_cols(32 * G + cl, nc);   // 8, 4 or 0 (nc is a multiple of 16)
+            if (run == 0) continue;
+            const bool full = 32 * G + 32 <= kChunkN && run == 8;
+            const int n0 = c * kChunkN + acc_out_col(32 * G + cl, nc);
+            // MODE_BWD_LAST addends: 8-byte loads, two words of each addend at a time (whole 16-byte runs of both addends
+            // next to the preloaded operands spill at 96 registers)
+            uint2 aw = make_uint2(0u, 0u), bw = make_uint2(0u, 0u);
+            // keep bits of the run (it lies inside one 16-column block), shifted so that bit 2 w is column n0 + 2 w
+            uint32_t kb = 0u;
+            if constexpr (MODE == MODE_FWD && DROP) kb = (uint32_t)__ldg(p.drop_bits + grow * nj + (n0 >> 4)) >> (n0 & 15);
+            uint32_t o[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+            for (int w = 0; w < 4; ++w) {
+              const int b = 4 * G + w;
+              if (b >= kChunkN / 8 || 2 * w >= run) break;
+              const int n = n0 + 2 * w;
+              const float v0 = acc[4 * b + 2 * h], v1 = acc[4 * b + 2 * h + 1];
+              if constexpr (MODE == MODE_BWD_COPY) {          // dOut = (S.P)(dZ) . W_h
+                o[w] = pack_bf2(v0, v1);
               } else {
-                float z0 = v0 + bf_lo(hw);
-                float z1 = v1 + bf_hi(hw);
-                if constexpr (HAS_BIAS) {
-                  z0 += s_bias[n];
-                  z1 += s_bias[n + 1];
-                }
-                if constexpr (MODE == MODE_FWD && DROP) {
-                  // nn.Dropout of base.py:139 in the epilogue: tau in f32, keep bit, exact f32 scale 1 / (1 - p), one rounding
-                  const uint32_t kb = __ldg(p.drop_bits + grow * nj + (n >> 4));
-                  const int bit = n & 15;
-                  z0 = ((kb >> bit) & 1u) ? act_t<ACT>(p.act_param, z0) * p.drop_scale : 0.f;
-                  z1 = ((kb >> (bit + 1)) & 1u) ? act_t<ACT>(p.act_param, z1) * p.drop_scale : 0.f;
-                  o = pack_bf2(z0, z1);
-                } else if constexpr (ACT == DMPNN_ACT_RELU) {
-                  o = act_word<ACT>(pack_bf2(z0, z1), 0.f);  // max after rounding == rounding after max
+                const uint32_t hw = hwv[h][b];
+                if constexpr (MODE == MODE_BWD_MASK || MODE == MODE_BWD_LAST) {
+                  // ... * tau'(.): from the activation output the row came from, or (LAST) from the pre-activation H_0
+                  const float g0 = MODE == MODE_BWD_LAST ? act_grad_from_pre(ACT, p.act_param, bf_lo(hw))
+                                                         : act_grad_from_out(ACT, p.act_param, bf_lo(hw));
+                  const float g1 = MODE == MODE_BWD_LAST ? act_grad_from_pre(ACT, p.act_param, bf_hi(hw))
+                                                         : act_grad_from_out(ACT, p.act_param, bf_hi(hw));
+                  float z0 = v0 * g0, z1 = v1 * g1;
+                  if (MODE == MODE_BWD_LAST && p.add0 != nullptr) {
+                    // dH_0 = (this step's masked gradient) + the earlier steps' dZ rows (L2 hits: prefetched by warp 3)
+                    if ((w & 1) == 0) {
+                      aw = __ldg(reinterpret_cast<const uint2*>(p.add0 + grow * p.ld + n));
+                      bw = p.add1 != nullptr ? __ldg(reinterpret_cast<const uint2*>(p.add1 + grow * p.ld + n)) : make_uint2(0u, 0u);
+                    }
+                    const uint32_t a = (w & 1) ? aw.y : aw.x, bb = (w & 1) ? bw.y : bw.x;
+                    z0 += bf_lo(a) + bf_lo(bb);
+                    z1 += bf_hi(a) + bf_hi(bb);
+                  }
+                  o[w] = pack_bf2(z0, z1);
                 } else {
-                  o = pack_bf2(act_t<ACT>(p.act_param, z0), act_t<ACT>(p.act_param, z1));
+                  float z0 = v0 + bf_lo(hw);
+                  float z1 = v1 + bf_hi(hw);
+                  if constexpr (HAS_BIAS) {
+                    z0 += s_bias[n];
+                    z1 += s_bias[n + 1];
+                  }
+                  if constexpr (MODE == MODE_FWD && DROP) {
+                    // nn.Dropout of base.py:139 in the epilogue: tau in f32, keep bit, exact f32 scale 1 / (1 - p), one rounding
+                    z0 = ((kb >> (2 * w)) & 1u) ? act_t<ACT>(p.act_param, z0) * p.drop_scale : 0.f;
+                    z1 = ((kb >> (2 * w + 1)) & 1u) ? act_t<ACT>(p.act_param, z1) * p.drop_scale : 0.f;
+                    o[w] = pack_bf2(z0, z1);
+                  } else if constexpr (ACT == DMPNN_ACT_RELU) {
+                    o[w] = act_word<ACT>(pack_bf2(z0, z1), 0.f);  // max after rounding == rounding after max
+                  } else {
+                    o[w] = pack_bf2(act_t<ACT>(p.act_param, z0), act_t<ACT>(p.act_param, z1));
+                  }
                 }
               }
             }
-            if (!(kExp && (p.exp_flags & 32768))) *reinterpret_cast<uint32_t*>(orow + n) = o;
+            if (!(kExp && (p.exp_flags & 32768))) {
+              if (full) *reinterpret_cast<uint4*>(orow + n0) = make_uint4(o[0], o[1], o[2], o[3]);
+              else *reinterpret_cast<uint2*>(orow + n0) = make_uint2(o[0], o[1]);
+            }
           }
         }
       }

@@ -121,6 +121,47 @@ __device__ __forceinline__ void st_global_2x128(void* ptr, const uint32_t (&v)[8
 __device__ __forceinline__ int acc_row0(int t) { return ((t >> 5) << 4) + ((t & 31) >> 2); }
 __device__ __forceinline__ int acc_col0(int t) { return (t & 3) << 1; }
 
+// Output column held by accumulator column j (0 <= j < nc) of an nc-column chunk / work item (nc % 8 == 0).  The weight
+// packers (k_pack_weight, k_pack_weight_tc) put W row `acc_out_col(j, nc)` at B row j, so that every thread's fragment covers
+// contiguous output columns and the epilogues load and store whole runs:
+// * in a 32-column group [32 g, 32 g + 32) (b and q swapped): accumulator column 32 g + 8 b + 2 q + e holds output column
+//   32 g + 8 q + 2 b + e, so thread q (acc_col0 = 2 q) holds columns 32 g + 8 q + [0, 8): one 16-byte run per row;
+// * in a 16-column tail (nc - 32 g in [16, 32)): 32 g + 8 b + 2 q + e holds 32 g + 4 q + 2 b + e, an 8-byte run per row;
+// * an 8-column tail stays in place: thread q holds its 2 columns 2 q + {0, 1}.
+// Every output column comes from the same products, summed in the same k order: only the register that holds it changes.
+__host__ __device__ __forceinline__ int acc_out_col(int j, int nc) {
+  const int base = j & ~31, rem = nc - base;
+  if (rem >= 32) return base + (((j >> 1) & 3) << 3) + (((j >> 3) & 3) << 1) + (j & 1);
+  if (rem >= 16 && j - base < 16) return base + (((j >> 1) & 3) << 2) + (((j >> 3) & 1) << 1) + (j & 1);
+  return j;
+}
+// Width of the run of output columns whose first column is acc_out_col(j, nc), for the first accumulator column j of a
+// thread in a group or tail (32 g + 2 q; 32 g + 16 + 2 q for an 8-column tail after a 16-column one): 8 in a full 32-column
+// group, 4 in a 16-column tail, 2 in an 8-column tail, 0 past the chunk
+__host__ __device__ __forceinline__ int acc_run_cols(int j, int nc) {
+  const int base = j & ~31, rem = nc - base;
+  if (rem >= 32) return 8;
+  if (rem >= 16 && j - base < 16) return 4;
+  return j < nc ? 2 : 0;
+}
+// A run of nw (4, 2 or 1) bf16x2 words: one 16-, 8- or 4-byte load / store (the address is aligned to its size)
+__device__ __forceinline__ void ld_run(const __nv_bfloat16* p, int nw, uint32_t (&v)[4]) {
+  if (nw == 4) {
+    const uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
+    v[0] = u.x; v[1] = u.y; v[2] = u.z; v[3] = u.w;
+  } else if (nw == 2) {
+    const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
+    v[0] = u.x; v[1] = u.y;
+  } else {
+    v[0] = __ldg(reinterpret_cast<const unsigned int*>(p));
+  }
+}
+__device__ __forceinline__ void st_run(__nv_bfloat16* p, int nw, const uint32_t (&v)[4]) {
+  if (nw == 4) *reinterpret_cast<uint4*>(p) = make_uint4(v[0], v[1], v[2], v[3]);
+  else if (nw == 2) *reinterpret_cast<uint2*>(p) = make_uint2(v[0], v[1]);
+  else *reinterpret_cast<uint32_t*>(p) = v[0];
+}
+
 __device__ __forceinline__ uint4 lds128(uint32_t a) {
   uint4 v;
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");

@@ -296,7 +296,9 @@ int dmpnn_act_bwd(const void* G, int g_dtype, int64_t ldg, const int32_t* gidx,
  * depth step: W_i (mixins.py:8-9, 22-23), W_o (base.py:180-182) and dX = dY.W of their autograd mirror.
  *   dmpnn_concat_bf16     A[r] = bf16([X1[i1(r)] || X2[i2(r)] || 0..])  (torch.cat of mixins.py:9 / base.py:180)
  *   dmpnn_pack_weight_tc  nn.Linear weight (or its transpose: transpose != 0 packs B[n][k] = W[k][n]) ->
- *                         per-k-slab shared-memory images
+ *                         per-k-slab shared-memory images.  The image layout (swizzle, and the rows permuted inside
+ *                         each 152-row work item so that the epilogue stores column runs) is internal to the library:
+ *                         only dmpnn_linear_tc_bf16 / dmpnn_linear_tc_rows_bf16 read it
  *   dmpnn_linear_tc_bf16  C[r, 0:N] = act(A[r, 0:K] . B^T + bias + res[r, 0:N]); A, C, res (nullable; the H_0
  *                         residual of base.py:138, ldres % 8 == 0) bf16 row-major, lda/ldc % 8 == 0,
  *                         ldc >= pad16(N), K <= 448, N <= 304; C columns [N, pad16(N)) are written as zeros.
@@ -399,6 +401,8 @@ int dmpnn_column_sum(const void* Y, int y_dtype, int64_t ldy, int64_t R, int64_t
 /* Debug aid: when set (device pointer to n_tiles x 12 uint64, zero-filled), block 0 of the fused
  * kernel records %globaltimer stamps of its pipeline phases for its first n_tiles tiles. NULL = off. */
 int dmpnn_set_trace_buffer(void* dev_ptr, int64_t n_tiles);
+/* W (f32, N x K) -> the fused step's bf16 weight image.  Its layout (80-row chunks x 64-column k slabs, swizzled, rows
+ * permuted inside each chunk so that the epilogue stores column runs) is internal: only the fused step kernels read it. */
 int dmpnn_pack_weight_bf16_bytes(int64_t N, int64_t K, size_t* bytes);
 int dmpnn_pack_weight_bf16(const float* W, int64_t ldw, int64_t N, int64_t K, void* Wpk, void* stream);
 int dmpnn_bond_step_fused_bf16(const void* H_prev, const void* H_0, void* H_next, int64_t ld,
