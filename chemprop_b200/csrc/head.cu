@@ -8,6 +8,14 @@
 //                        launch; updates running_mean / running_var (momentum, unbiased variance) like nn.BatchNorm1d
 //   dmpnn_bn_bwd         dX, dgamma, dbeta from the saved x_hat / invstd
 //   dmpnn_mse_loss       loss = sum(w_b * tw_t * mask * (p - y)^2) / sum(mask) and dLoss/dp, NaN targets masked, one launch
+//   dmpnn_bce_loss       the same reduction of binary_cross_entropy_with_logits (chemprop's BCELoss, metrics.py:291-294)
+//   dmpnn_ce_loss        the same reduction of cross_entropy over groups of C logits (CrossEntropyLoss, metrics.py:297-303)
+//   dmpnn_class_probs    eval-mode outputs of the classification predictors: sigmoid, or softmax per group of C columns
+#include <math_constants.h>
+
+#include <algorithm>
+#include <cmath>
+
 #include "common.cuh"
 
 namespace dmpnn {
@@ -153,6 +161,143 @@ k_mse_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y
     }
 }
 
+// fixed-order sum of (l, cnt) over a block of up to 1024 threads; every thread gets {sum l, sum cnt}
+__device__ __forceinline__ float2 block_sum2(float l, float cnt) {
+  __shared__ float s_l[32], s_n[32];
+  __shared__ float2 s_tot;
+  for (int o = 16; o > 0; o >>= 1) {
+    l += __shfl_down_sync(0xffffffffu, l, o);
+    cnt += __shfl_down_sync(0xffffffffu, cnt, o);
+  }
+  if ((threadIdx.x & 31) == 0) { s_l[threadIdx.x >> 5] = l; s_n[threadIdx.x >> 5] = cnt; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float tl = 0.f, tn = 0.f;
+    for (int k = 0; k < (int)(blockDim.x >> 5); ++k) { tl += s_l[k]; tn += s_n[k]; }
+    s_tot = make_float2(tl, tn);
+  }
+  __syncthreads();
+  return s_tot;
+}
+
+// binary_cross_entropy_with_logits as torch computes it: (1 - y) x + mx + log(e^{-mx} + e^{-x-mx}), mx = max(-x, 0)
+__device__ __forceinline__ float bce_with_logits(float x, float y) {
+  const float mx = fmaxf(-x, 0.f);
+  return (1.f - y) * x + mx + logf(expf(-mx) + expf(-x - mx));
+}
+
+__device__ __forceinline__ float sigmoid_stable(float x) {
+  if (x >= 0.f) return 1.f / (1.f + expf(-x));
+  const float e = expf(x);
+  return e / (1.f + e);
+}
+
+// one block: loss[0] = sum_{b,t} w_b tw_t m_bt bce(p, y) / sum m,  dP = (sigmoid(p) - y) w tw m / sum m   (m = isfinite(y))
+__global__ void __launch_bounds__(1024)
+k_bce_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y, int64_t ldy, const float* __restrict__ w,
+           const float* __restrict__ tw, int64_t B, int T, float* __restrict__ loss, float* __restrict__ dP, int64_t lddp) {
+  const int64_t n = B * (int64_t)T;
+  float l = 0.f, cnt = 0.f;
+  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const int64_t b = i / T;
+    const int t = (int)(i - b * T);
+    const float y = Y[b * ldy + t];
+    if (isfinite(y)) {
+      l = fmaf((w ? w[b] : 1.f) * (tw ? tw[t] : 1.f), bce_with_logits(P[b * ldp + t], y), l);
+      cnt += 1.f;
+    }
+  }
+  const float2 tot = block_sum2(l, cnt);
+  if (threadIdx.x == 0) loss[0] = tot.y > 0.f ? tot.x / tot.y : 0.f;
+  const float inv_n = tot.y > 0.f ? 1.f / tot.y : 0.f;
+  if (dP != nullptr)
+    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+      const int64_t b = i / T;
+      const int t = (int)(i - b * T);
+      const float y = Y[b * ldy + t];
+      dP[b * lddp + t] = isfinite(y)
+          ? (sigmoid_stable(P[b * ldp + t]) - y) * (w ? w[b] : 1.f) * (tw ? tw[t] : 1.f) * inv_n : 0.f;
+    }
+}
+
+// class index of a finite label as torch's `.long()` truncates it; -1 when outside [0, C)
+__device__ __forceinline__ int class_of(float y, int C) {
+  const float k = truncf(y);
+  return (k >= 0.f && k < (float)C) ? (int)k : -1;
+}
+
+// one block; row (b, t) = logits P[b, t*C : (t+1)*C].  loss[0] = sum w_b tw_t m_bt (lse(row) - row[label]) / sum m,
+// dP row = (softmax(row) - onehot(label)) w tw m / sum m.  A finite label outside [0, C) makes its term and its dP row NaN.
+__global__ void __launch_bounds__(1024)
+k_ce_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y, int64_t ldy, const float* __restrict__ w,
+          const float* __restrict__ tw, int64_t B, int T, int C, float* __restrict__ loss, float* __restrict__ dP,
+          int64_t lddp) {
+  const int64_t n = B * (int64_t)T;
+  float l = 0.f, cnt = 0.f;
+  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const int64_t b = i / T;
+    const int t = (int)(i - b * T);
+    const float y = Y[b * ldy + t];
+    if (!isfinite(y)) continue;
+    const float* p = P + b * ldp + (int64_t)t * C;
+    const int k = class_of(y, C);
+    float mx = p[0];
+    for (int c = 1; c < C; ++c) mx = fmaxf(mx, p[c]);
+    float s = 0.f;
+    for (int c = 0; c < C; ++c) s += expf(p[c] - mx);
+    const float li = k >= 0 ? logf(s) + mx - p[k] : CUDART_NAN_F;
+    l = fmaf((w ? w[b] : 1.f) * (tw ? tw[t] : 1.f), li, l);
+    cnt += 1.f;
+  }
+  const float2 tot = block_sum2(l, cnt);
+  if (threadIdx.x == 0) loss[0] = tot.y > 0.f ? tot.x / tot.y : 0.f;
+  const float inv_n = tot.y > 0.f ? 1.f / tot.y : 0.f;
+  if (dP != nullptr)
+    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+      const int64_t b = i / T;
+      const int t = (int)(i - b * T);
+      const float y = Y[b * ldy + t];
+      const float* p = P + b * ldp + (int64_t)t * C;
+      float* d = dP + b * lddp + (int64_t)t * C;
+      if (!isfinite(y)) {
+        for (int c = 0; c < C; ++c) d[c] = 0.f;
+        continue;
+      }
+      const int k = class_of(y, C);
+      const float scale = (w ? w[b] : 1.f) * (tw ? tw[t] : 1.f) * inv_n;
+      float mx = p[0];
+      for (int c = 1; c < C; ++c) mx = fmaxf(mx, p[c]);
+      float s = 0.f;
+      for (int c = 0; c < C; ++c) s += expf(p[c] - mx);
+      const float inv_s = 1.f / s;
+      for (int c = 0; c < C; ++c)
+        d[c] = k >= 0 ? (expf(p[c] - mx) * inv_s - (c == k ? 1.f : 0.f)) * scale : CUDART_NAN_F;
+    }
+}
+
+// one thread per (b, t) group of C columns: sigmoid of every entry (softmax == 0) or the group's softmax
+__global__ void __launch_bounds__(256)
+k_class_probs(const float* __restrict__ P, int64_t ldp, int64_t B, int T, int C, int softmax, float* __restrict__ out,
+              int64_t ldo) {
+  const int64_t n = B * (int64_t)T;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / T;
+    const int t = (int)(i - b * T);
+    const float* p = P + b * ldp + (int64_t)t * C;
+    float* o = out + b * ldo + (int64_t)t * C;
+    if (!softmax) {
+      for (int c = 0; c < C; ++c) o[c] = sigmoid_stable(p[c]);
+      continue;
+    }
+    float mx = p[0];
+    for (int c = 1; c < C; ++c) mx = fmaxf(mx, p[c]);
+    float s = 0.f;
+    for (int c = 0; c < C; ++c) s += expf(p[c] - mx);
+    const float inv_s = 1.f / s;
+    for (int c = 0; c < C; ++c) o[c] = expf(p[c] - mx) * inv_s;
+  }
+}
+
 }  // namespace head
 }  // namespace dmpnn
 
@@ -191,5 +336,41 @@ extern "C" int dmpnn_mse_loss(const float* P, int64_t ldp, const float* Y, int64
   DMPNN_CHECK_ARG(ldp >= T && ldy >= T && (dP == nullptr || lddp >= T), "mse_loss: row strides too small");
   head::k_mse_loss<<<1, 1024, 0, st>>>(P, ldp, Y, ldy, weights, task_weights, B, (int)T, loss, dP, lddp);
   DMPNN_CHECK_LAUNCH("mse_loss", 1);
+  return 0;
+}
+
+extern "C" int dmpnn_bce_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                              const float* task_weights, int64_t B, int64_t T, float* loss, float* dP, int64_t lddp,
+                              void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(B >= 0 && T > 0 && T <= INT32_MAX && loss && (B == 0 || (P && Y)), "bce_loss: bad args");
+  DMPNN_CHECK_ARG(ldp >= T && ldy >= T && (dP == nullptr || lddp >= T), "bce_loss: row strides too small");
+  head::k_bce_loss<<<1, 1024, 0, st>>>(P, ldp, Y, ldy, weights, task_weights, B, (int)T, loss, dP, lddp);
+  DMPNN_CHECK_LAUNCH("bce_loss", 1);
+  return 0;
+}
+
+extern "C" int dmpnn_ce_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                             const float* task_weights, int64_t B, int64_t T, int64_t C, float* loss, float* dP, int64_t lddp,
+                             void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(B >= 0 && T > 0 && C > 0 && T * C <= INT32_MAX && loss && (B == 0 || (P && Y)), "ce_loss: bad args");
+  DMPNN_CHECK_ARG(ldp >= T * C && ldy >= T && (dP == nullptr || lddp >= T * C), "ce_loss: row strides too small");
+  head::k_ce_loss<<<1, 1024, 0, st>>>(P, ldp, Y, ldy, weights, task_weights, B, (int)T, (int)C, loss, dP, lddp);
+  DMPNN_CHECK_LAUNCH("ce_loss", 1);
+  return 0;
+}
+
+extern "C" int dmpnn_class_probs(const float* P, int64_t ldp, int64_t B, int64_t T, int64_t C, int softmax, float* out,
+                                 int64_t ldo, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(B >= 0 && T > 0 && C > 0 && T * C <= INT32_MAX && (softmax == 0 || softmax == 1) &&
+                      (B == 0 || (P && out)), "class_probs: bad args");
+  DMPNN_CHECK_ARG(ldp >= T * C && ldo >= T * C, "class_probs: row strides too small");
+  if (B == 0) return 0;
+  const int64_t groups = B * T;
+  const unsigned blocks = (unsigned)std::min<int64_t>((groups + 255) / 256, 1024);
+  head::k_class_probs<<<blocks, 256, 0, st>>>(P, ldp, B, (int)T, (int)C, softmax, out, ldo);
+  DMPNN_CHECK_LAUNCH("class_probs", 1);
   return 0;
 }

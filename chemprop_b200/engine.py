@@ -600,6 +600,33 @@ def mse_loss(P: Tensor, Y: Tensor, w, tw, loss: Tensor, dP: Tensor):
     _lib.check(rc, "dmpnn_mse_loss")
 
 
+def bce_loss(P: Tensor, Y: Tensor, w, tw, loss: Tensor, dP: Tensor):
+    lib = _lib.load()
+    B, T = P.shape
+    rc = lib.dmpnn_bce_loss(P.data_ptr(), P.stride(0) if B else T, Y.data_ptr(), Y.stride(0) if B else T, _ptr(w), _ptr(tw), B, T,
+                            loss.data_ptr(), dP.data_ptr(), dP.stride(0) if B else T, _stream())
+    _lib.check(rc, "dmpnn_bce_loss")
+
+
+def ce_loss(P: Tensor, Y: Tensor, w, tw, C: int, loss: Tensor, dP: Tensor):
+    """P: B x (T*C) logits (task t in columns [t*C, (t+1)*C)), Y: B x T class labels."""
+    lib = _lib.load()
+    B, TC = P.shape
+    T = Y.shape[1]
+    rc = lib.dmpnn_ce_loss(P.data_ptr(), P.stride(0) if B else TC, Y.data_ptr(), Y.stride(0) if B else T, _ptr(w), _ptr(tw), B,
+                           T, C, loss.data_ptr(), dP.data_ptr(), dP.stride(0) if B else TC, _stream())
+    _lib.check(rc, "dmpnn_ce_loss")
+
+
+def class_probs(P: Tensor, C: int, softmax: bool, out: Tensor):
+    """out = sigmoid(P) (softmax=False) or the softmax of every group of C columns of P (B x (T*C))."""
+    lib = _lib.load()
+    B, TC = P.shape
+    rc = lib.dmpnn_class_probs(P.data_ptr(), P.stride(0) if B else TC, B, TC // C, C, 1 if softmax else 0, out.data_ptr(),
+                               out.stride(0) if B else TC, _stream())
+    _lib.check(rc, "dmpnn_class_probs")
+
+
 def column_sum(Y: Tensor, R: int, N: int, out: Tensor, *, accumulate: bool = False):
     lib = _lib.load()
     n = C.c_size_t(0)

@@ -1,12 +1,13 @@
 """Molecule-level head of the training step on the engine's kernels (SURVEY.md section 8f-2): what chemprop's `MPNN` does
 after the encoder -- `H = agg(H_v, batch)`, `H = bn(H)`, `preds = predictor(H)`, `loss = criterion(preds, targets, mask, w)`
-(chemprop/models/model.py:126-161, nn/ffn.py:38-61, nn/predictors.py:101-170, nn/metrics.py:78-123, 139-141) -- for the
-regression case: Mean / Sum / Norm aggregation, optional BatchNorm1d, the MLP of `RegressionFFN`, masked + weighted MSE.
+(chemprop/models/model.py:126-161, nn/ffn.py:38-61, nn/predictors.py:101-170, 231-317, nn/metrics.py:78-123, 139-141,
+291-303) -- for regression and classification: Mean / Sum / Norm aggregation, optional BatchNorm1d, the MLP of
+`RegressionFFN` / `BinaryClassificationFFN` / `MulticlassClassificationFFN`, masked + weighted MSE, BCE or cross-entropy.
 
 Every arithmetic step is a libdmpnn launch (aggregation: dmpnn_segment_sum; batch norm: dmpnn_bn_train_fwd / dmpnn_bn_bwd;
 the MLP's GEMMs: dmpnn_linear_fwd / dmpnn_linear_wgrad with the activation in the epilogue; the criterion and its gradient:
-dmpnn_mse_loss), none synchronises with the host, so the encoder + head + backward (+ a capturable optimizer) replay as ONE CUDA
-graph (`chemprop_b200.graph.CudaGraphStep`).
+dmpnn_mse_loss / dmpnn_bce_loss / dmpnn_ce_loss; eval-mode probabilities: dmpnn_class_probs), none synchronises with the
+host, so the encoder + head + backward (+ a capturable optimizer) replay as ONE CUDA graph (`chemprop_b200.graph.CudaGraphStep`).
 
 Module tree and state-dict keys are the reference's: `bn.{weight,bias,running_mean,running_var,num_batches_tracked}`,
 `predictor.ffn.<i>.<j>.{weight,bias}`, `predictor.criterion.task_weights` -- a reference `MPNN` state dict loads with
@@ -123,7 +124,79 @@ class EngineLinear(nn.Linear):
         return LinearActFunction.apply(x, self.weight, self.bias, act, act_param)
 
 
+class BCELossFunction(torch.autograd.Function):
+    """chemprop's BCE criterion: sum(w_b * tw_t * mask * bce_with_logits(p, y)) / sum(mask), mask = isfinite(targets), soft
+    labels allowed; loss and dLoss/dLogits in one launch (dmpnn_bce_loss)."""
+
+    @staticmethod
+    def forward(ctx, preds, targets, weights, task_weights):
+        K._require_cuda(preds, targets)
+        P, Y = preds.float().contiguous(), targets.float().contiguous()
+        w = None if weights is None else weights.float().reshape(-1).contiguous()
+        tw = None if task_weights is None else task_weights.float().reshape(-1).contiguous()
+        loss = torch.empty(1, device=P.device)
+        dP = torch.empty_like(P)
+        K.bce_loss(P, Y, w, tw, loss, dP)
+        ctx.save_for_backward(dP)
+        ctx.pdtype = preds.dtype
+        return loss.reshape(())
+
+    backward = staticmethod(MSELossFunction.backward)
+
+
+class CrossEntropyLossFunction(torch.autograd.Function):
+    """chemprop's cross-entropy criterion on b x T x C logits and b x T class labels (truncated like `targets.long()`):
+    sum(w_b * tw_t * mask * ce) / sum(mask); loss and dLoss/dLogits in one launch (dmpnn_ce_loss)."""
+
+    @staticmethod
+    def forward(ctx, preds, targets, weights, task_weights):
+        K._require_cuda(preds, targets)
+        b, T, C = preds.shape
+        P, Y = preds.float().reshape(b, T * C).contiguous(), targets.float().contiguous()
+        w = None if weights is None else weights.float().reshape(-1).contiguous()
+        tw = None if task_weights is None else task_weights.float().reshape(-1).contiguous()
+        loss = torch.empty(1, device=P.device)
+        dP = torch.empty_like(P)
+        K.ce_loss(P, Y, w, tw, C, loss, dP)
+        ctx.save_for_backward(dP.view(b, T, C))
+        ctx.pdtype = preds.dtype
+        return loss.reshape(())
+
+    backward = staticmethod(MSELossFunction.backward)
+
+
+class ClassProbsFunction(torch.autograd.Function):
+    """Eval-mode outputs of the classification predictors (dmpnn_class_probs): sigmoid of every logit, or the softmax of every
+    group of C columns.  The mirror (torch elementwise ops) is off the training path; it exists because chemprop's `forward`
+    is differentiable."""
+
+    @staticmethod
+    def forward(ctx, logits, C, softmax):
+        K._require_cuda(logits)
+        X = logits.float().contiguous()
+        out = torch.empty_like(X)
+        K.class_probs(X, C, softmax, out)
+        ctx.save_for_backward(out)
+        ctx.cfg = (C, softmax, logits.dtype)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        (p,) = ctx.saved_tensors
+        C, softmax, dt = ctx.cfg
+        g = g.float()
+        if not softmax:
+            return (g * p * (1 - p)).to(dt), None, None
+        b, n = p.shape
+        p3, g3 = p.view(b, n // C, C), g.reshape(b, n // C, C)
+        return (p3 * (g3 - (g3 * p3).sum(-1, keepdim=True))).view(b, n).to(dt), None, None
+
+
 class _Criterion(nn.Module):
+    """chemprop's `ChempropMetric` interface (nn/metrics.py:59-123) around one loss kernel: `task_weights` buffer (1 x T),
+    NaN targets or `mask` select the terms, `weights` are per molecule."""
+    _loss_fn = MSELossFunction
+
     def __init__(self, task_weights):
         super().__init__()
         self.register_buffer("task_weights", torch.as_tensor(task_weights, dtype=torch.float).view(1, -1))
@@ -132,12 +205,23 @@ class _Criterion(nn.Module):
         if lt_mask is not None or gt_mask is not None:
             raise NotImplementedError("bounded MSE is not part of the engine's head; use the reference criterion")
         t = targets if mask is None else torch.where(mask, targets, torch.full_like(targets, float("nan")))
-        return MSELossFunction.apply(preds, t, weights, self.task_weights)
+        return self._loss_fn.apply(preds, t, weights, self.task_weights)
 
 
-class EngineRegressionFFN(nn.Module):
-    """`RegressionFFN` (chemprop/nn/predictors.py:156-164) with the reference's module tree; GEMMs on the engine."""
+class _BCECriterion(_Criterion):
+    """chemprop's BCELoss (nn/metrics.py:291-294)."""
+    _loss_fn = BCELossFunction
+
+
+class _CrossEntropyCriterion(_Criterion):
+    """chemprop's CrossEntropyLoss (nn/metrics.py:297-303)."""
+    _loss_fn = CrossEntropyLossFunction
+
+
+class _EngineFFNPredictor(nn.Module):
+    """`_FFNPredictorBase` (chemprop/nn/predictors.py:101-157) with the reference's module tree; GEMMs on the engine."""
     n_targets = 1
+    _criterion_cls = _Criterion
 
     def __init__(self, n_tasks: int = 1, input_dim: int = DEFAULT_HIDDEN_DIM, hidden_dim: int | Sequence[int] = 300,
                  n_layers: int = 1, dropout: float = 0.0, activation="relu", task_weights=None):
@@ -152,7 +236,7 @@ class EngineRegressionFFN(nn.Module):
                     e.load_state_dict(m.state_dict())
                     block[i] = e
         self.ffn = ffn
-        self.criterion = _Criterion(torch.ones(n_tasks) if task_weights is None else task_weights)
+        self.criterion = self._criterion_cls(torch.ones(n_tasks) if task_weights is None else task_weights)
         self.output_transform = nn.Identity()
 
     @property
@@ -167,7 +251,7 @@ class EngineRegressionFFN(nn.Module):
     def n_tasks(self) -> int:
         return self.output_dim
 
-    def forward(self, Z: Tensor) -> Tensor:
+    def _mlp(self, Z: Tensor) -> Tensor:
         """`self.ffn(Z)` (nn/ffn.py:38-61: Linear, then [act, dropout, Linear] per further layer) with every activation the
         engine fuses folded into the epilogue of the GEMM before it."""
         blocks = [list(b) for b in self.ffn]
@@ -183,9 +267,53 @@ class EngineRegressionFFN(nn.Module):
             else:
                 X = tau(lin(X))
             X = drop(X)                                      # identity when p = 0 or in eval mode
-        return self.output_transform(X)
+        return X
+
+
+class EngineRegressionFFN(_EngineFFNPredictor):
+    """`RegressionFFN` (chemprop/nn/predictors.py:156-164) with the reference's module tree; GEMMs on the engine."""
+
+    def forward(self, Z: Tensor) -> Tensor:
+        return self.output_transform(self._mlp(Z))
 
     train_step = forward
+
+
+class EngineBinaryClassificationFFN(_EngineFFNPredictor):
+    """`BinaryClassificationFFN` (chemprop/nn/predictors.py:235-247): `train_step` gives the b x T logits, `forward` their
+    sigmoid (dmpnn_class_probs; no output transform, as in the reference); criterion: masked, weighted BCE (dmpnn_bce_loss)."""
+    _criterion_cls = _BCECriterion
+
+    def forward(self, Z: Tensor) -> Tensor:
+        return ClassProbsFunction.apply(self._mlp(Z), 1, False)
+
+    def train_step(self, Z: Tensor) -> Tensor:
+        return self._mlp(Z)
+
+
+class EngineMulticlassClassificationFFN(_EngineFFNPredictor):
+    """`MulticlassClassificationFFN` (chemprop/nn/predictors.py:272-316): the MLP has n_tasks * n_classes outputs, task t in
+    columns [t * n_classes, (t + 1) * n_classes); `train_step` gives the logits as b x T x C, `forward` their softmax over
+    the classes (dmpnn_class_probs); criterion: masked, weighted cross-entropy (dmpnn_ce_loss)."""
+    _criterion_cls = _CrossEntropyCriterion
+
+    def __init__(self, n_classes: int, n_tasks: int = 1, input_dim: int = DEFAULT_HIDDEN_DIM,
+                 hidden_dim: int | Sequence[int] = 300, n_layers: int = 1, dropout: float = 0.0, activation="relu",
+                 task_weights=None):
+        task_weights = torch.ones(n_tasks) if task_weights is None else task_weights
+        super().__init__(n_tasks * n_classes, input_dim, hidden_dim, n_layers, dropout, activation, task_weights)
+        self.n_classes = n_classes
+        self.hparams.update(n_tasks=n_tasks, n_classes=n_classes)
+
+    @property
+    def n_tasks(self) -> int:
+        return self.output_dim // self.n_classes
+
+    def forward(self, Z: Tensor) -> Tensor:
+        return ClassProbsFunction.apply(self._mlp(Z), self.n_classes, True).reshape(Z.shape[0], -1, self.n_classes)
+
+    def train_step(self, Z: Tensor) -> Tensor:
+        return self._mlp(Z).reshape(Z.shape[0], -1, self.n_classes)
 
 
 class EngineBatchNorm1d(nn.BatchNorm1d):
@@ -208,8 +336,10 @@ class EngineBatchNorm1d(nn.BatchNorm1d):
 
 class EngineMPNN(nn.Module):
     """`chemprop.models.MPNN` reduced to the path (models/model.py:66-161): message passing -> aggregation -> batch norm ->
-    predictor -> criterion, all on the engine.  `training_loss(bmg, targets, weights=None)` is `MPNN.training_step` without
-    Lightning's logging; `forward(bmg)` gives the predictions."""
+    predictor -> criterion, all on the engine.  The predictor is EngineRegressionFFN (the default),
+    EngineBinaryClassificationFFN or EngineMulticlassClassificationFFN.  `training_loss(bmg, targets, weights=None)` is
+    `MPNN.training_step` without Lightning's logging; `forward(bmg)` gives the predictions (probabilities for the
+    classification predictors)."""
 
     def __init__(self, message_passing: nn.Module, agg: Aggregation | None = None, predictor: nn.Module | None = None,
                  batch_norm: bool = False):

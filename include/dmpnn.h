@@ -460,6 +460,21 @@ int dmpnn_wgrad_x3(const float* dY, int64_t lddy, const float* X, int64_t ldx, i
  *   dmpnn_bn_bwd        dX (and dgamma, dbeta when non-null) from dY, Xhat, invstd.
  *   dmpnn_mse_loss      chemprop's MSE criterion (nn/metrics.py:78-123, 139-141): loss[0] = sum_{b,t} w[b] tw[t] m (P - Y)^2
  *                       / sum m with m = isfinite(Y) (NaN target = masked, model.py:140-141); dP (nullable) = dloss/dP.
+ *   dmpnn_bce_loss      chemprop's BCELoss (nn/metrics.py:291-294) under the same reduction: loss[0] = sum_{b,t} w[b] tw[t] m
+ *                       L / sum m, L = binary_cross_entropy_with_logits(P, Y) in torch's stable form
+ *                       (1 - y) x + mx + log(e^{-mx} + e^{-x-mx}), mx = max(-x, 0); dP = (sigmoid(P) - Y) w tw m / sum m.
+ *                       Y may hold soft labels in [0, 1].  P, Y, dP: B x T.
+ *   dmpnn_ce_loss       chemprop's CrossEntropyLoss (nn/metrics.py:297-303): P is B x (T*C), task t owning columns
+ *                       [t*C, (t+1)*C) (the layout of ffn(Z).reshape(B, T, C)); Y is B x T.  L = logsumexp(row) -
+ *                       row[label] with label = trunc(Y) as torch's `.long()`; dP row = (softmax(row) - onehot) w tw m /
+ *                       sum m.  A finite label whose truncation lies outside [0, C) makes loss[0] NaN and that row of dP
+ *                       NaN: the reference raises there, which a kernel cannot do without synchronising with the host.
+ *                       C = 1 is legal (loss and gradient 0).
+ *   dmpnn_class_probs   eval-mode outputs of the classification predictors on P (B x (T*C)): softmax == 0 gives the
+ *                       sigmoid of every entry (binary, C = 1), softmax == 1 the softmax of every group of C columns.
+ * The three losses mask like dmpnn_mse_loss: m = isfinite(Y); with every target masked, loss[0] = 0 and dP = 0 (the
+ * reference's 0 / 0 would be NaN).  dP is written for every element, masked ones as zeros.  B = 0 is accepted; weights
+ * and task_weights are nullable (all ones).  One block per loss call.
  * All reductions run in a fixed order (deterministic); no host synchronisation.
  * ------------------------------------------------------------------------------------- */
 int dmpnn_bn_train_fwd(const float* X, int64_t ldx, int64_t B, int64_t d, const float* gamma, const float* beta,
@@ -470,6 +485,13 @@ int dmpnn_bn_bwd(const float* dY, int64_t lddy, const float* Xhat, int64_t ldh, 
                  void* stream);
 int dmpnn_mse_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
                    const float* task_weights, int64_t B, int64_t T, float* loss, float* dP, int64_t lddp, void* stream);
+int dmpnn_bce_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                   const float* task_weights, int64_t B, int64_t T, float* loss, float* dP, int64_t lddp, void* stream);
+int dmpnn_ce_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                  const float* task_weights, int64_t B, int64_t T, int64_t C, float* loss, float* dP, int64_t lddp,
+                  void* stream);
+int dmpnn_class_probs(const float* P, int64_t ldp, int64_t B, int64_t T, int64_t C, int softmax, float* out, int64_t ldo,
+                      void* stream);
 
 #ifdef __cplusplus
 }
