@@ -155,9 +155,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_linear_x3(Params p) {
     uint32_t ks = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
       const int t = item / p.n_pass, ps = item - t * p.n_pass;
-      float acc[64];
+      // two-level sum (see k_wgrad_x3): each 32-wide k slab chains from zero, slab sums are added with f32 round-to-nearest
+      float acc[64], tot[64];
 #pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      for (int i = 0; i < 64; ++i) { acc[i] = 0.f; tot[i] = 0.f; }
       for (int s = 0; s < p.nslab; ++s, ++ks) {
         const uint32_t st = ks % kStages, use = ks / kStages;
         mbar_wait(bar(B_FULL + st), use & 1);
@@ -176,6 +177,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_linear_x3(Params p) {
         wgmma_wait<0>();
         acc_fence(acc);
         mbar_arrive(bar(B_EMPTY + st));
+#pragma unroll
+        for (int i = 0; i < 64; ++i) { tot[i] = __fadd_rn(tot[i], acc[i]); acc[i] = 0.f; }
       }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -191,7 +194,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_linear_x3(Params p) {
             if (n + e >= p.ldc_pad) continue;
             float o = 0.f;
             if (n + e < p.N) {
-              float z = acc[4 * b + 2 * h + e];
+              float z = tot[4 * b + 2 * h + e];
               if (rrow != nullptr) z += __ldg(rrow + n + e);
               if (p.bias != nullptr) z += __ldg(p.bias + n + e);
               o = act_apply(p.act, p.act_param, z);
@@ -332,9 +335,14 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_x3(Params p) {
   } else {
     const int wg = (warp - 4) >> 2;
     const int tt = threadIdx.x - 128 - wg * 128;
-    float acc[64];
+    // Two-level sum: the wgmma accumulator chains kChainBlocks row blocks from zero, then is added into `tot` with
+    // round-to-nearest f32 adds.  The tensor core's own accumulation loses more than an f32 add, and its error grows with
+    // the chain: one chain over a slot's ~7 k (h = 600, 1.1 M rows) or ~10 k row blocks (one slot per tile above
+    // 1024 x 1024) broke the f32 bound (worst element 1.4e-5 / 4.8e-5 of sum |terms|, mean 2.4e-6 / 6.7e-6).
+    constexpr uint32_t kChainBlocks = 8;
+    float acc[64], tot[64];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int i = 0; i < 64; ++i) { acc[i] = 0.f; tot[i] = 0.f; }
     uint32_t ks = 0;
     for (int blk = slot; blk < p.n_blocks; blk += p.slots, ++ks) {
       const uint32_t st = ks % kStages, use = ks / kStages;
@@ -354,15 +362,21 @@ __global__ void __launch_bounds__(kThreads, 1) k_wgrad_x3(Params p) {
       wgmma_wait<0>();
       acc_fence(acc);
       mbar_arrive(bar(B_EMPTY + st));
+      if (ks % kChainBlocks == kChainBlocks - 1) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) { tot[i] = __fadd_rn(tot[i], acc[i]); acc[i] = 0.f; }
+      }
     }
-    // drain: zeros when this CTA had no block (acc stays 0)
+#pragma unroll
+    for (int i = 0; i < 64; ++i) tot[i] = __fadd_rn(tot[i], acc[i]);
+    // drain: zeros when this CTA had no block (tot stays 0)
     const int rl = wg * 64 + acc_row0(tt), cl = acc_col0(tt);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float* out = p.partial + ((size_t)blockIdx.x * kMT + rl + 8 * h) * kKT;
 #pragma unroll
       for (int b = 0; b < kKT / 8; ++b)
-        *reinterpret_cast<float2*>(out + 8 * b + cl) = make_float2(acc[4 * b + 2 * h], acc[4 * b + 2 * h + 1]);
+        *reinterpret_cast<float2*>(out + 8 * b + cl) = make_float2(tot[4 * b + 2 * h], tot[4 * b + 2 * h + 1]);
     }
   }
 }

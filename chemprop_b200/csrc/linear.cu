@@ -415,8 +415,10 @@ extern "C" int dmpnn_column_sum(const void* Y, int y_dtype, int64_t ldy, int64_t
   const int S = wgrad_splits(R);
   const int64_t rps = ((R + S - 1) / S + WR - 1) / WR * WR;
   float* bpart = (float*)workspace;
+  // the 4-wide kernel keeps 8 partial rows of N floats in shared memory; it runs while they fit the 48 KB a launch gets
+  // without opting in (N <= 1536), wider rows take the column-per-thread kernel
   DMPNN_DISPATCH_DTYPE(y_dtype, TY,
-    if (N % 4 == 0 && N <= 2048 && vec4_ok<TY>(Y, ldy)) {
+    if (N % 4 == 0 && 8 * N * sizeof(float) <= 48 * 1024 && vec4_ok<TY>(Y, ldy)) {
       k_colsum_partial_v4<TY><<<S, 256, 8 * N * sizeof(float), st>>>((const TY*)Y, ldy, bpart, R, (int)N, rps > 0 ? rps : WR);
     } else {
       dim3 g2(ceil_div_i64(N, 128), S);
