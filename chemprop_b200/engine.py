@@ -837,14 +837,16 @@ def atom_step_fused(H_prev: Tensor, H0: Tensor, H_next: Tensor, h: int, Wpk: Ten
 
 
 def atom_step_bwd_fused(dZ: Tensor, Yact: Tensor | None, dOut: Tensor, h: int, WpkT: Tensor, lay: Layout, act: int,
-                        act_param: float, G_out: Tensor | None = None, y_is_preact: bool = False):
-    """dOut[v] = ((sum_{e in in(v)} dZ[src(e)]) . W) [* act'(Yact[v])]; G_out also receives the gathered operand."""
+                        act_param: float, G_out: Tensor | None = None, y_is_preact: bool = False, addends: tuple = ()):
+    """dOut[v] = ((sum_{e in in(v)} dZ[src(e)]) . W) [* act'(Yact[v])] [+ addends (y_is_preact only)]; G_out also receives
+    the gathered operand."""
     lib = _lib.load()
     ta, te, info, nmax = atom_tables(lay)
     rc = lib.dmpnn_atom_step_bwd_fused_bf16(
         dZ.data_ptr(), _ptr(Yact), dOut.data_ptr(), _ld(dZ), dZ.shape[0], h, WpkT.data_ptr(), lay.rowptr.data_ptr(),
         lay.src_row.data_ptr(), ta.data_ptr(), te.data_ptr(), info.data_ptr(), nmax, act, float(act_param),
-        1 if y_is_preact else 0, None, None, _ptr(G_out), _stream())
+        1 if y_is_preact else 0, addends[0].data_ptr() if len(addends) > 0 else None,
+        addends[1].data_ptr() if len(addends) > 1 else None, _ptr(G_out), _stream())
     _lib.check(rc, "dmpnn_atom_step_bwd_fused_bf16")
 
 

@@ -9,9 +9,12 @@ within 1e-5) or "bf16" (bf16 hidden states + tensor-core depth step; within 1e-2
 Two execution tiers sit behind `forward`: the monolithic autograd functions of engine.py (tau fused into the
 kernels: ReLU / LeakyReLU / Tanh / ELU, dropout inactive) and the composed tier of composed.py (the reference's op
 sequence, one libdmpnn kernel per op, `self.tau` / `self.dropout` applied by torch in between) for everything else:
-PReLU, SELU or user activation modules, dropout > 0 in training, AtomMessagePassing(undirected=True).
+PReLU, SELU or user activation modules, LeakyReLU / ELU with a negative parameter, dropout > 0 in training,
+AtomMessagePassing(undirected=True).
 """
 from __future__ import annotations
+
+import math
 
 import torch
 from torch import Tensor, nn
@@ -47,25 +50,39 @@ def get_activation_function(activation) -> nn.Module:
 
 def engine_activation(tau: nn.Module) -> tuple[int, float]:
     """Map a torch activation module to the engine's fused activation code."""
-    if type(tau) is nn.ReLU:
-        return _lib.ACT_RELU, 0.0
+    if not is_fused_activation(tau):
+        raise NotImplementedError(
+            f"activation {activation_name(tau)} is not fused into the sm_90a kernels "
+            "(fused: ReLU, Tanh, Identity, LeakyReLU / ELU with a parameter >= 0; anything else runs on the composed tier)"
+        )
+    code = {nn.ReLU: _lib.ACT_RELU, nn.LeakyReLU: _lib.ACT_LEAKYRELU, nn.Tanh: _lib.ACT_TANH, nn.ELU: _lib.ACT_ELU,
+            nn.Identity: _lib.ACT_NONE}[type(tau)]
+    p = _act_param(tau)
+    return code, 0.0 if p is None else p
+
+
+def _act_param(tau: nn.Module) -> float | None:
     if type(tau) is nn.LeakyReLU:
-        return _lib.ACT_LEAKYRELU, float(tau.negative_slope)
-    if type(tau) is nn.Tanh:
-        return _lib.ACT_TANH, 0.0
+        return float(tau.negative_slope)
     if type(tau) is nn.ELU:
-        return _lib.ACT_ELU, float(tau.alpha)
-    if type(tau) is nn.Identity:
-        return _lib.ACT_NONE, 0.0
-    raise NotImplementedError(
-        f"activation {type(tau).__name__} is not fused into the sm_90a kernels "
-        "(fused: ReLU, LeakyReLU, Tanh, ELU; anything else runs on the composed tier)"
-    )
+        return float(tau.alpha)
+    return None
 
 
 def is_fused_activation(tau: nn.Module) -> bool:
-    """Exact stock classes only: a user subclass may override forward, so it goes to the composed tier."""
-    return type(tau) in _FUSED_ACTS
+    """Exact stock classes only: a user subclass may override forward, so it goes to the composed tier.  LeakyReLU and ELU
+    only with a finite parameter >= 0: the kernels' backward passes take tau' from the stored output (act_grad_from_out in
+    csrc/common.cuh: y > 0 ? 1 : slope, y > 0 ? 1 : y + alpha), which is tau'(z) only while tau keeps the sign of z."""
+    if type(tau) not in _FUSED_ACTS:
+        return False
+    p = _act_param(tau)
+    return p is None or (math.isfinite(p) and p >= 0.0)
+
+
+def activation_name(tau: nn.Module) -> str:
+    """How the composed-tier warnings name an activation: the class, or the module with its parameter when only the
+    parameter keeps it off the fused path."""
+    return repr(tau) if type(tau) in _FUSED_ACTS else type(tau).__name__
 
 
 class _MessagePassingBase(nn.Module):
@@ -150,7 +167,7 @@ class _MessagePassingBase(nn.Module):
             if self.precision == "bf16":
                 # no silent cliff: this tier keeps f32 hidden states; its W_h GEMMs run as 3xTF32 on the tensor cores (a sixth
                 # of the bf16 rate), W_i / W_o on the f32 FMA pipes, and every reference op is a launch of its own
-                why = (f"activation {type(self.tau).__name__}" if not is_fused_activation(self.tau) else
+                why = (f"activation {activation_name(self.tau)}" if not is_fused_activation(self.tau) else
                        "undirected AtomMessagePassing" if (self.undirected and type(self)._kind == 1) else
                        "training-mode dropout outside the fused ReLU path")
                 _warn_once("composed_bf16", f"chemprop_b200: precision='bf16' requested, but this configuration ({why}) runs on "

@@ -24,8 +24,8 @@ from torch import Tensor, nn
 from .. import composed
 from ..engine import MABMPFunction, MPConfig, _warn_once, get_layout, mab_bf16_limits
 from ..exceptions import InvalidShapeError
-from .message_passing import (DEFAULT_ATOM_FDIM, DEFAULT_BOND_FDIM, DEFAULT_HIDDEN_DIM, engine_activation,
-                              get_activation_function, is_fused_activation)
+from .message_passing import (DEFAULT_ATOM_FDIM, DEFAULT_BOND_FDIM, DEFAULT_HIDDEN_DIM, activation_name,
+                              engine_activation, get_activation_function, is_fused_activation)
 
 
 class _MABMessagePassingBase(nn.Module):
@@ -76,7 +76,7 @@ class _MABMessagePassingBase(nn.Module):
     def composed_reason(self) -> str | None:
         """Why this module, as configured now, runs on the composed tier with precision='bf16' (None: it does not)."""
         if not is_fused_activation(self.tau):
-            return f"activation {type(self.tau).__name__}"
+            return f"activation {activation_name(self.tau)}"
         if self.undirected:
             return "undirected=True"
         if self.training and self.dropout.p > 0:

@@ -24,23 +24,24 @@ from torch.nn import functional as F
 
 
 # --- activations: chemprop/nn/utils.py:43-55 ------------------------------------------------
-def activation(name, prelu_weight: Tensor | None = None):
-    """utils.py:19-55.  `name` may also be a callable (utils.py:37-42 passes modules through); "prelu" takes the
-    learnable slope (nn.PReLU: one parameter, initial value 0.25)."""
+def activation(name, prelu_weight: Tensor | None = None, param: float | None = None):
+    """utils.py:19-55.  `name` may also be a callable (utils.py:37-42 passes modules through, e.g. nn.LeakyReLU(0.3));
+    "prelu" takes the learnable slope (nn.PReLU: one parameter, initial value 0.25); `param` replaces the default
+    negative slope of "leakyrelu" (0.1) and alpha of "elu" (1.0)."""
     if callable(name):
         return name
     name = name.lower()
     if name == "relu":
         return torch.relu
     if name == "leakyrelu":
-        return lambda x: F.leaky_relu(x, 0.1)
+        return lambda x: F.leaky_relu(x, 0.1 if param is None else param)
     if name == "prelu":
         assert prelu_weight is not None, "prelu needs its weight"
         return lambda x: F.prelu(x, prelu_weight)
     if name == "tanh":
         return torch.tanh
     if name == "elu":
-        return F.elu
+        return F.elu if param is None else (lambda x: F.elu(x, param))
     if name == "selu":
         return F.selu
     if name == "softplus":
@@ -136,12 +137,13 @@ def finalize(M, V, W_o, b_o, tau, V_d=None, W_d=None, b_d=None, dropout=_no_drop
 
 def message_passing_forward(kind, V, E, edge_index, rev_edge_index, W_i, b_i, W_h, b_h, W_o, b_o, depth, act="relu",
                             undirected=False, V_d=None, W_d=None, b_d=None, return_intermediates=False,
-                            prelu_weight=None, dropout_masks=None):
+                            prelu_weight=None, dropout_masks=None, act_param=None):
     """_MessagePassingBase.forward, base.py:196-212.  kind in {"bond", "atom"}.
     `dropout_masks`: training-mode dropout with the masks given explicitly -- a list of already scaled
     (0 or 1/(1-p)) tensors consumed in call order (one E x h mask per depth step, base.py:139; one V x h mask after
-    W_o, base.py:182; one after W_d, base.py:188), so a run can be compared mask for mask."""
-    tau = activation(act, prelu_weight)
+    W_o, base.py:182; one after W_d, base.py:188), so a run can be compared mask for mask.
+    `act_param`: the LeakyReLU slope / ELU alpha when `act` is a name."""
+    tau = activation(act, prelu_weight, act_param)
     masks = list(dropout_masks) if dropout_masks is not None else None
     dropout = _no_dropout if masks is None else (lambda H: H * masks.pop(0))
     n_atoms = V.shape[0]

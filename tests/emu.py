@@ -453,13 +453,15 @@ def atom_step_fused(H_prev, H0, H_next, h, Wpk, bias, lay, act, act_param, first
         N_out[:V, :hp] = N.to(N_out.dtype)
 
 
-def atom_step_bwd_fused(dZ, Yact, dOut, h, WpkT, lay, act, act_param, G_out=None, y_is_preact=False):
-    """dOut = (A dZ) . W [* tau'(Yact)];  G_out = A dZ   (WpkT holds B = W^T of A . B^T)."""
+def atom_step_bwd_fused(dZ, Yact, dOut, h, WpkT, lay, act, act_param, G_out=None, y_is_preact=False, addends=()):
+    """dOut = (A dZ) . W [* tau'(Yact)] [+ addends];  G_out = A dZ   (WpkT holds B = W^T of A . B^T)."""
     V, hp = lay.V, _pad16(h)
     G = _neighbour_sum_packed(dZ.float()[:V, :hp], lay)
     D = _mma(G, WpkT, h)
     if Yact is not None:
         D = D * _dact(Yact[:V, :hp].float(), act, act_param, y_is_preact)
+    for a in addends:
+        D = D + a[:V, :hp].float()
     dOut[:V, :hp] = D.to(dOut.dtype)
     if G_out is not None:
         G_out[:V, :hp] = G.to(G_out.dtype)
