@@ -302,6 +302,10 @@ int dmpnn_act_bwd(const void* G, int g_dtype, int64_t ldg, const int32_t* gidx,
  *   dmpnn_linear_tc_bf16  C[r, 0:N] = act(A[r, 0:K] . B^T + bias + res[r, 0:N]); A, C, res (nullable; the H_0
  *                         residual of base.py:138, ldres % 8 == 0) bf16 row-major, lda/ldc % 8 == 0,
  *                         ldc >= pad16(N), K <= 448, N <= 304; C columns [N, pad16(N)) are written as zeros.
+ *                         Precondition: res columns [N, pad16(N)) are zero.  The epilogue adds res to whole column
+ *                         runs, so C's padding is act(res's padding); NaN there would reach the padding that the fused
+ *                         depth step reads as zeros.  (A per-column guard cost 0.7 % of C2 throughput on an
+ *                         H100 80GB HBM3 at 700 W; DESIGN.md section 4.2.)
  * ------------------------------------------------------------------------------------- */
 int dmpnn_concat_bf16(const void* X1, int x1_dtype, int64_t ld1, const int32_t* idx1, int64_t K1,
                       const void* X2, int x2_dtype, int64_t ld2, const int32_t* idx2, int64_t K2,

@@ -7,31 +7,20 @@ import pytest
 import torch
 
 from chemprop_b200 import _lib, engine
+from tests.test_gpu_fused_activations import U, _check_bound, _dtau64, _lip, _tau64
 from tests.test_mab_bf16_host import BF16_GOLDENS, _close_bf16, _golden_module, sweep_case
 from tests.util import load_golden
 
 pytestmark = pytest.mark.gpu
 
 ACTS = [(_lib.ACT_NONE, 0.0), (_lib.ACT_RELU, 0.0), (_lib.ACT_LEAKYRELU, 0.1), (_lib.ACT_TANH, 0.0), (_lib.ACT_ELU, 1.0)]
+_NAME = {_lib.ACT_NONE: "none", _lib.ACT_RELU: "relu", _lib.ACT_LEAKYRELU: "leakyrelu", _lib.ACT_TANH: "tanh",
+         _lib.ACT_ELU: "elu"}
 
 
 def _act(x, act, p):
     return {_lib.ACT_NONE: lambda: x, _lib.ACT_RELU: lambda: torch.relu(x), _lib.ACT_LEAKYRELU: lambda: torch.where(x > 0, x, p * x),
             _lib.ACT_TANH: lambda: torch.tanh(x), _lib.ACT_ELU: lambda: torch.where(x > 0, x, p * torch.expm1(x))}[act]()
-
-
-def _dact(y, act, p, pre):
-    one = torch.ones_like(y)
-    if act == _lib.ACT_RELU:
-        return (y > 0).float()
-    if act == _lib.ACT_LEAKYRELU:
-        return torch.where(y > 0, one, one * p)
-    if act == _lib.ACT_TANH:
-        t = torch.tanh(y) if pre else y
-        return 1 - t * t
-    if act == _lib.ACT_ELU:
-        return torch.where(y > 0, one, p * torch.exp(y) if pre else y + p)
-    return one
 
 
 @pytest.mark.parametrize("N", [40, 64, 300])
@@ -42,17 +31,22 @@ def test_rows_kernel_forward_mode(N, act, ap):
     R, K = 300, 14 + N
     A = torch.randn(R, K, generator=g).to(torch.bfloat16)
     W, b = torch.randn(N, K, generator=g) / K ** 0.5, torch.randn(N, generator=g)
-    ref = _act(A.float() @ W.to(torch.bfloat16).float().t() + b, act, ap)
     Ad = torch.zeros(R, (K + 15) // 16 * 16, dtype=torch.bfloat16, device="cuda")
     Ad[:, :K] = A.cuda()
     Wpk = engine.pack_weight_tc(W.cuda())
     out32 = torch.full((R, N), float("nan"), device="cuda")
     engine.linear_tc_rows(Ad, K, Wpk, N, out32, bias=b.cuda(), act=act, act_param=ap)
-    torch.testing.assert_close(out32.cpu(), ref, rtol=1e-4, atol=1e-4)
     n16 = (N + 15) // 16 * 16
     out16 = torch.full((R, engine.pad_hidden(N)), float("nan"), dtype=torch.bfloat16, device="cuda")
     engine.linear_tc_rows(Ad, K, Wpk, N, out16, bias=b.cuda(), act=act, act_param=ap)
-    torch.testing.assert_close(out16[:, :N].float().cpu(), ref, rtol=1e-2, atol=1e-2)
+    # float64 with the kernel's rounding points (tests/test_gpu_fused_activations.py): the f32 accumulation, tau in f32, and
+    # half a bf16 ulp for the bf16 store
+    a64, w64, b64 = A.double(), W.to(torch.bfloat16).double(), b.double()
+    Z = a64 @ w64.t()
+    y = _tau64(_NAME[act], ap, Z + b64)
+    delta = _lip(_NAME[act], ap) * (2 * K * U * (a64.abs() @ w64.abs().t()) + 3 * U * (Z.abs() + b64.abs())) + 8 * U * y.abs()
+    _check_bound(out32.cpu(), y, delta, f"rows forward f32 N={N} act={act}", bf16_out=False)
+    _check_bound(out16[:, :N].cpu(), y, delta, f"rows forward bf16 N={N} act={act}")
     assert bool((out16[:, N:n16] == 0).all())
 
 
@@ -73,13 +67,22 @@ def test_rows_kernel_mirror_mode(N, act, ap, pre):
     z = torch.randn(Rc, N, generator=g)
     Y = (z if pre else _act(z, act, ap)).to(torch.bfloat16)
     q, s = out_row.long(), res_row.long()
-    ref = (A.float() @ W.to(torch.bfloat16).float().t() + res.float()[s]) * _dact(Y.float()[q], act, ap, pre)
+    a64, w64 = A.double(), W.to(torch.bfloat16).double()
+    D, Ua = a64 @ w64.t(), a64.abs() @ w64.abs().t()
+
+    def bound_check(got, r, Yq, what):
+        """(D + r) * tau'(Yq) in float64, bounded by the f32 accumulation, the f32 residual add and tau', and half a bf16 ulp."""
+        d = _dtau64(_NAME[act], ap, Yq.double(), pre)
+        ref = (D + r) * d
+        delta = d.abs() * (2 * K * U * Ua + 2 * U * (D.abs() + r.abs())) + 8 * U * (1 + d.abs()) * (D + r).abs()
+        _check_bound(got, ref, delta, f"rows mirror {what} N={N} act={act} pre={pre}")
+
     dev = lambda x, cols: torch.cat([x, torch.zeros(x.shape[0], cols - x.shape[1], dtype=x.dtype)], 1).cuda()  # noqa: E731
     out = torch.full((Rc, hp), 7.0, dtype=torch.bfloat16, device="cuda")
     engine.linear_tc_rows(dev(A, hp), K, engine.pack_weight_tc(W.cuda()), N, out, act=act, act_param=ap, Y=dev(Y, hp),
                           from_preact=pre, out_row=out_row.cuda(), res=dev(res, hp), res_row=res_row.cuda())
     out = out.cpu()
-    torch.testing.assert_close(out[q, :N].float(), ref, rtol=1e-2, atol=1e-2)
+    bound_check(out[q, :N], res.double()[s], Y[q], "with maps")
     assert bool((out[q, N:(N + 15) // 16 * 16] == 0).all())
     untouched = torch.ones(Rc, dtype=torch.bool)
     untouched[q] = False
@@ -88,8 +91,7 @@ def test_rows_kernel_mirror_mode(N, act, ap, pre):
     out2 = torch.zeros((R, hp), dtype=torch.bfloat16, device="cuda")
     engine.linear_tc_rows(dev(A, hp), K, engine.pack_weight_tc(W.cuda()), N, out2, act=act, act_param=ap, Y=dev(Y[:R], hp),
                           from_preact=pre)
-    ref2 = (A.float() @ W.to(torch.bfloat16).float().t()) * _dact(Y.float()[:R], act, ap, pre)
-    torch.testing.assert_close(out2[:, :N].float().cpu(), ref2, rtol=1e-2, atol=1e-2)
+    bound_check(out2[:, :N].cpu(), torch.zeros_like(D), Y[:R], "identity rows")
 
 
 @pytest.mark.parametrize("name", BF16_GOLDENS)
