@@ -90,7 +90,16 @@ SIGNATURES = {
     "dmpnn_bce_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i64, _vp]),
     "dmpnn_ce_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _i64, _vp]),
     "dmpnn_class_probs": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _i32, _vp, _i64, _vp]),
+    "dmpnn_pred_transform": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _i64, _vp, _vp, _vp, _i64, _vp]),
+    "dmpnn_pred_transform_bwd": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _i64, _i32, _i64, _vp, _vp, _i64, _vp]),
+    "dmpnn_mve_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i64, _vp]),
+    "dmpnn_evidential_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _f32, _vp, _vp, _i64, _vp]),
+    "dmpnn_quantile_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _i64, _vp]),
+    "dmpnn_dirichlet_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _f32, _vp, _vp, _i64, _vp]),
 }
+
+# dmpnn_pred_transform kinds (include/dmpnn.h)
+PRED_REGRESSION, PRED_MVE, PRED_EVIDENTIAL, PRED_QUANTILE, PRED_DIRICHLET, PRED_DIRICHLET_PROBS, PRED_DIRICHLET_BINARY = range(7)
 
 
 class DmpnnError(RuntimeError):

@@ -11,6 +11,10 @@
 //   dmpnn_bce_loss       the same reduction of binary_cross_entropy_with_logits (chemprop's BCELoss, metrics.py:291-294)
 //   dmpnn_ce_loss        the same reduction of cross_entropy over groups of C logits (CrossEntropyLoss, metrics.py:297-303)
 //   dmpnn_class_probs    eval-mode outputs of the classification predictors: sigmoid, or softmax per group of C columns
+//   dmpnn_pred_transform(_bwd)  raw MLP output -> the output of the regression / MVE / evidential / quantile / Dirichlet
+//                        predictors (softplus, + 1, eval-mode unscaling), and its mirror
+//   dmpnn_mve_loss, dmpnn_evidential_loss, dmpnn_quantile_loss, dmpnn_dirichlet_loss
+//                        the uncertainty criteria (metrics.py:202-257, 502-544, 588-613) under the same reduction, one launch
 #include <math_constants.h>
 
 #include <algorithm>
@@ -298,6 +302,264 @@ k_class_probs(const float* __restrict__ P, int64_t ldp, int64_t B, int T, int C,
   }
 }
 
+// ---- uncertainty predictors (chemprop/nn/predictors.py:172-228, 250-270, 319-336; nn/metrics.py:202-257, 502-544,
+// 588-613) ------------------------------------------------------------------------------------------------------------
+enum PredKind { kRegression = 0, kMve = 1, kEvidential = 2, kQuantile = 3, kDirichlet = 4, kDirichletProbs = 5,
+                kDirichletBinary = 6 };
+
+// F.softplus(x) (beta 1, threshold 20) and its derivative as torch's softplus_backward computes it
+__device__ __forceinline__ float softplus20(float x) { return x > 20.f ? x : log1pf(expf(x)); }
+__device__ __forceinline__ float softplus20_grad(float x) {
+  if (x > 20.f) return 1.f;
+  const float z = expf(x);
+  return z / (z + 1.f);
+}
+
+// digamma and trigamma for x >= 1 (every argument the losses pass: softplus + 1, y + (1 - y) alpha, sums of those):
+// the recurrence lifts x to >= 6, where the asymptotic series is below f32 resolution after the terms kept
+constexpr float kPsiSwitch = 6.f;
+__device__ __forceinline__ float digamma_ge1(float x) {
+  float acc = 0.f;
+  while (x < kPsiSwitch) { acc -= 1.f / x; x += 1.f; }
+  const float r = 1.f / x, r2 = r * r;
+  return acc + logf(x) - 0.5f * r - r2 * (1.f / 12.f - r2 * (1.f / 120.f - r2 * (1.f / 252.f)));
+}
+__device__ __forceinline__ float trigamma_ge1(float x) {
+  float acc = 0.f;
+  while (x < kPsiSwitch) { acc += 1.f / (x * x); x += 1.f; }
+  const float r = 1.f / x, r2 = r * r;
+  return acc + r * (1.f + r * (0.5f + r * (1.f / 6.f - r2 * (1.f / 30.f - r2 * (1.f / 42.f - r2 * (1.f / 30.f))))));
+}
+
+// one thread per (b, t): raw MLP output X (B x (T*u)) -> predictor output (B x T x u).  Regression family: target j of task
+// t is column j*T + t (torch.chunk); Dirichlet family: class c of task t is column t*u + c (reshape).  mean / scale
+// (nullable, T entries) apply UnscaleTransform's eval mode; products and sums are rounded one by one as torch does.
+__global__ void __launch_bounds__(256)
+k_pred_transform(const float* __restrict__ X, int64_t ldx, int64_t B, int T, int kind, int u, const float* __restrict__ mean,
+                 const float* __restrict__ scale, float* __restrict__ out, int64_t ldo) {
+  const int64_t n = B * (int64_t)T;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / T;
+    const int t = (int)(i - b * T);
+    const float* x = X + b * ldx;
+    float* o = out + b * ldo + (int64_t)t * u;
+    const float s = scale ? scale[t] : 1.f, m = mean ? mean[t] : 0.f;
+    const float s2 = __fmul_rn(s, s);
+    auto unscale = [&](float v) { return scale ? __fadd_rn(__fmul_rn(v, s), m) : v; };
+    auto unscale_var = [&](float v) { return scale ? __fmul_rn(v, s2) : v; };
+    switch (kind) {
+      case kRegression: o[0] = unscale(x[t]); break;
+      case kMve:
+        o[0] = unscale(x[t]);
+        o[1] = unscale_var(softplus20(x[T + t]));
+        break;
+      case kEvidential:
+        o[0] = unscale(x[t]);
+        o[1] = softplus20(x[T + t]);
+        o[2] = softplus20(x[2 * T + t]) + 1.f;
+        o[3] = unscale_var(softplus20(x[3 * T + t]));
+        break;
+      case kQuantile: {
+        const float lo = unscale(x[t]), hi = unscale(x[T + t]);
+        o[0] = (lo + hi) * 0.5f;
+        o[1] = hi - lo;
+        break;
+      }
+      default: {                                   // Dirichlet family: alpha = softplus + 1 per class
+        const float* xr = x + (int64_t)t * u;
+        if (kind == kDirichlet) {
+          for (int c = 0; c < u; ++c) o[c] = softplus20(xr[c]) + 1.f;
+          break;
+        }
+        float S = 0.f;
+        for (int c = 0; c < u; ++c) S += softplus20(xr[c]) + 1.f;
+        if (kind == kDirichletProbs) {
+          for (int c = 0; c < u; ++c) o[c] = (softplus20(xr[c]) + 1.f) / S;
+        } else {                                   // binary: (alpha_1 / S, 2 / S)
+          o[0] = (softplus20(xr[1]) + 1.f) / S;
+          o[1] = 2.f / S;
+        }
+      }
+    }
+  }
+}
+
+// mirror of k_pred_transform for kinds kRegression .. kDirichlet: dOut (B x T x u) -> dX (B x (T*u))
+__global__ void __launch_bounds__(256)
+k_pred_transform_bwd(const float* __restrict__ X, int64_t ldx, const float* __restrict__ dO, int64_t lddo, int64_t B, int T,
+                     int kind, int u, const float* __restrict__ scale, float* __restrict__ dX, int64_t lddx) {
+  const int64_t n = B * (int64_t)T;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / T;
+    const int t = (int)(i - b * T);
+    const float* x = X + b * ldx;
+    const float* g = dO + b * lddo + (int64_t)t * u;
+    float* d = dX + b * lddx;
+    const float s = scale ? scale[t] : 1.f, s2 = s * s;
+    switch (kind) {
+      case kRegression: d[t] = g[0] * s; break;
+      case kMve:
+        d[t] = g[0] * s;
+        d[T + t] = g[1] * s2 * softplus20_grad(x[T + t]);
+        break;
+      case kEvidential:
+        d[t] = g[0] * s;
+        d[T + t] = g[1] * softplus20_grad(x[T + t]);
+        d[2 * T + t] = g[2] * softplus20_grad(x[2 * T + t]);
+        d[3 * T + t] = g[3] * s2 * softplus20_grad(x[3 * T + t]);
+        break;
+      case kQuantile:                              // mean = (lo + hi) / 2, interval = hi - lo
+        d[t] = (0.5f * g[0] - g[1]) * s;
+        d[T + t] = (0.5f * g[0] + g[1]) * s;
+        break;
+      default:
+        for (int c = 0; c < u; ++c) d[(int64_t)t * u + c] = g[c] * softplus20_grad(x[(int64_t)t * u + c]);
+    }
+  }
+}
+
+__device__ __forceinline__ float loss_weight(const float* w, const float* tw, int64_t b, int t) {
+  return (w ? w[b] : 1.f) * (tw ? tw[t] : 1.f);
+}
+
+// MVELoss (metrics.py:213-219) on preds (mean, var): L = (mean - y)^2 / (2 var) + log(2 pi var) / 2
+__device__ __forceinline__ float mve_term(const float* p, float y, float* g) {
+  const float e = p[0] - y, v = p[1];
+  if (g) {
+    g[0] = e / v;
+    g[1] = 0.5f / v - e * e / (2.f * v * v);
+  }
+  return e * e / (2.f * v) + 0.5f * logf(2.f * CUDART_PI_F * v);
+}
+
+// EvidentialLoss (metrics.py:241-257) on preds (mean, v, alpha, beta); d|r|/dr = 0 at r = 0, as torch's abs
+__device__ __forceinline__ float evidential_term(const float* p, float y, float v_kl, float eps, float* g) {
+  const float mu = p[0], v = p[1], a = p[2], be = p[3];
+  const float r = y - mu, ar = fabsf(r);
+  const float om = 2.f * be * (1.f + v);
+  const float D = v * r * r + om;
+  if (g) {
+    const float sg = r > 0.f ? 1.f : (r < 0.f ? -1.f : 0.f);
+    g[0] = -(a + 0.5f) * 2.f * v * r / D - v_kl * (2.f * v + a) * sg;
+    g[1] = -0.5f / v - a * 2.f * be / om + (a + 0.5f) * (r * r + 2.f * be) / D + v_kl * 2.f * ar;
+    g[2] = -logf(om) + logf(D) + digamma_ge1(a) - digamma_ge1(a + 0.5f) + v_kl * ar;
+    g[3] = -a * 2.f * (1.f + v) / om + (a + 0.5f) * 2.f * (1.f + v) / D;
+  }
+  const float nll = 0.5f * logf(CUDART_PI_F / v) - a * logf(om) + (a + 0.5f) * logf(D) + lgammaf(a) - lgammaf(a + 0.5f);
+  return nll + v_kl * ((2.f * v + a) * ar - eps);
+}
+
+// amax over two candidates with torch's backward: a tie splits the gradient evenly
+__device__ __forceinline__ float amax2(float x0, float x1, float t0, float t1, float* dt) {
+  if (x0 > x1) { *dt = t0; return x0; }
+  if (x1 > x0) { *dt = t1; return x1; }
+  *dt = 0.5f * (t0 + t1);
+  return x0;
+}
+
+// QuantileLoss (metrics.py:602-610) on preds (mean, interval): bounds mean -/+ interval / 2, pinball loss at alpha / 2 and
+// 1 - alpha / 2 with tau = [[alpha/2, 1 - alpha/2], [alpha/2 - 1, -alpha/2]]
+__device__ __forceinline__ float quantile_term(const float* p, float y, float alpha, float* g) {
+  const float m = p[0], I = p[1];
+  const float e0 = y - (m + (-0.5f) * I), e1 = y - (m + 0.5f * I);
+  const float ta = 0.5f * alpha;
+  float d0, d1;
+  const float l0 = amax2(ta * e0, (ta - 1.f) * e0, ta, ta - 1.f, &d0);
+  const float l1 = amax2((1.f - ta) * e1, -ta * e1, 1.f - ta, -ta, &d1);
+  if (g) {
+    g[0] = -(d0 + d1);
+    g[1] = 0.5f * d0 - 0.5f * d1;
+  }
+  return l0 + l1;
+}
+
+// label of torch.eye(C)[targets.long()]: truncation, then [-C, 0) counts from the end; -1 where torch would raise
+__device__ __forceinline__ int wrapped_class_of(float y, int C) {
+  const float k = truncf(y);
+  if (k >= 0.f && k < (float)C) return (int)k;
+  if (k < 0.f && k >= -(float)C) return (int)k + C;
+  return -1;
+}
+
+// DirichletLoss (metrics.py:517-541) on alpha (C entries): L = sum (onehot - p)^2 + sum p (1 - p) / (S + 1) + v_kl KL, with
+// KL = lgamma(Sa) - sum lgamma(a~) - lgamma(C) + sum (a~ - 1)(psi(a~) - psi(Sa)), a~ = onehot + (1 - onehot) alpha
+__device__ __forceinline__ float dirichlet_term(const float* a, float y, int C, float v_kl, float* g) {
+  const int k = wrapped_class_of(y, C);
+  if (k < 0) {
+    if (g) for (int c = 0; c < C; ++c) g[c] = CUDART_NAN_F;
+    return CUDART_NAN_F;
+  }
+  float S = 0.f, Sa = 0.f;
+  for (int c = 0; c < C; ++c) {
+    S += a[c];
+    Sa += c == k ? 1.f : a[c];
+  }
+  float A = 0.f, Bq = 0.f, sp = 0.f, sp2 = 0.f, lg = 0.f, kl = 0.f, sam1 = 0.f;
+  const float psiS = digamma_ge1(Sa);
+  for (int c = 0; c < C; ++c) {
+    const float p = a[c] / S, yc = c == k ? 1.f : 0.f, at = c == k ? 1.f : a[c];
+    A += (yc - p) * (yc - p);
+    Bq += p * (1.f - p);
+    sp += p;
+    sp2 += p * p;
+    lg += lgammaf(at);
+    kl += (at - 1.f) * (digamma_ge1(at) - psiS);
+    sam1 += at - 1.f;
+  }
+  if (g) {
+    const float pk = a[k] / S, inv1 = 1.f / (S + 1.f), tS = trigamma_ge1(Sa);
+    for (int c = 0; c < C; ++c) {
+      const float p = a[c] / S, yc = c == k ? 1.f : 0.f;
+      const float dA = -2.f / S * ((yc - p) - (pk - sp2));
+      const float dB = ((1.f - 2.f * p) - sp + 2.f * sp2) / S * inv1 - Bq * inv1 * inv1;
+      const float dK = c == k ? 0.f : (a[c] - 1.f) * trigamma_ge1(a[c]) - tS * sam1;
+      g[c] = dA + dB + v_kl * dK;
+    }
+  }
+  return A + Bq * (1.f / (S + 1.f)) + v_kl * (lgammaf(Sa) - lg - lgammaf((float)C) + kl);
+}
+
+// one block; row (b, t) = preds P[b, t*u : (t+1)*u].  loss[0] = sum w_b tw_t m_bt L / sum m, dP = dL/dP w tw m / sum m
+template <int KIND>
+__global__ void __launch_bounds__(1024)
+k_uq_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y, int64_t ldy, const float* __restrict__ w,
+          const float* __restrict__ tw, int64_t B, int T, int u, float p1, float p2, float* __restrict__ loss,
+          float* __restrict__ dP, int64_t lddp) {
+  const int64_t n = B * (int64_t)T;
+  auto term = [&](const float* p, float y, float* g) {
+    if constexpr (KIND == kMve) return mve_term(p, y, g);
+    else if constexpr (KIND == kEvidential) return evidential_term(p, y, p1, p2, g);
+    else if constexpr (KIND == kQuantile) return quantile_term(p, y, p1, g);
+    else return dirichlet_term(p, y, u, p1, g);
+  };
+  float l = 0.f, cnt = 0.f;
+  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const int64_t b = i / T;
+    const int t = (int)(i - b * T);
+    const float y = Y[b * ldy + t];
+    if (!isfinite(y)) continue;
+    l = fmaf(loss_weight(w, tw, b, t), term(P + b * ldp + (int64_t)t * u, y, nullptr), l);
+    cnt += 1.f;
+  }
+  const float2 tot = block_sum2(l, cnt);
+  if (threadIdx.x == 0) loss[0] = tot.y > 0.f ? tot.x / tot.y : 0.f;
+  const float inv_n = tot.y > 0.f ? 1.f / tot.y : 0.f;
+  if (dP != nullptr)
+    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+      const int64_t b = i / T;
+      const int t = (int)(i - b * T);
+      const float y = Y[b * ldy + t];
+      float* d = dP + b * lddp + (int64_t)t * u;
+      if (!isfinite(y)) {
+        for (int c = 0; c < u; ++c) d[c] = 0.f;
+        continue;
+      }
+      term(P + b * ldp + (int64_t)t * u, y, d);
+      const float sc = loss_weight(w, tw, b, t) * inv_n;
+      for (int c = 0; c < u; ++c) d[c] *= sc;
+    }
+}
+
 }  // namespace head
 }  // namespace dmpnn
 
@@ -373,4 +635,92 @@ extern "C" int dmpnn_class_probs(const float* P, int64_t ldp, int64_t B, int64_t
   head::k_class_probs<<<blocks, 256, 0, st>>>(P, ldp, B, (int)T, (int)C, softmax, out, ldo);
   DMPNN_CHECK_LAUNCH("class_probs", 1);
   return 0;
+}
+
+// outputs per task of each kind; 0 = any u >= 1 (the Dirichlet kinds: the number of classes)
+static int pred_kind_u(int kind) {
+  switch (kind) {
+    case head::kRegression: return 1;
+    case head::kMve: case head::kQuantile: case head::kDirichletBinary: return 2;
+    case head::kEvidential: return 4;
+    default: return 0;
+  }
+}
+
+extern "C" int dmpnn_pred_transform(const float* X, int64_t ldx, int64_t B, int64_t T, int kind, int64_t u,
+                                    const float* mean, const float* scale, float* out, int64_t ldo, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(kind >= head::kRegression && kind <= head::kDirichletBinary, "pred_transform: unknown kind");
+  DMPNN_CHECK_ARG(B >= 0 && T > 0 && u > 0 && T * u <= INT32_MAX && (B == 0 || (X && out)), "pred_transform: bad args");
+  DMPNN_CHECK_ARG(pred_kind_u(kind) == 0 || pred_kind_u(kind) == u, "pred_transform: u does not match the kind");
+  DMPNN_CHECK_ARG((mean == nullptr && scale == nullptr) || (kind <= head::kQuantile && mean && scale),
+                  "pred_transform: mean and scale go together, and only with the regression kinds");
+  DMPNN_CHECK_ARG(ldx >= T * u && ldo >= T * u, "pred_transform: row strides too small");
+  if (B == 0) return 0;
+  const unsigned blocks = (unsigned)std::min<int64_t>((B * T + 255) / 256, 1024);
+  head::k_pred_transform<<<blocks, 256, 0, st>>>(X, ldx, B, (int)T, kind, (int)u, mean, scale, out, ldo);
+  DMPNN_CHECK_LAUNCH("pred_transform", 1);
+  return 0;
+}
+
+extern "C" int dmpnn_pred_transform_bwd(const float* X, int64_t ldx, const float* dOut, int64_t lddo, int64_t B, int64_t T,
+                                        int kind, int64_t u, const float* scale, float* dX, int64_t lddx, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(kind >= head::kRegression && kind <= head::kDirichlet, "pred_transform_bwd: unknown kind");
+  DMPNN_CHECK_ARG(B >= 0 && T > 0 && u > 0 && T * u <= INT32_MAX && (B == 0 || (X && dOut && dX)),
+                  "pred_transform_bwd: bad args");
+  DMPNN_CHECK_ARG(pred_kind_u(kind) == 0 || pred_kind_u(kind) == u, "pred_transform_bwd: u does not match the kind");
+  DMPNN_CHECK_ARG(scale == nullptr || kind <= head::kQuantile, "pred_transform_bwd: scale only with the regression kinds");
+  DMPNN_CHECK_ARG(ldx >= T * u && lddo >= T * u && lddx >= T * u, "pred_transform_bwd: row strides too small");
+  if (B == 0) return 0;
+  const unsigned blocks = (unsigned)std::min<int64_t>((B * T + 255) / 256, 1024);
+  head::k_pred_transform_bwd<<<blocks, 256, 0, st>>>(X, ldx, dOut, lddo, B, (int)T, kind, (int)u, scale, dX, lddx);
+  DMPNN_CHECK_LAUNCH("pred_transform_bwd", 1);
+  return 0;
+}
+
+// shared host checks and launch of the four uncertainty losses (u outputs per task)
+template <int KIND>
+static int uq_loss(const char* name, const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                   const float* task_weights, int64_t B, int64_t T, int64_t u, float p1, float p2, float* loss, float* dP,
+                   int64_t lddp, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(B >= 0 && T > 0 && u > 0 && T * u <= INT32_MAX && loss && (B == 0 || (P && Y)), name);
+  DMPNN_CHECK_ARG(ldp >= T * u && ldy >= T && (dP == nullptr || lddp >= T * u), name);
+  head::k_uq_loss<KIND><<<1, 1024, 0, st>>>(P, ldp, Y, ldy, weights, task_weights, B, (int)T, (int)u, p1, p2, loss, dP,
+                                              lddp);
+  DMPNN_CHECK_LAUNCH(name, 1);
+  return 0;
+}
+
+extern "C" int dmpnn_mve_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                              const float* task_weights, int64_t B, int64_t T, float* loss, float* dP, int64_t lddp,
+                              void* stream) {
+  return uq_loss<head::kMve>("mve_loss: bad args or row strides too small", P, ldp, Y, ldy, weights, task_weights, B, T, 2,
+                             0.f, 0.f, loss, dP, lddp, stream);
+}
+
+extern "C" int dmpnn_evidential_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                                     const float* task_weights, int64_t B, int64_t T, float v_kl, float eps, float* loss,
+                                     float* dP, int64_t lddp, void* stream) {
+  DMPNN_CHECK_ARG(std::isfinite(v_kl) && std::isfinite(eps), "evidential_loss: v_kl and eps must be finite");
+  return uq_loss<head::kEvidential>("evidential_loss: bad args or row strides too small", P, ldp, Y, ldy, weights,
+                                    task_weights, B, T, 4, v_kl, eps, loss, dP, lddp, stream);
+}
+
+extern "C" int dmpnn_quantile_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                                   const float* task_weights, int64_t B, int64_t T, float alpha, float* loss, float* dP,
+                                   int64_t lddp, void* stream) {
+  DMPNN_CHECK_ARG(std::isfinite(alpha), "quantile_loss: alpha must be finite");
+  return uq_loss<head::kQuantile>("quantile_loss: bad args or row strides too small", P, ldp, Y, ldy, weights, task_weights,
+                                  B, T, 2, alpha, 0.f, loss, dP, lddp, stream);
+}
+
+extern "C" int dmpnn_dirichlet_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                                    const float* task_weights, int64_t B, int64_t T, int64_t C, float v_kl, float* loss,
+                                    float* dP, int64_t lddp, void* stream) {
+  DMPNN_CHECK_ARG(std::isfinite(v_kl), "dirichlet_loss: v_kl must be finite");
+  DMPNN_CHECK_ARG(C >= 1, "dirichlet_loss: bad args (C must be >= 1)");
+  return uq_loss<head::kDirichlet>("dirichlet_loss: bad args or row strides too small", P, ldp, Y, ldy, weights,
+                                   task_weights, B, T, C, v_kl, 0.f, loss, dP, lddp, stream);
 }

@@ -627,6 +627,65 @@ def class_probs(P: Tensor, C: int, softmax: bool, out: Tensor):
     _lib.check(rc, "dmpnn_class_probs")
 
 
+def pred_transform(X: Tensor, kind: int, u: int, mean, scale, out: Tensor):
+    """out (B x T*u, read as B x T x u) = the predictor output of `kind` (_lib.PRED_*) from the raw MLP output X (B x T*u);
+    mean / scale (T entries each, or None) apply UnscaleTransform's eval mode."""
+    lib = _lib.load()
+    B, Tu = X.shape
+    rc = lib.dmpnn_pred_transform(X.data_ptr(), X.stride(0) if B else Tu, B, Tu // u, kind, u, _ptr(mean), _ptr(scale),
+                                  out.data_ptr(), out.stride(0) if B else Tu, _stream())
+    _lib.check(rc, "dmpnn_pred_transform")
+
+
+def pred_transform_bwd(X: Tensor, dOut: Tensor, kind: int, u: int, scale, dX: Tensor):
+    lib = _lib.load()
+    B, Tu = X.shape
+    rc = lib.dmpnn_pred_transform_bwd(X.data_ptr(), X.stride(0) if B else Tu, dOut.data_ptr(), dOut.stride(0) if B else Tu, B,
+                                      Tu // u, kind, u, _ptr(scale), dX.data_ptr(), dX.stride(0) if B else Tu, _stream())
+    _lib.check(rc, "dmpnn_pred_transform_bwd")
+
+
+def _uq_args(P: Tensor, Y: Tensor, u: int):
+    B, Tu = P.shape
+    T = Y.shape[1]
+    return P.data_ptr(), P.stride(0) if B else Tu, Y.data_ptr(), Y.stride(0) if B else T, B, T
+
+
+def mve_loss(P: Tensor, Y: Tensor, w, tw, loss: Tensor, dP: Tensor):
+    """P: B x (T*2) = (mean, var) per task, Y: B x T."""
+    lib = _lib.load()
+    p, ldp, y, ldy, B, T = _uq_args(P, Y, 2)
+    rc = lib.dmpnn_mve_loss(p, ldp, y, ldy, _ptr(w), _ptr(tw), B, T, loss.data_ptr(), _ptr(dP), ldp, _stream())
+    _lib.check(rc, "dmpnn_mve_loss")
+
+
+def evidential_loss(P: Tensor, Y: Tensor, w, tw, v_kl: float, eps: float, loss: Tensor, dP: Tensor):
+    """P: B x (T*4) = (mean, v, alpha, beta) per task, Y: B x T."""
+    lib = _lib.load()
+    p, ldp, y, ldy, B, T = _uq_args(P, Y, 4)
+    rc = lib.dmpnn_evidential_loss(p, ldp, y, ldy, _ptr(w), _ptr(tw), B, T, float(v_kl), float(eps), loss.data_ptr(),
+                                   _ptr(dP), ldp, _stream())
+    _lib.check(rc, "dmpnn_evidential_loss")
+
+
+def quantile_loss(P: Tensor, Y: Tensor, w, tw, alpha: float, loss: Tensor, dP: Tensor):
+    """P: B x (T*2) = (mean, interval) per task, Y: B x T."""
+    lib = _lib.load()
+    p, ldp, y, ldy, B, T = _uq_args(P, Y, 2)
+    rc = lib.dmpnn_quantile_loss(p, ldp, y, ldy, _ptr(w), _ptr(tw), B, T, float(alpha), loss.data_ptr(), _ptr(dP), ldp,
+                                 _stream())
+    _lib.check(rc, "dmpnn_quantile_loss")
+
+
+def dirichlet_loss(P: Tensor, Y: Tensor, w, tw, C: int, v_kl: float, loss: Tensor, dP: Tensor):
+    """P: B x (T*C) = alpha per task and class, Y: B x T class labels."""
+    lib = _lib.load()
+    p, ldp, y, ldy, B, T = _uq_args(P, Y, C)
+    rc = lib.dmpnn_dirichlet_loss(p, ldp, y, ldy, _ptr(w), _ptr(tw), B, T, C, float(v_kl), loss.data_ptr(), _ptr(dP), ldp,
+                                  _stream())
+    _lib.check(rc, "dmpnn_dirichlet_loss")
+
+
 def column_sum(Y: Tensor, R: int, N: int, out: Tensor, *, accumulate: bool = False):
     lib = _lib.load()
     n = C.c_size_t(0)

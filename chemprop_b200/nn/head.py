@@ -2,7 +2,12 @@
 after the encoder -- `H = agg(H_v, batch)`, `H = bn(H)`, `preds = predictor(H)`, `loss = criterion(preds, targets, mask, w)`
 (chemprop/models/model.py:126-161, nn/ffn.py:38-61, nn/predictors.py:101-170, 231-317, nn/metrics.py:78-123, 139-141,
 291-303) -- for regression and classification: Mean / Sum / Norm aggregation, optional BatchNorm1d, the MLP of
-`RegressionFFN` / `BinaryClassificationFFN` / `MulticlassClassificationFFN`, masked + weighted MSE, BCE or cross-entropy.
+`RegressionFFN` / `BinaryClassificationFFN` / `MulticlassClassificationFFN`, masked + weighted MSE, BCE or cross-entropy;
+and for chemprop's uncertainty predictors `MveFFN` / `EvidentialFFN` / `QuantileFFN` / `BinaryDirichletFFN` /
+`MulticlassDirichletFFN` (predictors.py:172-228, 250-270, 319-336) with their criteria (metrics.py:202-257, 502-544,
+588-613): the MLP output goes through dmpnn_pred_transform (softplus, + 1, eval-mode unscaling; mirror
+dmpnn_pred_transform_bwd), the criterion is one launch (dmpnn_mve_loss / dmpnn_evidential_loss / dmpnn_quantile_loss /
+dmpnn_dirichlet_loss).
 
 Every arithmetic step is a libdmpnn launch (aggregation: dmpnn_segment_sum; batch norm: dmpnn_bn_train_fwd / dmpnn_bn_bwd;
 the MLP's GEMMs: dmpnn_linear_fwd / dmpnn_linear_wgrad with the activation in the epilogue; the criterion and its gradient:
@@ -192,6 +197,73 @@ class ClassProbsFunction(torch.autograd.Function):
         return (p3 * (g3 - (g3 * p3).sum(-1, keepdim=True))).view(b, n).to(dt), None, None
 
 
+class PredTransformFunction(torch.autograd.Function):
+    """Raw MLP output X (b x T*u) -> the predictor output (b x T x u) of `kind` (_lib.PRED_*) in one launch
+    (dmpnn_pred_transform), with UnscaleTransform's eval mode when mean / scale are given.  Mirror: dmpnn_pred_transform_bwd
+    for the training outputs; the eval-only Dirichlet probabilities take theirs in torch, as ClassProbsFunction does."""
+
+    @staticmethod
+    def forward(ctx, X, kind, u, mean, scale):
+        K._require_cuda(X)
+        Xc = X.float().contiguous()
+        m = None if mean is None else mean.detach().float().reshape(-1).contiguous()
+        s = None if scale is None else scale.detach().float().reshape(-1).contiguous()
+        out = torch.empty_like(Xc)
+        K.pred_transform(Xc, kind, u, m, s, out)
+        ctx.save_for_backward(Xc, s)
+        ctx.cfg = (kind, u, X.dtype)
+        return out.view(Xc.shape[0], Xc.shape[1] // u, u)
+
+    @staticmethod
+    def backward(ctx, g):
+        Xc, s = ctx.saved_tensors
+        kind, u, dt = ctx.cfg
+        b, n = Xc.shape
+        g = g.float().reshape(b, n).contiguous()
+        if kind <= _lib.PRED_DIRICHLET:
+            dX = torch.empty_like(Xc)
+            K.pred_transform_bwd(Xc, g, kind, u, s, dX)
+        else:
+            with torch.enable_grad():
+                x = Xc.detach().requires_grad_(True)
+                a = torch.nn.functional.softplus(x.view(b, n // u, u)) + 1
+                S = a.sum(-1, keepdim=True)
+                y = a / S if kind == _lib.PRED_DIRICHLET_PROBS else torch.stack(((a / S)[..., 1], 2 / S[..., 0]), 2)
+                (dX,) = torch.autograd.grad(y, x, g.view_as(y))
+        return dX.to(dt), None, None, None, None
+
+
+class UncertaintyLossFunction(torch.autograd.Function):
+    """The uncertainty criteria on b x T x u predictions under the MSE criterion's reduction: loss and dLoss/dPreds in one
+    launch (engine.<name>: dmpnn_mve_loss / dmpnn_evidential_loss / dmpnn_quantile_loss / dmpnn_dirichlet_loss)."""
+
+    @staticmethod
+    def forward(ctx, preds, targets, weights, task_weights, name, args):
+        K._require_cuda(preds, targets)
+        b, T, u = preds.shape
+        if targets.shape != (b, T):
+            raise ValueError(f"targets must be {b} x {T}, got {tuple(targets.shape)}")
+        P, Y = preds.float().reshape(b, T * u).contiguous(), targets.float().contiguous()
+        w = None if weights is None else weights.float().reshape(-1).contiguous()
+        tw = None if task_weights is None else task_weights.float().reshape(-1)
+        if tw is not None and tw.numel() == 1:                 # a scalar task weight broadcasts, as in the reference
+            tw = tw.expand(T)
+        if (w is not None and w.numel() != b) or (tw is not None and tw.numel() != T):
+            raise ValueError(f"weights must have {b} entries and task_weights 1 or {T}")
+        tw = None if tw is None else tw.contiguous()
+        loss = torch.empty(1, device=P.device)
+        dP = torch.empty_like(P)
+        getattr(K, name)(P, Y, w, tw, *args, loss, dP)
+        ctx.save_for_backward(dP.view(b, T, u))
+        ctx.pdtype = preds.dtype
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        (dP,) = ctx.saved_tensors
+        return (dP * g).to(ctx.pdtype), None, None, None, None, None
+
+
 class _Criterion(nn.Module):
     """chemprop's `ChempropMetric` interface (nn/metrics.py:59-123) around one loss kernel: `task_weights` buffer (1 x T),
     NaN targets or `mask` select the terms, `weights` are per molecule."""
@@ -205,7 +277,10 @@ class _Criterion(nn.Module):
         if lt_mask is not None or gt_mask is not None:
             raise NotImplementedError("bounded MSE is not part of the engine's head; use the reference criterion")
         t = targets if mask is None else torch.where(mask, targets, torch.full_like(targets, float("nan")))
-        return self._loss_fn.apply(preds, t, weights, self.task_weights)
+        return self._loss(preds, t, weights)
+
+    def _loss(self, preds, targets, weights):
+        return self._loss_fn.apply(preds, targets, weights, self.task_weights)
 
 
 class _BCECriterion(_Criterion):
@@ -218,17 +293,85 @@ class _CrossEntropyCriterion(_Criterion):
     _loss_fn = CrossEntropyLossFunction
 
 
+class EngineMVELoss(_Criterion):
+    """chemprop's MVELoss (nn/metrics.py:202-219) on b x T x 2 (mean, var) predictions (dmpnn_mve_loss)."""
+
+    def __init__(self, task_weights=1.0):
+        super().__init__(task_weights)
+
+    def _loss(self, preds, targets, weights):
+        return UncertaintyLossFunction.apply(preds, targets, weights, self.task_weights, "mve_loss", ())
+
+
+class EngineEvidentialLoss(_Criterion):
+    """chemprop's EvidentialLoss (nn/metrics.py:222-260) on b x T x 4 (mean, v, alpha, beta) predictions
+    (dmpnn_evidential_loss)."""
+
+    def __init__(self, task_weights=1.0, v_kl: float = 0.2, eps: float = 1e-8):
+        super().__init__(task_weights)
+        self.v_kl = v_kl
+        self.eps = eps
+
+    def _loss(self, preds, targets, weights):
+        return UncertaintyLossFunction.apply(preds, targets, weights, self.task_weights, "evidential_loss",
+                                             (self.v_kl, self.eps))
+
+    def extra_repr(self) -> str:
+        return f"v_kl={self.v_kl}, eps={self.eps}"
+
+
+class EngineQuantileLoss(_Criterion):
+    """chemprop's QuantileLoss (nn/metrics.py:588-613) on b x T x 2 (mean, interval) predictions (dmpnn_quantile_loss); the
+    `bounds` and `tau` buffers are the reference's, so that its state dicts load strictly."""
+
+    def __init__(self, task_weights=1.0, alpha: float = 0.1):
+        super().__init__(task_weights)
+        self.alpha = alpha
+        self.register_buffer("bounds", torch.tensor([-1 / 2, 1 / 2]).view(-1, 1, 1))
+        self.register_buffer("tau", torch.tensor([[alpha / 2, 1 - alpha / 2], [alpha / 2 - 1, -alpha / 2]]).view(2, 2, 1, 1))
+
+    def _loss(self, preds, targets, weights):
+        return UncertaintyLossFunction.apply(preds, targets, weights, self.task_weights, "quantile_loss", (self.alpha,))
+
+    def extra_repr(self) -> str:
+        return f"alpha={self.alpha}"
+
+
+class EngineDirichletLoss(_Criterion):
+    """chemprop's DirichletLoss (nn/metrics.py:502-544) on b x T x C concentrations alpha and b x T class labels
+    (dmpnn_dirichlet_loss)."""
+
+    def __init__(self, task_weights=1.0, v_kl: float = 0.2):
+        super().__init__(task_weights)
+        self.v_kl = v_kl
+
+    def _loss(self, preds, targets, weights):
+        return UncertaintyLossFunction.apply(preds, targets, weights, self.task_weights, "dirichlet_loss",
+                                             (preds.shape[2], self.v_kl))
+
+    def extra_repr(self) -> str:
+        return f"v_kl={self.v_kl}"
+
+
 class _EngineFFNPredictor(nn.Module):
-    """`_FFNPredictorBase` (chemprop/nn/predictors.py:101-157) with the reference's module tree; GEMMs on the engine."""
+    """`_FFNPredictorBase` (chemprop/nn/predictors.py:101-157) with the reference's module tree; GEMMs on the engine.  The
+    MLP has n_tasks * n_targets outputs.  `criterion` replaces the default criterion (built from `task_weights`), and
+    `output_transform` (an UnscaleTransform) unscales the regression predictors' outputs in eval mode; each is recorded in
+    `hparams` when given."""
     n_targets = 1
     _criterion_cls = _Criterion
 
     def __init__(self, n_tasks: int = 1, input_dim: int = DEFAULT_HIDDEN_DIM, hidden_dim: int | Sequence[int] = 300,
-                 n_layers: int = 1, dropout: float = 0.0, activation="relu", task_weights=None):
+                 n_layers: int = 1, dropout: float = 0.0, activation="relu", task_weights=None, *, criterion=None,
+                 output_transform=None):
         super().__init__()
         self.hparams = dict(n_tasks=n_tasks, input_dim=input_dim, hidden_dim=hidden_dim, n_layers=n_layers, dropout=dropout,
                             activation=activation, cls=self.__class__)
-        ffn = build_mlp(input_dim, n_tasks, hidden_dim, n_layers, dropout, activation)
+        if criterion is not None:
+            self.hparams["criterion"] = criterion
+        if output_transform is not None:
+            self.hparams["output_transform"] = output_transform
+        ffn = build_mlp(input_dim, n_tasks * self.n_targets, hidden_dim, n_layers, dropout, activation)
         for block in ffn:                         # same tree, engine-backed Linear layers
             for i, m in enumerate(block):
                 if isinstance(m, nn.Linear):
@@ -236,8 +379,9 @@ class _EngineFFNPredictor(nn.Module):
                     e.load_state_dict(m.state_dict())
                     block[i] = e
         self.ffn = ffn
-        self.criterion = self._criterion_cls(torch.ones(n_tasks) if task_weights is None else task_weights)
-        self.output_transform = nn.Identity()
+        self.criterion = criterion if criterion is not None else self._criterion_cls(
+            torch.ones(n_tasks) if task_weights is None else task_weights)
+        self.output_transform = output_transform if output_transform is not None else nn.Identity()
 
     @property
     def input_dim(self) -> int:
@@ -249,7 +393,7 @@ class _EngineFFNPredictor(nn.Module):
 
     @property
     def n_tasks(self) -> int:
-        return self.output_dim
+        return self.output_dim // self.n_targets
 
     def _mlp(self, Z: Tensor) -> Tensor:
         """`self.ffn(Z)` (nn/ffn.py:38-61: Linear, then [act, dropout, Linear] per further layer) with every activation the
@@ -271,12 +415,49 @@ class _EngineFFNPredictor(nn.Module):
 
 
 class EngineRegressionFFN(_EngineFFNPredictor):
-    """`RegressionFFN` (chemprop/nn/predictors.py:156-164) with the reference's module tree; GEMMs on the engine."""
+    """`RegressionFFN` (chemprop/nn/predictors.py:160-169) with the reference's module tree; GEMMs on the engine.  With an
+    UnscaleTransform as `output_transform`, eval-mode predictions are `Y * scale + mean` (dmpnn_pred_transform)."""
+    _kind = _lib.PRED_REGRESSION
+
+    def _unscale(self):
+        t = self.output_transform
+        if isinstance(t, nn.Identity) or t.training:      # UnscaleTransform is the identity in training mode
+            return None, None
+        return t.mean, t.scale
 
     def forward(self, Z: Tensor) -> Tensor:
-        return self.output_transform(self._mlp(Z))
+        Y = self._mlp(Z)
+        mean, scale = self._unscale()
+        if self._kind == _lib.PRED_REGRESSION:
+            return Y if mean is None else PredTransformFunction.apply(Y, self._kind, 1, mean, scale).view(Y.shape)
+        return PredTransformFunction.apply(Y, self._kind, self.n_targets, mean, scale)
 
     train_step = forward
+
+
+class EngineMveFFN(EngineRegressionFFN):
+    """`MveFFN` (chemprop/nn/predictors.py:172-188): b x T x 2 (mean, softplus(var)); in eval mode with an output transform
+    the mean is unscaled and the variance multiplied by scale^2.  Criterion: EngineMVELoss."""
+    n_targets = 2
+    _kind = _lib.PRED_MVE
+    _criterion_cls = EngineMVELoss
+
+
+class EngineEvidentialFFN(EngineRegressionFFN):
+    """`EvidentialFFN` (chemprop/nn/predictors.py:191-209): b x T x 4 (mean, softplus(v), softplus(alpha) + 1,
+    softplus(beta)); in eval mode with an output transform the mean is unscaled and beta multiplied by scale^2.
+    Criterion: EngineEvidentialLoss."""
+    n_targets = 4
+    _kind = _lib.PRED_EVIDENTIAL
+    _criterion_cls = EngineEvidentialLoss
+
+
+class EngineQuantileFFN(EngineRegressionFFN):
+    """`QuantileFFN` (chemprop/nn/predictors.py:212-228): b x T x 2 (mean, interval) of the two predicted bounds, each
+    unscaled in eval mode with an output transform.  Criterion: EngineQuantileLoss."""
+    n_targets = 2
+    _kind = _lib.PRED_QUANTILE
+    _criterion_cls = EngineQuantileLoss
 
 
 class EngineBinaryClassificationFFN(_EngineFFNPredictor):
@@ -299,21 +480,48 @@ class EngineMulticlassClassificationFFN(_EngineFFNPredictor):
 
     def __init__(self, n_classes: int, n_tasks: int = 1, input_dim: int = DEFAULT_HIDDEN_DIM,
                  hidden_dim: int | Sequence[int] = 300, n_layers: int = 1, dropout: float = 0.0, activation="relu",
-                 task_weights=None):
+                 task_weights=None, *, criterion=None, output_transform=None):
         task_weights = torch.ones(n_tasks) if task_weights is None else task_weights
-        super().__init__(n_tasks * n_classes, input_dim, hidden_dim, n_layers, dropout, activation, task_weights)
+        super().__init__(n_tasks * n_classes, input_dim, hidden_dim, n_layers, dropout, activation, task_weights,
+                         criterion=criterion, output_transform=output_transform)
         self.n_classes = n_classes
         self.hparams.update(n_tasks=n_tasks, n_classes=n_classes)
 
     @property
     def n_tasks(self) -> int:
-        return self.output_dim // self.n_classes
+        return self.output_dim // (self.n_targets * self.n_classes)
 
     def forward(self, Z: Tensor) -> Tensor:
         return ClassProbsFunction.apply(self._mlp(Z), self.n_classes, True).reshape(Z.shape[0], -1, self.n_classes)
 
     def train_step(self, Z: Tensor) -> Tensor:
         return self._mlp(Z).reshape(Z.shape[0], -1, self.n_classes)
+
+
+class EngineBinaryDirichletFFN(_EngineFFNPredictor):
+    """`BinaryDirichletFFN` (chemprop/nn/predictors.py:250-269): the MLP has 2 outputs per task, task t in columns
+    [2t, 2t + 2); `train_step` gives alpha = softplus + 1 as b x T x 2, `forward` the b x T x 2 pair (alpha_1 / S, 2 / S)
+    (dmpnn_pred_transform).  Criterion: EngineDirichletLoss."""
+    n_targets = 2
+    _criterion_cls = EngineDirichletLoss
+
+    def forward(self, Z: Tensor) -> Tensor:
+        return PredTransformFunction.apply(self._mlp(Z), _lib.PRED_DIRICHLET_BINARY, 2, None, None)
+
+    def train_step(self, Z: Tensor) -> Tensor:
+        return PredTransformFunction.apply(self._mlp(Z), _lib.PRED_DIRICHLET, 2, None, None)
+
+
+class EngineMulticlassDirichletFFN(EngineMulticlassClassificationFFN):
+    """`MulticlassDirichletFFN` (chemprop/nn/predictors.py:319-336): `train_step` gives alpha = softplus + 1 as b x T x C,
+    `forward` alpha / sum(alpha) (dmpnn_pred_transform).  Criterion: EngineDirichletLoss."""
+    _criterion_cls = EngineDirichletLoss
+
+    def forward(self, Z: Tensor) -> Tensor:
+        return PredTransformFunction.apply(self._mlp(Z), _lib.PRED_DIRICHLET_PROBS, self.n_classes, None, None)
+
+    def train_step(self, Z: Tensor) -> Tensor:
+        return PredTransformFunction.apply(self._mlp(Z), _lib.PRED_DIRICHLET, self.n_classes, None, None)
 
 
 class EngineBatchNorm1d(nn.BatchNorm1d):
@@ -337,21 +545,24 @@ class EngineBatchNorm1d(nn.BatchNorm1d):
 class EngineMPNN(nn.Module):
     """`chemprop.models.MPNN` reduced to the path (models/model.py:66-161): message passing -> aggregation -> batch norm ->
     predictor -> criterion, all on the engine.  The predictor is EngineRegressionFFN (the default),
-    EngineBinaryClassificationFFN or EngineMulticlassClassificationFFN.  `training_loss(bmg, targets, weights=None)` is
-    `MPNN.training_step` without Lightning's logging; `forward(bmg)` gives the predictions (probabilities for the
-    classification predictors)."""
+    EngineBinaryClassificationFFN, EngineMulticlassClassificationFFN or one of the uncertainty predictors (EngineMveFFN,
+    EngineEvidentialFFN, EngineQuantileFFN, EngineBinaryDirichletFFN, EngineMulticlassDirichletFFN).
+    `training_loss(bmg, targets, weights=None)` is `MPNN.training_step` without Lightning's logging; `forward(bmg)` gives
+    the predictions (probabilities for the classification predictors).  `X_d_transform` (a ScaleTransform, as
+    models/model.py:97) scales extra molecule descriptors X_d in eval mode before they join the fingerprint."""
 
     def __init__(self, message_passing: nn.Module, agg: Aggregation | None = None, predictor: nn.Module | None = None,
-                 batch_norm: bool = False):
+                 batch_norm: bool = False, X_d_transform: nn.Module | None = None):
         super().__init__()
         self.message_passing = message_passing
         self.agg = agg if agg is not None else MeanAggregation()
         self.bn = EngineBatchNorm1d(message_passing.output_dim) if batch_norm else nn.Identity()
         self.predictor = predictor if predictor is not None else EngineRegressionFFN(input_dim=message_passing.output_dim)
+        self.X_d_transform = X_d_transform if X_d_transform is not None else nn.Identity()
 
     def fingerprint(self, bmg, V_d: Tensor | None = None, X_d: Tensor | None = None) -> Tensor:
         H = self.bn(self.agg(self.message_passing(bmg, V_d), bmg.batch))
-        return H if X_d is None else torch.cat((H, X_d), dim=1)
+        return H if X_d is None else torch.cat((H, self.X_d_transform(X_d)), dim=1)
 
     def forward(self, bmg, V_d: Tensor | None = None, X_d: Tensor | None = None) -> Tensor:
         return self.predictor(self.fingerprint(bmg, V_d, X_d))

@@ -497,6 +497,54 @@ int dmpnn_ce_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, cons
 int dmpnn_class_probs(const float* P, int64_t ldp, int64_t B, int64_t T, int64_t C, int softmax, float* out, int64_t ldo,
                       void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Uncertainty predictors and target unscaling (csrc/head.cu; chemprop/nn/predictors.py:160-228, 250-270, 319-336,
+ * nn/transforms.py:45-55, nn/metrics.py:202-257, 502-544, 588-613):
+ *   dmpnn_pred_transform      X (B x (T*u), the raw MLP output) -> out (B x T x u, row stride ldo >= T*u), one thread per
+ *                             (b, t).  kind / u:
+ *                               0 regression (u = 1)       out = x
+ *                               1 MVE (u = 2)              (mean, softplus(var))
+ *                               2 evidential (u = 4)       (mean, softplus(v), softplus(alpha) + 1, softplus(beta))
+ *                               3 quantile (u = 2)         (lo + hi) / 2, hi - lo
+ *                               4 Dirichlet (u = C >= 1)   alpha = softplus(x) + 1
+ *                               5 Dirichlet probabilities  alpha / sum(alpha)
+ *                               6 binary Dirichlet (u = 2) (alpha_1 / S, 2 / S), S = alpha_0 + alpha_1
+ *                             Kinds 0-3 read target j of task t from column j*T + t (torch.chunk of the MLP output);
+ *                             kinds 4-6 read class c of task t from column t*u + c (reshape(B, T, u)).  softplus is
+ *                             F.softplus with threshold 20.  mean and scale (T entries each, both or neither, kinds 0-3
+ *                             only) apply UnscaleTransform's eval mode: x*scale + mean to the mean / bounds, var*scale^2
+ *                             to MVE's var and evidential's beta, each product and sum rounded as torch rounds it.
+ *   dmpnn_pred_transform_bwd  the mirror for kinds 0-4: dX (B x (T*u)) from dOut (B x T x u) and the forward's X; scale
+ *                             (nullable) as in the forward.  Every column of dX in [0, T*u) is written.
+ *   dmpnn_mve_loss            MVELoss on P (B x T x 2: mean, var): L = (mean - y)^2 / (2 var) + log(2 pi var) / 2
+ *   dmpnn_evidential_loss     EvidentialLoss on P (B x T x 4: mean, v, alpha, beta) with v_kl and eps; d|r|/dr = 0 at r = 0
+ *   dmpnn_quantile_loss       QuantileLoss on P (B x T x 2: mean, interval) at `alpha`: pinball losses of the bounds
+ *                             mean -/+ interval / 2; where the two candidates of a bound's amax tie (target exactly on the
+ *                             bound) the gradient is split evenly between them, as torch's amax does
+ *   dmpnn_dirichlet_loss      DirichletLoss on P (B x T x C: alpha >= 1) with v_kl; its digamma / trigamma are written for
+ *                             arguments >= 1 (recurrence below 6, asymptotic series above)
+ * The four losses reduce like dmpnn_mse_loss: loss[0] = sum_{b,t} w[b] tw[t] m L / sum m with m = isfinite(Y), dP (nullable,
+ * B x T x u, written for every element, masked ones as zeros) = dloss/dP; with every target masked loss[0] = 0 and dP = 0
+ * (the reference's 0 / 0 would be NaN).  One block per call; fixed reduction order; no host synchronisation.
+ * Dirichlet labels follow torch.eye(C)[Y.long()]: trunc(Y) in [0, C) is the class, in [-C, 0) it counts from the end
+ * (class trunc(Y) + C); outside [-C, C) the reference raises, and the kernel makes loss[0] NaN and that row of dP NaN.
+ * ------------------------------------------------------------------------------------- */
+int dmpnn_pred_transform(const float* X, int64_t ldx, int64_t B, int64_t T, int kind, int64_t u, const float* mean,
+                         const float* scale, float* out, int64_t ldo, void* stream);
+int dmpnn_pred_transform_bwd(const float* X, int64_t ldx, const float* dOut, int64_t lddo, int64_t B, int64_t T, int kind,
+                             int64_t u, const float* scale, float* dX, int64_t lddx, void* stream);
+int dmpnn_mve_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                   const float* task_weights, int64_t B, int64_t T, float* loss, float* dP, int64_t lddp, void* stream);
+int dmpnn_evidential_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                          const float* task_weights, int64_t B, int64_t T, float v_kl, float eps, float* loss, float* dP,
+                          int64_t lddp, void* stream);
+int dmpnn_quantile_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                        const float* task_weights, int64_t B, int64_t T, float alpha, float* loss, float* dP, int64_t lddp,
+                        void* stream);
+int dmpnn_dirichlet_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                         const float* task_weights, int64_t B, int64_t T, int64_t C, float v_kl, float* loss, float* dP,
+                         int64_t lddp, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
