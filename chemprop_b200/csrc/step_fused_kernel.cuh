@@ -23,13 +23,9 @@ constexpr int kWHalfSlabs = 3;
 constexpr int kMaxPasses = (kMaxSlabs + kWHalfSlabs - 1) / kWHalfSlabs;   // 2
 constexpr int kWStageBytes = kWHalfSlabs * kChunkN * 128;   // 30 KB
 constexpr int kWStages = 2;
-// Timing experiments compiled in only with -DDMPNN_EXPERIMENTS=1 (DMPNN_EXP selects at run time; results are wrong by
-// construction): 32768 epilogue skips its global stores, 65536 message warps skip their shared-memory gathers, 131072
-// message warps skip the A operand stores, 262144 the MMA warpgroups issue no MMA.
-#ifndef DMPNN_EXPERIMENTS
-#define DMPNN_EXPERIMENTS 0
-#endif
-constexpr bool kExp = DMPNN_EXPERIMENTS != 0;
+// Timing experiments (tc::kExp builds; DMPNN_EXP selects at run time; results are wrong by construction): 32768 epilogue
+// skips its global stores, 65536 message warps skip their shared-memory gathers, 131072 message warps skip the A operand
+// stores, 262144 the MMA warpgroups issue no MMA.
 constexpr int kThreads = 640;
 constexpr int kSWarps = 8;          // message warps (12..19)
 constexpr int kMmaThreads = 256;    // two MMA + epilogue warpgroups (warps 4..7, 8..11)
@@ -90,18 +86,7 @@ static_assert(kMaxSlabs == 5 && kMaxChunks <= 4, "barrier numbering assumes thes
 
 using namespace dmpnn::tc;
 
-// This kernel's bounded wait: the timeout of tc::mbar_wait, without its printf.  A function call anywhere in the kernel makes
-// ptxas serialise every wgmma (C7510), so on a timeout it only traps: a protocol bug still fails loudly (the launch ends in a
-// sticky error that the next synchronising CUDA call reports) instead of hanging the GPU, but it no longer names the block,
-// thread and barrier.  Swapping in tc::mbar_wait, whose printf names them, brings that report back for debugging (at the
-// cost of serialised wgmmas).
-__device__ __forceinline__ void mbar_wait_trap(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) asm volatile("trap;");
-  }
-}
+// Every bounded wait of this kernel is tc::mbar_wait_trap: it makes no call, which would serialise the wgmmas (C7510).
 
 constexpr int kTraceEvents = 16;
 __device__ __forceinline__ void trace_ev(const Params& p, int it, int ev) {

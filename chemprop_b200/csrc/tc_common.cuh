@@ -6,8 +6,16 @@
 #include "common.cuh"
 #include "wgmma_ops.cuh"
 
+// Timing experiments are compiled in only with -DDMPNN_EXPERIMENTS=1; the DMPNN_EXP environment variable then selects them
+// at run time, one bit each (listed where each kernel tests them).  Their results are wrong by construction.
+#ifndef DMPNN_EXPERIMENTS
+#define DMPNN_EXPERIMENTS 0
+#endif
+
 namespace dmpnn {
 namespace tc {
+
+constexpr bool kExp = DMPNN_EXPERIMENTS != 0;
 
 // ---- PTX wrappers ---------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -44,6 +52,18 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
              threadIdx.x, bar, parity);
       __trap();
     }
+  }
+}
+// The bounded wait of the kernels that keep wgmma groups in flight (fused depth step, k_wgrad_tc): the timeout of mbar_wait
+// without its printf.  A function call anywhere in a kernel makes ptxas serialise every wgmma (C7510), so on a timeout it
+// only traps: a protocol bug still fails loudly (the launch ends in a sticky error that the next synchronising CUDA call
+// reports) instead of hanging the GPU, but it no longer names the block, thread and barrier.  Swapping in mbar_wait, whose
+// printf names them, brings that report back for debugging (at the cost of serialised wgmmas).
+__device__ __forceinline__ void mbar_wait_trap(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > 4000000000LL) asm volatile("trap;");
   }
 }
 // one lane of a CONVERGED warp; keeps the warp on the uniform datapath (UTMALDG operands live

@@ -5,16 +5,25 @@
 // columns (SWIZZLE_128B) of the row-major dY / X matrices is exactly the canonical MN-major SW128 atom
 // stack (row r = K index at 128-byte pitch, 64 contiguous columns = MN index); the tensor core transposes them.
 //
-//   CTA (mt, kt, slot): output rows n in [128*mt, 128*mt+128), columns k in [192*kt, 192*kt+192); loops over 64-row
-//   blocks slot, slot+S, ...
-//     warp 0      TMA producer: 2 dY boxes per term + up to 3 X boxes per 64-row stage, 3-stage ring
-//     warps 4-11  two consumer warpgroups (output rows [0, 64) / [64, 128) of the tile): wgmma m64n64k16 with
-//                 transposed operands, D[64 x 192] (registers, fp32) += dY_blk^T . X_blk; after the last block the
-//                 accumulator is written as f32 partial[cta][128][Kpad] to global memory
+//   CTA (mt, kt, slot): output rows n in [128*mt, 128*mt+128), columns k in [192*kt, 192*kt+kw), kw = min(192, Kpad - 192*kt);
+//   loops over 64-row blocks slot, slot+S, ...
+//     warp 0      TMA producer: one dY box per term and working warpgroup + ceil(kw / 64) X boxes per 64-row stage,
+//                 3-stage ring
+//     warps 4-11  two consumer warpgroups (output rows [0, 64) / [64, 128) of the tile): per k16 step of a block ONE wgmma
+//                 m64n{kw}k16 with transposed operands (the B descriptor walks the X boxes through its leading-dimension
+//                 offset), D[64 x kw] (registers, fp32) += dY_blk^T . X_blk.  The groups of block i stay in flight while
+//                 the warpgroup waits for block i+1 and issues it; a stage is released when the groups that read it have
+//                 retired.  After the last block the accumulator is written as f32 partial[cta][128][Kpad] to global memory.
+//                 A warpgroup whose 64 output rows all lie at or beyond N does not run: it gets no dY box, issues no MMA
+//                 and writes no partial (k_wgrad_reduce reads rows below N only), and the barriers count the other one.
 //   a second kernel adds the partials of each mt in fixed order (deterministic) into dW.
 // Up to three dY TERMS may share one launch (dW = sum_t dY_t^T X): the X boxes of a stage are loaded once and every term
 // accumulates into the same registers -- the W_i gradient of the bf16 mirror, whose dH_0 is a sum of per-step terms that
 // is never formed (engine.bond_backward_tc), reads X_0 once instead of once per term.
+//
+// ptxas must not serialise the wgmmas (C7510 / C7519 / C7520 in -Xptxas -v), so the kernel follows the fused depth step's
+// rules (DESIGN.md section 4.1): warp role broadcast from lane 0, no call in the bounded wait, and every term's four k16
+// steps are one straight run behind one fence that is its own wgmma group.
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -34,7 +43,6 @@ constexpr int kXBoxesPerTile = kKT / 64;
 constexpr int kStageBytes = (2 * 3 + kXBoxesPerTile) * kBoxBytes;   // 72 KB (three terms)
 constexpr int kStages = 3;
 constexpr int kThreads = 384;
-constexpr int kConsumers = 256;
 constexpr int kOffBar = kStages * kStageBytes;    // 221184
 constexpr int kSmemBytes = kOffBar + 8 * 8;
 constexpr int kSmemAlloc = kSmemBytes + 1024;
@@ -42,11 +50,63 @@ static_assert(kSmemAlloc <= 232448, "exceeds shared memory");
 
 enum { B_FULL = 0, B_EMPTY = 3 };
 
+// Timing experiments (tc::kExp builds, DMPNN_EXP bits): kExpNoMma -- the consumers wait for a stage and release it, the floor
+// of the memory path; kExpOneBox -- one dY box and one X box per stage, every MMA kept (on stale shared memory), the floor
+// of the MMA issue path.
+constexpr int kExpNoMma = 524288, kExpOneBox = 1048576;
+
 struct Params {
   float* partial;       // [gridDim.x][128][Kpad]
   int64_t R;
   int N, Kx, Kpad, nxb, n_mt, slots, n_blocks, n_terms;
+  int exp_flags;        // timing experiments only; 0 in production
 };
+
+// One consumer warpgroup of a CTA whose accumulator is NW columns wide: the block loop and the drain.
+template <int NW>
+__device__ __forceinline__ void consume(const Params& p, uint32_t sbase, uint32_t sBar, int slot, int kt, int wg, int tt,
+                                        uint32_t x_off) {
+  auto bar = [&](int i) { return sBar + 8u * (uint32_t)i; };
+  const int nt = p.n_terms;
+  float acc[NW / 2];
+#pragma unroll
+  for (int i = 0; i < NW / 2; ++i) acc[i] = 0.f;
+  uint32_t ks = 0, st_prev = 0;
+  for (int blk = slot; blk < p.n_blocks; blk += p.slots, ++ks) {
+    const uint32_t st = ks % kStages, use = ks / kStages;
+    mbar_wait_trap(bar(B_FULL + st), use & 1);
+    const uint32_t base = sbase + st * kStageBytes;
+    if (!(kExp && (p.exp_flags & kExpNoMma))) {
+#pragma unroll
+      for (int t = 0; t < 3; ++t) {
+        if (t >= nt) break;
+        const uint32_t a0 = base + (2 * t + wg) * kBoxBytes, b0 = base + x_off;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kRowsPerStage / 16; ++kk)
+          wgmma_bf16_mn(acc, desc_mn_sw128(a0 + kk * 2048, kBoxBytes), desc_mn_sw128(b0 + kk * 2048, kBoxBytes));
+        wgmma_commit();   // one group per term: a commit after the term loop would sit at a join ptxas guards (C7519)
+      }
+    }
+    if (ks > 0) {   // the previous block's groups have retired once at most this block's nt groups are in flight
+      if (nt >= 3) wgmma_wait<3>();
+      else if (nt == 2) wgmma_wait<2>();
+      else wgmma_wait<1>();
+      mbar_arrive(bar(B_EMPTY + st_prev));
+    }
+    st_prev = st;
+  }
+  wgmma_wait<0>();
+  acc_fence(acc);
+  // drain: rows 64 wg + acc_row0 (+8), columns 8 j + acc_col0 (+1); zeros when this CTA had no block
+  const int rl = wg * 64 + acc_row0(tt), cl = acc_col0(tt);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float* out = p.partial + ((size_t)blockIdx.x * 128 + rl + 8 * h) * p.Kpad + kt * kKT + cl;
+#pragma unroll
+    for (int j = 0; j < NW / 8; ++j) *reinterpret_cast<float2*>(out + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+  }
+}
 
 __global__ void __launch_bounds__(kThreads, 1)
 k_wgrad_tc(const __grid_constant__ CUtensorMap tmapY, const __grid_constant__ CUtensorMap tmapY1,
@@ -55,83 +115,64 @@ k_wgrad_tc(const __grid_constant__ CUtensorMap tmapY, const __grid_constant__ CU
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t sbase = smem_u32(smem);
   const uint32_t sBar = sbase + kOffBar;
-  const int warp = threadIdx.x >> 5;
+  // broadcast from lane 0, so that ptxas sees a warp-uniform role (a role taken from threadIdx.x directly is a divergent
+  // path to the compiler, and it guards the wgmmas inside it)
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   auto bar = [&](int i) { return sBar + 8u * (uint32_t)i; };
   const int mt = blockIdx.x % p.n_mt, slot = blockIdx.x / p.n_mt;
   const int kt = blockIdx.y;
   const int kw = min(kKT, p.Kpad - kt * kKT);        // accumulator columns of this CTA (multiple of 16)
-  const int nxb = (kw + 63) / 64;                    // X boxes per stage
+  const int n_wg = mt * 128 + 64 < p.N ? 2 : 1;      // warpgroups that own an output row below N
+  const bool one_box = kExp && (p.exp_flags & kExpOneBox);
+  const int nxb = one_box ? 1 : (kw + 63) / 64;      // X boxes per stage
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(bar(B_FULL + i), 1);
-      mbar_init(bar(B_EMPTY + i), kConsumers);
+      mbar_init(bar(B_EMPTY + i), 128 * n_wg);
     }
     fence_barrier_init();
   }
   __syncthreads();
   const int nt = p.n_terms;
-  const uint32_t stage_tx = (uint32_t)(2 * nt + nxb) * kBoxBytes;
   const uint32_t x_off = (uint32_t)(2 * nt) * kBoxBytes;      // a stage = [2 boxes per term | X boxes]
 
   if (warp == 0) {
+    const int nyb = one_box ? 1 : nt * n_wg;                    // dY boxes per stage
+    const uint32_t stage_tx = (uint32_t)(nyb + nxb) * kBoxBytes;
     uint32_t ks = 0;
     for (int blk = slot; blk < p.n_blocks; blk += p.slots, ++ks) {
       const uint32_t st = ks % kStages, use = ks / kStages;
-      mbar_wait(bar(B_EMPTY + st), (use & 1) ^ 1);
+      mbar_wait_trap(bar(B_EMPTY + st), (use & 1) ^ 1);
       if (elect_one()) {
         const uint32_t base = sbase + st * kStageBytes;
         mbar_expect_tx(bar(B_FULL + st), stage_tx);
-        for (int t = 0; t < nt; ++t) {
+        for (int t = 0; t < (one_box ? 1 : nt); ++t) {
           const CUtensorMap* my = t == 0 ? &tmapY : (t == 1 ? &tmapY1 : &tmapY2);
-          tma_load_2d(base + (2 * t) * kBoxBytes, my, bar(B_FULL + st), mt * 128, blk * kRowsPerStage);
-          tma_load_2d(base + (2 * t + 1) * kBoxBytes, my, bar(B_FULL + st), mt * 128 + 64, blk * kRowsPerStage);
+          for (int g = 0; g < (one_box ? 1 : n_wg); ++g)
+            tma_load_2d(base + (2 * t + g) * kBoxBytes, my, bar(B_FULL + st), mt * 128 + 64 * g, blk * kRowsPerStage);
         }
         for (int xb = 0; xb < nxb; ++xb)
           tma_load_2d(base + x_off + xb * kBoxBytes, &tmapX, bar(B_FULL + st), kt * kKT + xb * 64, blk * kRowsPerStage);
       }
       __syncwarp();
     }
-  } else if (warp >= 4) {
+  } else if (warp >= 4 && ((warp - 4) >> 2) < n_wg) {
     const int wg = (warp - 4) >> 2;
     const int tt = threadIdx.x - 128 - wg * 128;
-    float acc[kXBoxesPerTile][32];
-#pragma unroll
-    for (int b = 0; b < kXBoxesPerTile; ++b)
-#pragma unroll
-      for (int i = 0; i < 32; ++i) acc[b][i] = 0.f;
-    uint32_t ks = 0;
-    for (int blk = slot; blk < p.n_blocks; blk += p.slots, ++ks) {
-      const uint32_t st = ks % kStages, use = ks / kStages;
-      mbar_wait(bar(B_FULL + st), use & 1);
-      const uint32_t base = sbase + st * kStageBytes;
-      wgmma_fence();
-      for (int t = 0; t < nt; ++t)
-#pragma unroll
-        for (int kk = 0; kk < kRowsPerStage / 16; ++kk) {
-          const uint64_t adesc = desc_mn_sw128(base + (2 * t + wg) * kBoxBytes + kk * 2048, kBoxBytes);
-#pragma unroll
-          for (int b = 0; b < kXBoxesPerTile; ++b)
-            if (b < nxb) wgmma_bf16_n64_mn(acc[b], adesc, desc_mn_sw128(base + x_off + b * kBoxBytes + kk * 2048, kBoxBytes), 1u);
-        }
-      wgmma_commit();
-      wgmma_wait<0>();
-#pragma unroll
-      for (int b = 0; b < kXBoxesPerTile; ++b) acc_fence(acc[b]);
-      mbar_arrive(bar(B_EMPTY + st));
-    }
-    // drain: rows 64 wg + acc_row0 (+8), columns 64 b + 8 j + acc_col0 (+1); zeros when this CTA had no block
-    const int rl = wg * 64 + acc_row0(tt), cl = acc_col0(tt);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float* out = p.partial + ((size_t)blockIdx.x * 128 + rl + 8 * h) * p.Kpad + kt * kKT;
-#pragma unroll
-      for (int b = 0; b < kXBoxesPerTile; ++b)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int c = 64 * b + 8 * j + cl;
-          if (c < kw) *reinterpret_cast<float2*>(out + c) = make_float2(acc[b][4 * j + 2 * h], acc[b][4 * j + 2 * h + 1]);
-        }
+    switch (kw) {   // block-uniform
+      case 16: consume<16>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 32: consume<32>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 48: consume<48>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 64: consume<64>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 80: consume<80>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 96: consume<96>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 112: consume<112>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 128: consume<128>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 144: consume<144>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 160: consume<160>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      case 176: consume<176>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
+      default: consume<192>(p, sbase, sBar, slot, kt, wg, tt, x_off); break;
     }
   }
 }
@@ -258,6 +299,9 @@ extern "C" int dmpnn_wgrad_tc_multi_bf16(const void* const* dYs, int n_terms, in
     p.slots = g.slots;
     p.n_blocks = (int)((R + kRowsPerStage - 1) / kRowsPerStage);
     p.n_terms = n_terms;
+    static int exp_flags = -1;
+    if (exp_flags < 0) { const char* e = kExp ? getenv("DMPNN_EXP") : nullptr; exp_flags = e ? atoi(e) : 0; }
+    p.exp_flags = exp_flags;
     static bool attr_set = false;
     if (!attr_set) {
       cudaError_t e = cudaFuncSetAttribute(k_wgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemAlloc);
