@@ -17,10 +17,6 @@ from . import _lib
 from ._lib import (ACT_ELU, ACT_LEAKYRELU, ACT_NONE, ACT_RELU, ACT_TANH, BF16, F32, SCALE_DIV_CONST,
                    SCALE_INV_COUNT, SCALE_NONE, DmpnnError)
 
-# backward of the bf16 tier: True = the last mirror step sums the dZ^t into dH_0 in its epilogue (one W_i GEMM);
-# False = the terms stay apart and the W_i gradient accumulates one GEMM per term (measured faster at depth 3)
-SUM_IN_EPILOGUE = False
-
 # True: a BatchMolGraph that carries host-computed layout meta words (our collate: dmpnn_batch_meta_host) is trusted
 # and the step never synchronises on the device copy; False: always read the device-computed words (one sync per batch)
 HOST_META = os.environ.get("DMPNN_HOST_META", "1") != "0"      # DMPNN_HOST_META=0: A/B switch for measurements
@@ -909,6 +905,62 @@ def atom_step_bwd_fused(dZ: Tensor, Yact: Tensor | None, dOut: Tensor, h: int, W
     _lib.check(rc, "dmpnn_atom_step_bwd_fused_bf16")
 
 
+def _readout_pad(d_v: int, h: int) -> int:
+    """Column at which M_v starts inside the read-out operand [V || M_v]: d_v rounded up to 8 columns (16-byte aligned bf16 rows
+    for the vectorised segment sum that writes M_v in place; d_v = 106 of the reaction graphs left it on the scalar kernel:
+    1.2 ms per step at C4), unless that would exceed the GEMM's K limit."""
+    dvp = (d_v + 7) // 8 * 8
+    return dvp if dvp + h <= 448 else d_v
+
+
+def _wo_padded(Wo: Tensor, d_v: int, dvp: int) -> Tensor:
+    """W_o with zero columns for the padding between V and M_v"""
+    if dvp == d_v:
+        return Wo
+    return torch.cat([Wo[:, :d_v], Wo.new_zeros((Wo.shape[0], dvp - d_v)), Wo[:, d_v:]], 1)
+
+
+def _wo_unpadded(dWo_p: Tensor, d_v: int, dvp: int) -> Tensor:
+    return dWo_p if dvp == d_v else torch.cat([dWo_p[:, :d_v], dWo_p[:, dvp:]], 1)
+
+
+def _readout_operand(lay: Layout, V: Tensor, Hprev: Tensor, first: bool, h: int, cfg: MPConfig, idx: Tensor | None, dvp: int,
+                     ones: bool):
+    """The bf16 read-out operand [V || 0-pad to dvp || M_v || 0-pad to pad16(h) || 1] (the torch.cat of base.py:180), M_v
+    (base.py:208-211) written in place by the segment sum of Hprev: over the in-edge rows of each atom (`idx` None: bonds) or
+    over the rows idx[e] of its in-edges e (atoms: `src_row`).  `ones`: the last column holds ones when K = dvp + pad16(h) + 1
+    fits the GEMM, and the W_o weight-gradient GEMM then delivers db_o (the column sums of dY) as its last column -- no
+    column-sum pass over V x h.  Returns (XO, ones_col), ones_col None without the ones column; _readout_grads decodes it."""
+    hc = (h + 15) // 16 * 16       # M_v zero-padded to pad16(h): 16-byte stores in the segment sum
+    # columns beyond the K a GEMM asks for are clipped by its TMA descriptor
+    XO = torch.empty((max(lay.V, 1), (dvp + hc + 1 + 15) // 16 * 16), dtype=cfg.hidden_dtype, device=V.device)
+    concat_bf16(V, V.shape[1], XO, lay.V, width=dvp)
+    segment_sum(Hprev, lay.rowptr, lay.V, h, XO[:, dvp:dvp + h], idx=idx, act=(cfg.act if first else ACT_NONE),
+                act_param=cfg.act_param, pad_to=hc)
+    ones_col = dvp + hc if ones and dvp + hc + 1 <= 448 else None
+    if ones_col is not None:
+        XO[:, ones_col].fill_(1.0)
+    return XO, ones_col
+
+
+def _readout_grads(dY: Tensor, saved: dict, nV: int, h: int, d_v: int, bias: bool):
+    """(dW_o, db_o) of the bf16 mirrors from dY and the read-out operand saved["XO"] of _readout_operand: one weight-gradient
+    GEMM whose columns of the padding after V are dropped from dW_o; db_o is its ones column when the forward added one, else
+    a column sum of dY (None without `bias`)."""
+    dvp, oc = saved["dvp"], saved["ones_col"] if bias else None
+    K = dvp + h if oc is None else oc + 1
+    dWo_p = torch.empty((h, K), dtype=torch.float32, device=dY.device)
+    wgrad_tc(dY, saved["XO"], nV, h, K, dWo_p)
+    dWo = _wo_unpadded(dWo_p[:, :dvp + h], d_v, dvp)
+    if oc is not None:
+        return dWo, dWo_p[:, oc]
+    dbo = None
+    if bias:
+        dbo = torch.zeros(h, dtype=torch.float32, device=dY.device)
+        column_sum(dY, nV, h, dbo)
+    return dWo, dbo
+
+
 def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor | None, bo,
                  cfg: MPConfig, for_backward: bool = False, readout_f32: bool = False):
     """BondMessagePassing.forward up to W_o (chemprop/nn/message_passing/base.py:196-212 with
@@ -922,6 +974,7 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
     nE, nV = lay.E, lay.V
     a, ap = cfg.act, cfg.act_param
     tc = _tc_ok(cfg, h, d_v + d_e, d_v + h)
+    X0 = X0f = None
     # H_0 = W_i([V[src] || E])   (mixins.py:8-9); rows in dst-sorted order
     if tc and nE > 0:
         kx = (d_v + d_e + 15) // 16 * 16
@@ -932,14 +985,12 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
     elif _x3_ok(cfg, h, d_v + h) and nE > 0:
         # fp32 tier on the tensor cores: [V[src] || E] materialised once in f32 (zero-padded to a multiple of 4 columns),
         # W_i as a 3xTF32 GEMM; the same operand serves the W_i gradient
-        X0 = None
         kx4 = (d_v + d_e + 3) // 4 * 4
         X0f = torch.empty((nE, kx4), dtype=torch.float32, device=dev)
         concat_f32(V, d_v, X0f, nE, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm)
         H0 = _hidden(nE, hp, T, dev)
         linear_x3(X0f, kx4, pack_weight_x3(Wi), h, H0, bias=bi, R=nE, pad_to=hp)
     else:
-        X0 = None
         H0 = _hidden(nE, hp, T, dev)
         linear_fwd(V, d_v, Wi, H0, h, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm, bias=bi, R=nE, pad_to=hp)
     Hs, Ms, Hbars = [], [], []
@@ -996,22 +1047,10 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             Ms.append(M)
         Hs.append(Hn)
         Hprev, first = Hn, False
-    if Wo is None:
-        XO = Mv = Hv = None
-    elif tc:
-        # [V || M_v] assembled once in bf16 (torch.cat of base.py:180), M_v written in place by the segment sum
-        hc = (h + 15) // 16 * 16       # zero columns up to pad16(h): 16-byte stores in the segment sum
-        ko = (d_v + hc + 1 + 15) // 16 * 16
-        XO = torch.empty((max(nV, 1), ko), dtype=T, device=dev)   # columns beyond the K a GEMM asks for are clipped by its TMA descriptor
-        concat_bf16(V, d_v, XO, nV, width=d_v)
+    XO = Mv = Hv = ones_col = None
+    if Wo is not None and tc:
+        XO, ones_col = _readout_operand(lay, V, Hprev, first, h, cfg, None, d_v, for_backward and bo is not None)
         Mv = XO[:, d_v:d_v + h]
-        segment_sum(Hprev, lay.rowptr, nV, h, Mv, act=(a if first else ACT_NONE), act_param=ap, pad_to=hc)
-        ones_col = None
-        if for_backward and bo is not None and d_v + hc + 1 <= 448:
-            # a column of ones after [V || M_v || 0-pad]: the W_o weight-gradient GEMM over K = d_v + pad16(h) + 1 then delivers
-            # the bias gradient (the column sums of dY) as its last column -- no separate column-sum pass over V x h
-            ones_col = d_v + hc
-            XO[:, ones_col].fill_(1.0)
         if readout_f32:
             Hv = torch.empty((max(nV, 1), h), dtype=torch.float32, device=dev)[:nV]
             linear_tc_rows(XO, d_v + h, pack_weight_tc(Wo), h, Hv, R=nV, bias=bo, act=a, act_param=ap)
@@ -1021,10 +1060,9 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             if cfg.dropout_p > 0:
                 _dropout_(Hvp, cfg)                                                    # base.py:182
             Hv = Hvp[:nV, :h]
-    else:
+    elif Wo is not None:
         if cfg.dropout_p > 0:
             raise DmpnnError("dropout on the monolithic tier needs the tensor-core path (see dropout_fused_ok)")
-        XO = None
         if x3 and nV > 0:
             # [V || M_v] assembled once in f32 (torch.cat of base.py:180): V copied in, M_v written in place by the segment sum
             XO = torch.empty((nV, d_v + h), dtype=T, device=dev)
@@ -1040,8 +1078,8 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             # H_v = tau(W_o([V || M_v]))   (base.py:180-182)
             Hv = torch.empty((nV, h), dtype=T, device=dev)
             linear_fwd(V, d_v, Wo, Hv, h, X2=Mv, K2=h, bias=bo, act=a, act_param=ap, R=nV, pad_to=h)
-    saved = dict(H0=H0, Hs=Hs, Ms=Ms, Hbars=Hbars, Mv=Mv, Hv=Hv, X0=X0, XO=XO, tc=tc, x3=x3, X0f=locals().get("X0f"),
-                 ones_col=locals().get("ones_col"))
+    saved = dict(H0=H0, Hs=Hs, Ms=Ms, Hbars=Hbars, Mv=Mv, Hv=Hv, X0=X0, XO=XO, tc=tc, x3=x3, X0f=X0f, dvp=d_v,
+                 ones_col=ones_col)
     return Hv, saved
 
 
@@ -1099,22 +1137,19 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
         else:
             WhT = None if (tc or x3) else Wh.t().contiguous()
             WhT_pk = pack_weight_tc(Wh, transpose=True) if tc else None
-            WhT_f = None                                   # W_h^T packed for the fused mirror (undirected fused steps)
             WhT_x3 = pack_weight_x3(Wh, transpose=True) if x3 else None
             dZ = _hidden(nE, hp, T, dev)
             act_bwd(dMv, Hs[-1], nE, h, act=a, act_param=ap, gidx=lay.dst_row, dZ=dZ, acc=dH0)
+            # undirected steps that ran on the fused kernel (they saved no M^t): their mirror on the fused kernel too
+            fused_undirected = cfg.undirected and tc and Ms[0] is None
+            WhT_f = pack_weight_bf16(Wh.t().contiguous()) if fused_undirected else None
             for t in range(cfg.depth - 1, 0, -1):
                 # inputs of step t: Hin = H^{t-1} (or tau(H_0) when t == 1)
                 first = t == 1
                 Hin = H0 if first else Hs[t - 2]
-                M = Ms[t - 1]
-                if M is None and cfg.undirected and tc and _fused_step_ok(cfg, lay, h):
-                    # undirected step that ran on the fused kernel: its mirror on the fused kernel too.
+                if fused_undirected:
                     # dH~^{t-1} = (S.P)(dZ . W_h) = ((S.P) dZ) . W_h, unmasked; the gathered operand G = (S.P) dZ is the left
-                    # factor of the W_h gradient (dZ^T . M^t = G^T . H~^{t-1}, H~^{t-1} saved by the forward's prologue);
-                    # then the adjoint of the average (self-adjoint) and tau' as in the generic mirror
-                    if WhT_f is None:
-                        WhT_f = pack_weight_bf16(Wh.t().contiguous())
+                    # factor of the W_h gradient (dZ^T . M^t = G^T . H~^{t-1}, H~^{t-1} saved by the forward's prologue)
                     if dbh is not None:
                         column_sum(dZ, nE, h, dbh, accumulate=True)
                     G = _empty_hidden(nE, hp, T, dev)
@@ -1123,43 +1158,39 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
                     wgrad_tc(G, Hbars[t - 1], nE, h, h, dWh, accumulate=True)
                     dHin = _hidden(nE, hp, T, dev)
                     rev_average(dHbar, lay, h, dHin)
-                    if first:
-                        act_bwd(dHin, H0, nE, h, act=a, act_param=ap, from_preact=True, acc=dH0)
+                else:
+                    M = Ms[t - 1]
+                    if M is None:  # fused forward did not materialise M^t: recompute it
+                        M = _hidden(nE, hp, T, dev)
+                        if cfg.undirected:
+                            bond_message(Hbars[t - 1], lay, h, M)
+                        else:
+                            bond_message(Hin, lay, h, M, act=(a if first else ACT_NONE), act_param=ap)
+                    if tc:
+                        wgrad_tc(dZ, M, nE, h, h, dWh, accumulate=True)
+                        if dbh is not None:
+                            column_sum(dZ, nE, h, dbh, accumulate=True)
+                    elif x3:
+                        wgrad_x3(dZ, M, nE, h, h, dWh, accumulate=True)
+                        if dbh is not None:
+                            column_sum(dZ, nE, h, dbh, accumulate=True)
                     else:
-                        dZ = _hidden(nE, hp, T, dev)
-                        act_bwd(dHin, Hin, nE, h, act=a, act_param=ap, dZ=dZ, acc=dH0)
-                    continue
-                if M is None:  # fused forward did not materialise M^t: recompute it
-                    M = _hidden(nE, hp, T, dev)
+                        linear_wgrad(dZ, M, h, dWh, h, dbias=dbh, accumulate=True, R=nE)
+                    if tc:
+                        dM = _empty_hidden(nE, hp, T, dev)
+                        linear_tc(dZ, h, WhT_pk, h, dM, R=nE)
+                    elif x3:
+                        dM = _hidden(nE, hp, T, dev)
+                        linear_x3(dZ, h, WhT_x3, h, dM, R=nE, pad_to=hp)
+                    else:
+                        dM = _hidden(nE, hp, T, dev)
+                        linear_fwd(dZ, h, WhT, dM, h, R=nE, pad_to=hp)
+                    dHin = _hidden(nE, hp, T, dev)
+                    bond_message(dM, lay, h, dHin, permute_on_read=True)
                     if cfg.undirected:
-                        bond_message(Hbars[t - 1], lay, h, M)
-                    else:
-                        bond_message(Hin, lay, h, M, act=(a if first else ACT_NONE), act_param=ap)
-                if tc:
-                    wgrad_tc(dZ, M, nE, h, h, dWh, accumulate=True)
-                    if dbh is not None:
-                        column_sum(dZ, nE, h, dbh, accumulate=True)
-                elif x3:
-                    wgrad_x3(dZ, M, nE, h, h, dWh, accumulate=True)
-                    if dbh is not None:
-                        column_sum(dZ, nE, h, dbh, accumulate=True)
-                else:
-                    linear_wgrad(dZ, M, h, dWh, h, dbias=dbh, accumulate=True, R=nE)
-                if tc:
-                    dM = _empty_hidden(nE, hp, T, dev)
-                    linear_tc(dZ, h, WhT_pk, h, dM, R=nE)
-                elif x3:
-                    dM = _hidden(nE, hp, T, dev)
-                    linear_x3(dZ, h, WhT_x3, h, dM, R=nE, pad_to=hp)
-                else:
-                    dM = _hidden(nE, hp, T, dev)
-                    linear_fwd(dZ, h, WhT, dM, h, R=nE, pad_to=hp)
-                dHin = _hidden(nE, hp, T, dev)
-                bond_message(dM, lay, h, dHin, permute_on_read=True)
-                if cfg.undirected:
-                    tmp = _hidden(nE, hp, T, dev)
-                    rev_average(dHin, lay, h, tmp)
-                    dHin = tmp
+                        tmp = _hidden(nE, hp, T, dev)
+                        rev_average(dHin, lay, h, tmp)
+                        dHin = tmp
                 if first:
                     act_bwd(dHin, H0, nE, h, act=a, act_param=ap, from_preact=True, acc=dH0)
                 else:
@@ -1185,9 +1216,9 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
 
 def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
                      saved: dict, gHv: Tensor | None, need_bias: tuple[bool, bool, bool], entry=None):
-    """bf16-tier autograd mirror on the tensor-core kernels (directed bonds).  Differences from the generic
-    mirror: every GEMM is on the tensor cores (wgmma); tau' is fused into the backward message kernel; dH_0 is never kept as an f32
-    read-modify-write accumulator -- the per-step dZ^t stay in bf16 and are summed once, in f32, at the end.
+    """bf16-tier autograd mirror of bond_forward on the fused depth step (directed bonds).  Differences from the generic
+    mirror: every GEMM is on the tensor cores (wgmma); each depth step's mirror is one launch of the fused kernel (_fused_mirror);
+    dH_0 is never formed -- its terms stay in bf16 and are contracted with X_0 by one multi-term weight-gradient launch.
     `gHv` None: no read-out (dW_o, db_o None).  `entry(dMv, Y, from_preact, out)` (the mol-atom-bond edge head) replaces the
     pass that starts the loop, out = dM_v[dst(r)] * tau'(Y[r]): it writes out = (its own term + dM_v[dst(r)]) * tau'(Y[r]),
     dMv None when there is no read-out."""
@@ -1207,15 +1238,9 @@ def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
     no_e = nE == 0
     dWi = torch.zeros_like(Wi, dtype=torch.float32) if no_e else torch.empty_like(Wi, dtype=torch.float32)
     dWh = torch.zeros_like(Wh, dtype=torch.float32) if (no_e or cfg.depth == 1) else torch.empty_like(Wh, dtype=torch.float32)
-    dWo = torch.empty_like(Wo, dtype=torch.float32) if gHv is not None else None
-    wh_acc = [False]                                  # has dW_h been written yet?
-
-    def wgrad_h(dYt, Xt):
-        wgrad_tc(dYt, Xt, nE, h, h, dWh, accumulate=wh_acc[0])
-        wh_acc[0] = True
+    dWo = dbo = None
     dbi = torch.zeros(h, **f32) if need_bias[0] else None
     dbh = torch.zeros(h, **f32) if need_bias[1] else None
-    dbo = torch.zeros(h, **f32) if (need_bias[2] and gHv is not None) else None
     # Training-mode dropout (cfg.dropout_p > 0; ReLU only, dropout_fused_ok): a gradient that crosses a dropout site is
     # multiplied by the keep mask and by s = 1 / (1 - p).  With ReLU the mask is already in tau' of the stored POST-dropout
     # state ([H_post > 0] = mask * [H_pre > 0]), and s, a scalar, folds into the packed weight of the GEMM that produces
@@ -1228,15 +1253,7 @@ def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
             gHv = gHv.contiguous()
         dY = _empty_hidden(nV, hp, T, dev)
         act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)      # dY / s_v
-        oc = saved.get("ones_col")
-        if dbo is not None and oc is not None:
-            dWo_ext = torch.empty((h, oc + 1), **f32)            # [dW_o | 0 | db_o]: the ones column of XO (bond_forward)
-            wgrad_tc(dY, saved["XO"], nV, h, oc + 1, dWo_ext)
-            dWo, dbo = dWo_ext[:, : d_v + h], dWo_ext[:, oc]
-        else:
-            wgrad_tc(dY, saved["XO"], nV, h, d_v + h, dWo)
-            if dbo is not None:
-                column_sum(dY, nV, h, dbo)
+        dWo, dbo = _readout_grads(dY, saved, nV, h, d_v, need_bias[2])
         if s_v != 1.0:
             dWo.mul_(s_v)
             if dbo is not None:
@@ -1248,87 +1265,64 @@ def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
         dMv = _empty_hidden(nV, hp, T, dev)
         Wo_m = Wo[:, d_v:] if s_v * s_e == 1.0 else Wo[:, d_v:] * (s_v * s_e)
         linear_tc(dY, h, pack_weight_tc(Wo_m, transpose=True), h, dMv, R=nV)
-    dH0b = _empty_hidden(nE, hp, T, dev)
     if cfg.depth == 1:
+        dH0b = _empty_hidden(nE, hp, T, dev)
         if entry is not None:
             entry(dMv, H0, True, dH0b)
         else:
             act_bwd(dMv, H0, nE, hc, act=a, act_param=ap, gidx=lay.dst_row, from_preact=True, dZ=dH0b)
+        terms = [dH0b]
     else:
-        fused_bwd = _fused_step_ok(cfg, lay, h)      # the depth step's mirror on the same fused wgmma kernel
-        if s_drop != 1.0 and not fused_bwd:
-            raise DmpnnError("dropout on the monolithic tier needs the fused depth step (see dropout_fused_ok)")
-        WhT_pk = None if fused_bwd else pack_weight_tc(Wh, transpose=True)
-        WhT_pkf = pack_weight_bf16(Wh.t().contiguous()) if fused_bwd else None
+        WhT = pack_weight_bf16(Wh.t().contiguous())
         # mirror steps whose result arrives at a dropout site (every one but the last, which lands on H^0) carry s
-        WhT_pkf_s = WhT_pkf if s_drop == 1.0 else pack_weight_bf16((Wh * s_drop).t().contiguous())
+        WhT_s = WhT if s_drop == 1.0 else pack_weight_bf16((Wh * s_drop).t().contiguous())
         dZ = _empty_hidden(nE, hp, T, dev)
         if entry is not None:
             entry(dMv, Hs[-1], False, dZ)
         else:
             act_bwd(dMv, Hs[-1], nE, hc, act=a, act_param=ap, gidx=lay.dst_row, dZ=dZ)    # dZ^{T-1}
-        dZs, dH_first, fused_sum, dH0_terms = [dZ], None, False, None
-        for t in range(cfg.depth - 1, 0, -1):
-            first = t == 1
-            Hin = H0 if first else Hs[t - 2]
-            if dbh is not None:
-                column_sum(dZ, nE, h, dbh, accumulate=True)
-            if fused_bwd:
-                # dH^{t-1} = (S.P)(dZ . W_h) = ((S.P) dZ) . W_h: gather on the A operand, tau' in the epilogue.
-                # W_h gradient without recomputing M^t:  dZ^T . M^t = dZ^T . (P.S) H^{t-1} = ((S.P) dZ)^T . H^{t-1};
-                # the kernel writes its gathered operand G = (S.P) dZ out.  t = 1 has no stored tau(H_0): it uses
-                # the M^1 the forward kernel saved.
-                M1 = saved["Ms"][0] if first else None
-                if first and M1 is None:
-                    M1 = _empty_hidden(nE, hp, T, dev)
-                    bond_message(H0, lay, h, M1, act=a, act_param=ap)
-                if first:
-                    wgrad_h(dZ, M1)
-                    if SUM_IN_EPILOGUE and len(dZs) <= 2:
-                        # last mirror step writes dH_0 itself: tau'(H_0) mask and the sum over the dZ^t in its epilogue
-                        bond_step_bwd_fused(dZ, H0, dH0b, h, WhT_pkf, lay, a, ap, y_is_preact=True, addends=tuple(dZs))
-                        fused_sum = True
-                    elif not SUM_IN_EPILOGUE:
-                        # dH_0 = sum_t dZ^t + dH^0 * tau'(H_0) is only ever contracted with X_0 (and summed for the
-                        # bias): keep the terms apart -- the last mirror step applies tau'(H_0) in its epilogue and
-                        # the W_i gradient accumulates one GEMM per term instead of a 5-stream summing pass
-                        bond_step_bwd_fused(dZ, H0, dH0b, h, WhT_pkf, lay, a, ap, y_is_preact=True)
-                        dH0_terms = dZs + [dH0b]
-                    else:
-                        dH_first = _empty_hidden(nE, hp, T, dev)
-                        bond_step_bwd_fused(dZ, None, dH_first, h, WhT_pkf, lay, a, ap)
-                else:
-                    dZn = _empty_hidden(nE, hp, T, dev)
-                    G = _empty_hidden(nE, hp, T, dev)
-                    bond_step_bwd_fused(dZ, Hin, dZn, h, WhT_pkf_s, lay, a, ap, G_out=G)
-                    wgrad_h(G, Hin)
-                    dZ = dZn
-                    dZs.append(dZ)
-                continue
-            M = _empty_hidden(nE, hp, T, dev)                # M^t, recomputed
-            bond_message(Hin, lay, h, M, act=(a if first else ACT_NONE), act_param=ap)
-            wgrad_h(dZ, M)
-            dM = _empty_hidden(nE, hp, T, dev)
-            linear_tc(dZ, h, WhT_pk, h, dM, R=nE)
-            if first:
-                dH_first = _empty_hidden(nE, hp, T, dev)     # dH^0 (tau' from the pre-activation H_0 is applied below)
-                bond_message(dM, lay, h, dH_first, permute_on_read=True)
-            else:
-                dZ = _empty_hidden(nE, hp, T, dev)           # dZ^{t-1} = S.P(dM) * tau'(H^{t-1})
-                bond_message_bwd_masked(dM, Hin, lay, h, dZ, act=a, act_param=ap)
-                dZs.append(dZ)
-        if dH0_terms is not None:
-            wgrad_tc_multi(dH0_terms, saved["X0"], nE, h, d_v + d_e, dWi)     # X_0 read once for all terms
-            if dbi is not None:
-                for i, P in enumerate(dH0_terms):
-                    column_sum(P, nE, h, dbi, accumulate=i > 0)
-            return dWi, dbi, dWh, dbh, dWo, dbo
-        if not fused_sum:
-            sum_act_bwd(dZs, dH_first, H0, dH0b, nE, hc, act=a, act_param=ap)
-    wgrad_tc(dH0b, saved["X0"], nE, h, d_v + d_e, dWi)
+        M1 = saved["Ms"][0]
+        assert M1 is not None, "M^1 is saved by the fused forward step whenever a weight needs a gradient"
+        terms = _fused_mirror(bond_step_bwd_fused, dZ, H0, Hs, M1, WhT, WhT_s, dWh, dbh, nE, h, lay, cfg)
+    # dH_0 = sum_t dZ^t + dH^0 * tau'(H_0) is only ever contracted with X_0 (and summed for the bias): the terms stay apart and
+    # the W_i gradient takes them all in one weight-gradient launch (X_0 read once), instead of a summing pass over E x h
+    wgrad_tc_multi(terms, saved["X0"], nE, h, d_v + d_e, dWi)
     if dbi is not None:
-        column_sum(dH0b, nE, h, dbi)
+        for i, P in enumerate(terms):
+            column_sum(P, nE, h, dbi, accumulate=i > 0)
     return dWi, dbi, dWh, dbh, dWo, dbo
+
+
+def _fused_mirror(step, dZ: Tensor, H0: Tensor, Hs: list, first_op: Tensor, WT1: Tensor, WT: Tensor, dWh: Tensor,
+                  dbh: Tensor | None, R: int, h: int, lay: Layout, cfg: MPConfig) -> list:
+    """The depth loop of the fused bf16 mirrors (DESIGN.md section 5), bonds and atoms alike.  `step` is the mirror mode of the
+    fused depth step (bond_step_bwd_fused / atom_step_bwd_fused): dH^{t-1} = (B dZ^t) . W_h [* tau'], B the sibling gather
+    S.P of bonds or the adjacency A of atoms, with its gathered operand G^t = B dZ^t written out.  G^t is the left factor of the
+    step's W_h gradient (dZ^T . M^t = G^T . H^{t-1}); t = 1 has no stored tau(H_0) and contracts dZ^1 with `first_op`, the M^1 /
+    N^1 the forward saved.  `WT1` is the packed W_h^T of the t = 1 step, `WT` that of the others (for bonds it carries the
+    dropout scale).  dW_h is written by its first GEMM, db_h accumulated.  From dZ = dZ^{T-1}, returns the dH_0 terms
+    [dZ^{T-1}, ..., dZ^1, dH^0 * tau'(H_0)]."""
+    a, ap = cfg.act, cfg.act_param
+    hp, T, dev = pad_hidden(h), cfg.hidden_dtype, dZ.device
+    terms = [dZ]
+    for t in range(cfg.depth - 1, 0, -1):
+        accumulate = t < cfg.depth - 1
+        if dbh is not None:
+            column_sum(dZ, R, h, dbh, accumulate=True)
+        if t == 1:
+            wgrad_tc(dZ, first_op, R, h, h, dWh, accumulate=accumulate)
+            dH0 = _empty_hidden(R, hp, T, dev)
+            step(dZ, H0, dH0, h, WT1, lay, a, ap, y_is_preact=True)                          # dH^0 * tau'(H_0)
+            terms.append(dH0)
+        else:
+            Hin = Hs[t - 2]
+            dZn = _empty_hidden(R, hp, T, dev)
+            G = _empty_hidden(R, hp, T, dev)
+            step(dZ, Hin, dZn, h, WT, lay, a, ap, G_out=G)                                   # dZ^{t-1}
+            wgrad_tc(G, Hin, R, h, h, dWh, accumulate=accumulate)
+            dZ = dZn
+            terms.append(dZ)
+    return terms
 
 
 def _refuse_feature_grads(ctx):
@@ -1460,25 +1454,6 @@ def atom_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
     return dWi, dbi, dWh, dbh, dWo, dbo
 
 
-def _readout_pad(d_v: int, h: int) -> int:
-    """Column at which M_v starts inside the read-out operand [V || M_v]: d_v rounded up to 8 columns (16-byte aligned bf16 rows
-    for the vectorised segment sum that writes M_v in place; d_v = 106 of the reaction graphs left it on the scalar kernel:
-    1.2 ms per step at C4), unless that would exceed the GEMM's K limit."""
-    dvp = (d_v + 7) // 8 * 8
-    return dvp if dvp + h <= 448 else d_v
-
-
-def _wo_padded(Wo: Tensor, d_v: int, dvp: int) -> Tensor:
-    """W_o with zero columns for the padding between V and M_v"""
-    if dvp == d_v:
-        return Wo
-    return torch.cat([Wo[:, :d_v], Wo.new_zeros((Wo.shape[0], dvp - d_v)), Wo[:, d_v:]], 1)
-
-
-def _wo_unpadded(dWo_p: Tensor, d_v: int, dvp: int) -> Tensor:
-    return dWo_p if dvp == d_v else torch.cat([dWo_p[:, :d_v], dWo_p[:, dvp:]], 1)
-
-
 def _atom_tc_ok(cfg: MPConfig, h: int, d_v: int, d_e: int) -> bool:
     return _tc_ok(cfg, h, d_v, h + d_e, d_v + h) and h % 4 == 0
 
@@ -1486,20 +1461,12 @@ def _atom_tc_ok(cfg: MPConfig, h: int, d_v: int, d_e: int) -> bool:
 def _atom_readout_tc(lay: Layout, V: Tensor, Hprev: Tensor, first: bool, h: int, Wo: Tensor, bo, cfg: MPConfig, rows: int,
                      with_ones: bool, readout_f32: bool):
     """H_v = tau(W_o([V || M_v])) of the atom tiers (base.py:180-182, 208-211): returns (H_v, XO, dvp, ones_col).  `with_ones`:
-    a ones column after [V || M_v || 0-pad] delivers db_o with dW_o's GEMM (see bond_forward)."""
+    a ones column delivers db_o with dW_o's GEMM (_readout_operand)."""
     dev, T, nV = V.device, cfg.hidden_dtype, lay.V
     a, ap = cfg.act, cfg.act_param
     d_v = V.shape[1]
-    hc = (h + 15) // 16 * 16
     dvp = _readout_pad(d_v, h)
-    ones_col = dvp + hc if (with_ones and bo is not None and dvp + hc + 1 <= 448) else None
-    ko = (dvp + hc + 1 + 15) // 16 * 16 if ones_col is not None else (dvp + h + 15) // 16 * 16
-    XO = torch.empty((rows, ko), dtype=T, device=dev)
-    concat_bf16(V, d_v, XO, nV, width=dvp)
-    segment_sum(Hprev, lay.rowptr, nV, h, XO[:, dvp:dvp + h], idx=lay.src_row, act=(a if first else ACT_NONE),
-                act_param=ap, pad_to=(hc if dvp + hc <= ko else h))                           # base.py:208-211
-    if ones_col is not None:
-        XO[:, ones_col].fill_(1.0)
+    XO, ones_col = _readout_operand(lay, V, Hprev, first, h, cfg, lay.src_row, dvp, with_ones and bo is not None)
     Wpk = pack_weight_tc(_wo_padded(Wo, d_v, dvp))
     if readout_f32:
         Hv = torch.empty((rows, h), dtype=torch.float32, device=dev)[:nV]
@@ -1553,7 +1520,7 @@ def atom_forward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tenso
     Hv = XO = dvp = None
     if Wo is not None:
         Hv, XO, dvp, _ = _atom_readout_tc(lay, V, Hprev, first, h, Wo, bo, cfg, rows, False, readout_f32)
-    return Hv, dict(H0=H0, Hs=Hs, XAs=XAs, XO=XO, Xv=Xv, Hv=Hv, tc=True, dvp=dvp)
+    return Hv, dict(H0=H0, Hs=Hs, XAs=XAs, XO=XO, Xv=Xv, Hv=Hv, tc=True, dvp=dvp, ones_col=None)
 
 
 def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
@@ -1569,7 +1536,7 @@ def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
     T = cfg.hidden_dtype
     nV = lay.V
     a, ap = cfg.act, cfg.act_param
-    H0, Hs, XAs, XO, Xv, Hv = saved["H0"], saved["Hs"], saved["XAs"], saved["XO"], saved["Xv"], saved["Hv"]
+    H0, Hs, XAs, Xv, Hv = saved["H0"], saved["Hs"], saved["XAs"], saved["Xv"], saved["Hv"]
     f32 = dict(dtype=torch.float32, device=dev)
     dWi = torch.zeros_like(Wi, dtype=torch.float32)
     dWh = torch.zeros_like(Wh, dtype=torch.float32)
@@ -1585,15 +1552,7 @@ def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
             gHv = gHv.contiguous()
         dY = _empty_hidden(nV, hp, T, dev)
         act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)
-        dvp = saved.get("dvp", d_v)
-        if dvp == d_v:
-            wgrad_tc(dY, XO, nV, h, d_v + h, dWo)
-        else:
-            dWo_p = torch.empty((h, dvp + h), dtype=torch.float32, device=dev)
-            wgrad_tc(dY, XO, nV, h, dvp + h, dWo_p)
-            dWo = _wo_unpadded(dWo_p, d_v, dvp)
-        if dbo is not None:
-            column_sum(dY, nV, h, dbo)
+        dWo, dbo = _readout_grads(dY, saved, nV, h, d_v, dbo is not None)
         dMv = _empty_hidden(nV, hp, T, dev)
         linear_tc(dY, h, pack_weight_tc(Wo[:, d_v:], transpose=True), h, dMv, R=nV)
         # d(Ha^{T-1})[u] = sum_{e' in in(u)} dM_v[src(e')]   (rev is an involution)
@@ -1692,14 +1651,13 @@ def atom_backward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tenso
     T = cfg.hidden_dtype
     nV = lay.V
     a, ap = cfg.act, cfg.act_param
-    H0, Hs, N1, SEb, XO, Xv, Hv = (saved[k] for k in ("H0", "Hs", "N1", "SEb", "XO", "Xv", "Hv"))
+    H0, Hs, N1, Xv, Hv = (saved[k] for k in ("H0", "Hs", "N1", "Xv", "Hv"))
     f32 = dict(dtype=torch.float32, device=dev)
     dWi = torch.empty_like(Wi, dtype=torch.float32)
     dWh = torch.empty_like(Wh, dtype=torch.float32)
-    dWo = torch.empty_like(Wo, dtype=torch.float32) if gHv is not None else None
+    dWo = dbo = None
     dbi = torch.zeros(h, **f32) if need_bias[0] else None
     dbh = torch.zeros(h, **f32) if need_bias[1] else None
-    dbo = torch.zeros(h, **f32) if (need_bias[2] and gHv is not None) else None
     if gHv is not None:
         if gHv.stride(1) != 1:
             gHv = gHv.contiguous()
@@ -1709,21 +1667,7 @@ def atom_backward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tenso
             # act_bwd writes h columns; the fused mirror below reads dY up to pad16(h), where a NaN left by the allocator
             # would reach every output column through the zero rows of the packed weight (0 * NaN = NaN)
             dY[:, h:hc].zero_()
-        dvp = saved.get("dvp", d_v)
-        oc = saved.get("ones_col")
-        if dbo is not None and oc is not None:
-            dWo_p = torch.empty((h, oc + 1), dtype=torch.float32, device=dev)      # [dW_o (padded) | 0 | db_o]
-            wgrad_tc(dY, XO, nV, h, oc + 1, dWo_p)
-            dWo, dbo = _wo_unpadded(dWo_p[:, :dvp + h], d_v, dvp), dWo_p[:, oc]
-        else:
-            if dvp == d_v:
-                wgrad_tc(dY, XO, nV, h, d_v + h, dWo)
-            else:
-                dWo_p = torch.empty((h, dvp + h), dtype=torch.float32, device=dev)
-                wgrad_tc(dY, XO, nV, h, dvp + h, dWo_p)
-                dWo = _wo_unpadded(dWo_p, d_v, dvp)
-            if dbo is not None:
-                column_sum(dY, nV, h, dbo)
+        dWo, dbo = _readout_grads(dY, saved, nV, h, d_v, need_bias[2])
     # dZ^{T-1} = (A (dY . W_o[:, d_v:])) * tau'(H^{T-1}) = ((A dY) . W_o[:, d_v:]) * tau'(H^{T-1}): the read-out GEMM, the
     # neighbour gather of its result and the tau' pass are ONE mirror launch of the fused kernel on dY (three launches before)
     if entry is None:
@@ -1742,36 +1686,19 @@ def atom_backward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tenso
             segment_sum(dMv, lay.rowptr, nV, h, dHa, idx=lay.src_row, pad_to=hc)
         entry(dHa, Hs[-1], False, dZ)
     WhT = pack_weight_bf16(Wh[:, :h].t().contiguous())
-    dWhN = dWh[:, :h]
-    terms, wrote = [dZ], False
-    dH0l = _empty_hidden(nV, hp, T, dev)
-    for t in range(cfg.depth - 1, 0, -1):
-        if dbh is not None:
-            column_sum(dZ, nV, h, dbh, accumulate=True)
-        if t == 1:
-            wgrad_tc(dZ, N1, nV, h, h, dWhN, accumulate=wrote)
-            atom_step_bwd_fused(dZ, H0, dH0l, h, WhT, lay, a, ap, y_is_preact=True)           # dH^0 * tau'(H_0)
-        else:
-            Hin = Hs[t - 2]
-            dZn = _empty_hidden(nV, hp, T, dev)
-            G = _empty_hidden(nV, hp, T, dev)
-            atom_step_bwd_fused(dZ, Hin, dZn, h, WhT, lay, a, ap, G_out=G)
-            wgrad_tc(G, Hin, nV, h, h, dWhN, accumulate=wrote)
-            dZ = dZn
-            terms.append(dZ)
-        wrote = True
+    terms = _fused_mirror(atom_step_bwd_fused, dZ, H0, Hs, N1, WhT, WhT, dWh[:, :h], dbh, nV, h, lay, cfg)
     if d_e > 0:
         # one pass over the dZ^t terms for both [V || sum_in E] blocks of Xv, then the dH^0 term for the V block alone
         kv = (d_v + 15) // 16 * 16
         dWx = torch.empty((h, kv + d_e), **f32)
-        wgrad_tc_multi(terms, Xv, nV, h, kv + d_e, dWx)
-        wgrad_tc(dH0l, Xv, nV, h, d_v, dWx[:, :d_v], accumulate=True)
+        wgrad_tc_multi(terms[:-1], Xv, nV, h, kv + d_e, dWx)
+        wgrad_tc(terms[-1], Xv, nV, h, d_v, dWx[:, :d_v], accumulate=True)
         dWi = dWx[:, :d_v]
         dWh[:, h:].copy_(dWx[:, kv:kv + d_e])
     else:
-        wgrad_tc_multi(terms + [dH0l], Xv, nV, h, d_v, dWi)
+        wgrad_tc_multi(terms, Xv, nV, h, d_v, dWi)
     if dbi is not None:
-        for i, P in enumerate(terms + [dH0l]):
+        for i, P in enumerate(terms):
             column_sum(P, nV, h, dbi, accumulate=i > 0)
     return dWi, dbi, dWh, dbh, dWo, dbo
 

@@ -3,6 +3,9 @@
 golden vectors of the real reference.  What this pins without a GPU: which op is called on which operand with
 which index table, in which order, and that every gradient (incl. a learnable activation's) is wired through.  The
 kernels themselves are checked on the H100 by the `-m gpu` tests."""
+import os
+import warnings
+
 import numpy as np
 import pytest
 import torch
@@ -627,3 +630,134 @@ def test_composed_tier_checks_its_x3_gemm_on_first_use(broken, monkeypatch):
     for k, p in mp.named_parameters():
         ref = P[k].grad
         assert float((p.grad.double() - ref).abs().max()) <= 1e-5 * max(1e-6, float(ref.abs().max())), k
+
+
+# ---- launch sequence of the bf16 tier ------------------------------------------------------------------------------------
+# Every kernel wrapper of engine.py that the bf16 tier calls.  A call is recorded with its wrapper's name and its scalar
+# arguments (sizes, flags, activation); a tensor argument as its presence, a list of tensors as its length, a packed weight
+# as the shape of the matrix packed.  wgrad_tc is a one-term wgrad_tc_multi (the same C launch).
+_LAUNCH_WRAPPERS = ("linear_fwd", "linear_wgrad", "segment_sum", "segment_bcast", "bond_message", "rev_average", "act_bwd",
+                    "pack_weight_tc", "pack_weight_bf16", "concat_bf16", "linear_tc", "linear_tc_rows", "wgrad_tc",
+                    "wgrad_tc_multi", "column_sum", "dropout_keep_bits", "scale_mask_", "bond_step_fused", "bond_step_bwd_fused",
+                    "atom_step_fused", "atom_step_bwd_fused", "bond_message_bwd_masked", "sum_act_bwd", "concat_f32",
+                    "linear_x3", "wgrad_x3", "pack_weight_x3")
+
+LAUNCH_CASES = {
+    # kind, depth, bias, extra
+    "bond-d1": ("bond", 1, False, {}),
+    "bond-d1-bias": ("bond", 1, True, {}),
+    "bond-d2": ("bond", 2, False, {}),
+    "bond-d2-bias": ("bond", 2, True, {}),
+    "bond-d3": ("bond", 3, False, {}),
+    "bond-d3-bias": ("bond", 3, True, {}),
+    "bond-d1-dropout": ("bond", 1, True, dict(dropout=0.3)),
+    "bond-d3-dropout": ("bond", 3, True, dict(dropout=0.3)),
+    "bond-d3-undirected": ("bond", 3, True, dict(undirected=True)),
+    "bond-d2-unfused": ("bond", 2, True, dict(fused=False)),
+    "atom-d2-bias": ("atom", 2, True, {}),
+    "atom-d3": ("atom", 3, False, {}),
+    "atom-d2-noedgefeatures": ("atom", 2, False, dict(d_e=0)),
+    "atom-d3-noedgefeatures-bias": ("atom", 3, True, dict(d_e=0)),
+    "atom-d3-bigatom": ("atom", 3, True, dict(bigatom=True)),
+    "mabbond-d1-bias": ("mabbond", 1, True, {}),
+    "mabbond-d3": ("mabbond", 3, False, {}),
+    "mabatom-d3-bias": ("mabatom", 3, True, {}),
+    "mabatom-d2-vertex": ("mabatom", 2, False, dict(edge=False)),
+}
+LAUNCH_GOLDEN = "launch_sequences.json"
+
+
+def _launch_record(name, sig, args, kwargs) -> list:
+    b = sig.bind(*args, **kwargs)
+    b.apply_defaults()
+    rec = []
+    for v in b.arguments.values():
+        if isinstance(v, torch.Tensor):
+            rec.append(list(v.shape) if name.startswith("pack_weight") else "T")
+        elif isinstance(v, (list, tuple)):
+            rec.append(len(v))
+        elif v is None or isinstance(v, (bool, int, float)):
+            rec.append(v)
+        else:                                       # layout, config: the same for every call of a run
+            rec.append(type(v).__name__)
+    if name == "wgrad_tc":                          # (dY, X, R, N, K, dW, acc) -> (dYs, X, R, N, K, dW, acc)
+        name, rec = "wgrad_tc_multi", [1] + rec[1:]
+    return [name] + rec
+
+
+def launch_sequence(case: str, monkeypatch) -> list:
+    """Forward + backward of LAUNCH_CASES[case] on the emulated kernels; returns the kernel-wrapper calls in order."""
+    import inspect
+
+    from chemprop_b200 import engine
+    from chemprop_b200.data import BatchMolGraph, make_molecules
+    from chemprop_b200.nn import (AtomMessagePassing, BondMessagePassing, MABAtomMessagePassing, MABBondMessagePassing,
+                                  MeanAggregation)
+    from tests import emu_mab
+
+    kind, depth, bias, x = LAUNCH_CASES[case]
+    sigs = {n: inspect.signature(getattr(engine, n)) for n in _LAUNCH_WRAPPERS}
+    emu_mab.patch_engine(monkeypatch)
+    seq = []
+    for n in _LAUNCH_WRAPPERS:
+        f0 = getattr(engine, n)
+        monkeypatch.setattr(engine, n, lambda *a, _f=f0, _n=n, **k: (seq.append(_launch_record(_n, sigs[_n], a, k)),
+                                                                     _f(*a, **k))[1])
+    torch.manual_seed(5)
+    d_v, d_e = (106, x.get("d_e", 14)) if kind != "bond" else (72, 14)
+    mgs = make_molecules(9, seed=3, mean_atoms=10, std_atoms=4, min_atoms=2, d_v=d_v, d_e=max(d_e, 1), shuffle_edges=True)
+    if x.get("bigatom"):
+        mgs += make_molecules(1, seed=4, mean_atoms=135.0, std_atoms=3.0, min_atoms=130, max_atoms=140, d_v=d_v, d_e=d_e)
+    if d_e == 0:
+        mgs = [type(m)(V=m.V, E=m.E[:, :0], edge_index=m.edge_index, rev_edge_index=m.rev_edge_index) for m in mgs]
+    bmg = BatchMolGraph(mgs)
+    kw = dict(d_v=d_v, d_e=d_e, d_h=36, depth=depth, bias=bias, precision="bf16")
+    if kind.startswith("mab"):
+        cls = MABBondMessagePassing if kind == "mabbond" else MABAtomMessagePassing
+        mp = cls(return_edge_embeddings=x.get("edge", True), **kw)
+        assert not mp.uses_composed_tier()
+        H_v, H_e = mp(bmg)
+        loss = MeanAggregation()(H_v, bmg.batch).square().sum() + (H_e.square().sum() if H_e is not None else 0.0)
+    else:
+        cls = BondMessagePassing if kind == "bond" else AtomMessagePassing
+        mp = cls(dropout=x.get("dropout", 0.0), undirected=x.get("undirected", False), **kw)
+        mp.fused = x.get("fused", True)
+        mp.train()
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore", RuntimeWarning)       # the > 128-atom batch leaves the fused atom step
+            loss = MeanAggregation()(mp(bmg), bmg.batch).float().square().sum()
+        assert not mp.uses_composed_tier(engine.get_layout(bmg))
+    loss.backward()
+    return seq
+
+
+@pytest.mark.parametrize("case", list(LAUNCH_CASES))
+def test_bf16_tier_launch_sequence(case, monkeypatch):
+    """The bf16 tier's kernel launches, forward and backward, in order, with their sizes and flags, for bond (depth 1-3, with
+    and without bias, training dropout, undirected, fused=False), fused atom (with and without bond features), the two-launch
+    atom step (a molecule of more than 128 atoms) and both mol-atom-bond kinds: a refactor of the host code must leave this
+    sequence as it is (tests/golden/launch_sequences.json, written by `python -m tests.test_host_logic`)."""
+    import json
+
+    from tests.util import GOLDEN_DIR
+
+    with open(os.path.join(GOLDEN_DIR, LAUNCH_GOLDEN)) as fh:
+        want = json.load(fh)[case]
+    got = json.loads(json.dumps(launch_sequence(case, monkeypatch)))
+    for i, (g, w) in enumerate(zip(got, want)):
+        assert g == w, (i, g, w)
+    assert len(got) == len(want)
+
+
+if __name__ == "__main__":
+    import json
+
+    from tests.util import GOLDEN_DIR
+
+    out = {}
+    for c in LAUNCH_CASES:
+        with pytest.MonkeyPatch.context() as m:
+            out[c] = launch_sequence(c, m)
+    with open(os.path.join(GOLDEN_DIR, LAUNCH_GOLDEN), "w") as fh:
+        json.dump(out, fh, indent=0)
+        fh.write("\n")

@@ -7,9 +7,6 @@ from chemprop_b200.data import BatchMolGraph, make_molecules
 from chemprop_b200.nn import BondMessagePassing, MeanAggregation
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 10000
-if len(sys.argv) > 2:
-    import chemprop_b200.engine as _eng
-    _eng.SUM_IN_EPILOGUE = bool(int(sys.argv[2]))
 steps = 5
 dev = torch.device("cuda")
 torch.manual_seed(0)
