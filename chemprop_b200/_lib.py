@@ -96,10 +96,19 @@ SIGNATURES = {
     "dmpnn_evidential_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _f32, _vp, _vp, _i64, _vp]),
     "dmpnn_quantile_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _i64, _vp]),
     "dmpnn_dirichlet_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _f32, _vp, _vp, _i64, _vp]),
+    "dmpnn_regression_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp, _i64, _vp]),
+    "dmpnn_spectral_transform": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _vp, _i64, _vp]),
+    "dmpnn_spectral_transform_bwd": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _i64, _i32, _vp, _i64, _vp]),
+    "dmpnn_spectral_loss_workspace_bytes": (C.c_int, [_i64, C.POINTER(_sz)]),
+    "dmpnn_sid_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _i64, _vp, _vp]),
+    "dmpnn_wasserstein_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _i64, _vp, _vp]),
 }
 
 # dmpnn_pred_transform kinds (include/dmpnn.h)
 PRED_REGRESSION, PRED_MVE, PRED_EVIDENTIAL, PRED_QUANTILE, PRED_DIRICHLET, PRED_DIRICHLET_PROBS, PRED_DIRICHLET_BINARY = range(7)
+# dmpnn_regression_loss kinds and dmpnn_spectral_transform activations (include/dmpnn.h)
+LOSS_MSE, LOSS_MAE, LOSS_RMSE = range(3)
+SPEC_SOFTPLUS, SPEC_EXP = range(2)
 
 
 class DmpnnError(RuntimeError):

@@ -15,6 +15,10 @@
 //                        predictors (softplus, + 1, eval-mode unscaling), and its mirror
 //   dmpnn_mve_loss, dmpnn_evidential_loss, dmpnn_quantile_loss, dmpnn_dirichlet_loss
 //                        the uncertainty criteria (metrics.py:202-257, 502-544, 588-613) under the same reduction, one launch
+//   dmpnn_regression_loss  MSE / MAE / RMSE and their bounded variants (metrics.py:128-169); dmpnn_mse_loss is its MSE case
+//   dmpnn_spectral_transform(_bwd), dmpnn_sid_loss, dmpnn_wasserstein_loss
+//                        SpectralFFN's output and the SID / Wasserstein criteria (predictors.py:342-376, metrics.py:547-585),
+//                        one CTA per spectrum row
 #include <math_constants.h>
 
 #include <algorithm>
@@ -122,10 +126,24 @@ k_bn_bwd(const float* __restrict__ dY, int64_t lddy, const float* __restrict__ X
     dX[r * lddx + c] = k * ((float)B * dY[r * lddy + c] - sdy - Xhat[r * ldh + c] * sdyx);
 }
 
-// one block: loss[0] = sum_{b,t} w_b tw_t m_bt (p - y)^2 / sum m,  dP = 2 w tw m (p - y) / sum m   (m = isfinite(y))
+enum RegLossKind { kMseLoss = 0, kMaeLoss = 1, kRmseLoss = 2 };
+
+// p - y, or 0 where BoundedMixin (metrics.py:144-149) replaces the prediction by the target: p < y with lt_mask set, or
+// p > y with gt_mask set (a censored target the prediction already satisfies; torch.where passes no gradient there)
+__device__ __forceinline__ float reg_residual(float p, float y, const uint8_t* lt, const uint8_t* gt, int64_t i) {
+  if ((lt && lt[i] && p < y) || (gt && gt[i] && p > y)) return 0.f;
+  return p - y;
+}
+
+// one block: MSE  loss[0] = sum_{b,t} w_b tw_t m_bt e^2 / sum m,  dP = 2 w tw m e / sum m   (m = isfinite(y), e = p - y)
+//            MAE  |e| in place of e^2, dP = w tw m sign(e) / sum m (sign(0) = 0, as torch's abs)
+//            RMSE sqrt of the MSE value, dP = the MSE's dP / (2 loss) (0 where the loss is 0)
+// lt / gt (nullable, row stride ldm): the bounded variants' residual (reg_residual)
 __global__ void __launch_bounds__(1024)
-k_mse_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y, int64_t ldy, const float* __restrict__ w,
-           const float* __restrict__ tw, int64_t B, int T, float* __restrict__ loss, float* __restrict__ dP, int64_t lddp) {
+k_regression_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y, int64_t ldy,
+                  const float* __restrict__ w, const float* __restrict__ tw, const uint8_t* __restrict__ lt,
+                  const uint8_t* __restrict__ gt, int64_t ldm, int64_t B, int T, int kind, float* __restrict__ loss,
+                  float* __restrict__ dP, int64_t lddp) {
   __shared__ float s_l[32], s_n[32];
   __shared__ float s_tot[2];
   const int64_t n = B * (int64_t)T;
@@ -135,8 +153,9 @@ k_mse_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y
     const int t = (int)(i - b * T);
     const float y = Y[b * ldy + t];
     if (isfinite(y)) {
-      const float e = P[b * ldp + t] - y;
-      l = fmaf((w ? w[b] : 1.f) * (tw ? tw[t] : 1.f) * e, e, l);
+      const float e = reg_residual(P[b * ldp + t], y, lt, gt, b * ldm + t);
+      if (kind == kMaeLoss) l = fmaf((w ? w[b] : 1.f) * (tw ? tw[t] : 1.f), fabsf(e), l);
+      else l = fmaf((w ? w[b] : 1.f) * (tw ? tw[t] : 1.f) * e, e, l);
       cnt += 1.f;
     }
   }
@@ -150,18 +169,29 @@ k_mse_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y
   if (threadIdx.x == 0) {
     float tl = 0.f, tn = 0.f;
     for (int k = 0; k < (int)(blockDim.x >> 5); ++k) { tl += s_l[k]; tn += s_n[k]; }
-    s_tot[0] = tl;
+    const float mse = tn > 0.f ? tl / tn : 0.f;
+    s_tot[0] = kind == kRmseLoss ? sqrtf(mse) : mse;
     s_tot[1] = tn;
-    loss[0] = tn > 0.f ? tl / tn : 0.f;
+    loss[0] = s_tot[0];
   }
   __syncthreads();
   const float inv_n = s_tot[1] > 0.f ? 1.f / s_tot[1] : 0.f;
+  const float rmse_scale = kind == kRmseLoss ? (s_tot[0] > 0.f ? 0.5f / s_tot[0] : 0.f) : 1.f;
   if (dP != nullptr)
     for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
       const int64_t b = i / T;
       const int t = (int)(i - b * T);
       const float y = Y[b * ldy + t];
-      dP[b * lddp + t] = isfinite(y) ? 2.f * (w ? w[b] : 1.f) * (tw ? tw[t] : 1.f) * (P[b * ldp + t] - y) * inv_n : 0.f;
+      float g = 0.f;
+      if (isfinite(y)) {
+        const float e = reg_residual(P[b * ldp + t], y, lt, gt, b * ldm + t);
+        if (kind == kMaeLoss)
+          g = (w ? w[b] : 1.f) * (tw ? tw[t] : 1.f) * (e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f)) * inv_n;
+        else
+          g = 2.f * (w ? w[b] : 1.f) * (tw ? tw[t] : 1.f) * e * inv_n;
+        if (kind == kRmseLoss) g *= rmse_scale;
+      }
+      dP[b * lddp + t] = g;
     }
 }
 
@@ -560,6 +590,223 @@ k_uq_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y,
     }
 }
 
+// ---- spectral predictor (chemprop/nn/predictors.py:339-376; nn/metrics.py:547-585) ---------------------------------------
+// One CTA of kRowThreads per spectrum row (b); a row of T bins is walked in chunks of kRowThreads, so any T works.  Every
+// sum and scan runs in thread order, then warp order: deterministic.
+constexpr int kRowThreads = 256;
+constexpr int kCountBlocks = 128;       // partial mask counts of the count prepass (workspace entries)
+enum SpecAct { kSpecSoftplus = 0, kSpecExp = 1 };
+
+// a(a(x)) (SpectralFFN's activation is applied twice) and its derivative; softplus is the predictors' softplus20
+template <int ACT>
+__device__ __forceinline__ float spec_act2(float x) {
+  if constexpr (ACT == kSpecExp) return expf(expf(x));
+  else return softplus20(softplus20(x));
+}
+template <int ACT>
+__device__ __forceinline__ float spec_act2_grad(float x) {
+  if constexpr (ACT == kSpecExp) {
+    const float e = expf(x);
+    return expf(e) * e;
+  } else {
+    return softplus20_grad(softplus20(x)) * softplus20_grad(x);
+  }
+}
+
+// inclusive prefix sum over the block in thread order (lanes by shuffles, then the preceding warps' totals in order); *total
+// gets the block's total.  Contains two __syncthreads.
+__device__ __forceinline__ float block_scan(float v, float* total) {
+  __shared__ float s_w[kRowThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float u = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += u;
+  }
+  if (lane == 31) s_w[warp] = v;
+  __syncthreads();
+  float off = 0.f, tot = 0.f;
+#pragma unroll
+  for (int k = 0; k < kRowThreads / 32; ++k) {
+    if (k == warp) off = tot;
+    tot += s_w[k];
+  }
+  __syncthreads();
+  *total = tot;
+  return v + off;
+}
+
+// out row = a(a(x)) / sum_j a(a(x_j))
+template <int ACT>
+__global__ void __launch_bounds__(kRowThreads)
+k_spectral_transform(const float* __restrict__ X, int64_t ldx, int T, float* __restrict__ out, int64_t ldo) {
+  const float* x = X + blockIdx.x * ldx;
+  float* o = out + blockIdx.x * ldo;
+  float s = 0.f;
+  for (int j = threadIdx.x; j < T; j += kRowThreads) s += spec_act2<ACT>(x[j]);
+  const float S = block_sum2(s, 0.f).x;
+  for (int j = threadIdx.x; j < T; j += kRowThreads) o[j] = spec_act2<ACT>(x[j]) / S;
+}
+
+// mirror: y = a(a(x)), S = sum y, dX_j = (g_j - sum_i g_i y_i / S) / S * a'(a(x_j)) a'(x_j)
+template <int ACT>
+__global__ void __launch_bounds__(kRowThreads)
+k_spectral_transform_bwd(const float* __restrict__ X, int64_t ldx, const float* __restrict__ dO, int64_t lddo, int T,
+                         float* __restrict__ dX, int64_t lddx) {
+  const float* x = X + blockIdx.x * ldx;
+  const float* g = dO + blockIdx.x * lddo;
+  float* d = dX + blockIdx.x * lddx;
+  float s = 0.f, gy = 0.f;
+  for (int j = threadIdx.x; j < T; j += kRowThreads) {
+    const float y = spec_act2<ACT>(x[j]);
+    s += y;
+    gy = fmaf(g[j], y, gy);
+  }
+  const float2 tot = block_sum2(s, gy);
+  const float S = tot.x, dot = tot.y / tot.x;
+  for (int j = threadIdx.x; j < T; j += kRowThreads) d[j] = (g[j] - dot) / S * spec_act2_grad<ACT>(x[j]);
+}
+
+// count prepass: cnt[k] = number of finite targets in rows k, k + gridDim.x, ... (exact integers)
+__global__ void __launch_bounds__(kRowThreads)
+k_spectral_count(const float* __restrict__ Y, int64_t ldy, int64_t B, int T, long long* __restrict__ cnt) {
+  __shared__ long long s_c[kRowThreads / 32];
+  long long c = 0;
+  for (int64_t b = blockIdx.x; b < B; b += gridDim.x)
+    for (int j = threadIdx.x; j < T; j += kRowThreads) c += isfinite(Y[b * ldy + j]) ? 1 : 0;
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
+  if ((threadIdx.x & 31) == 0) s_c[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    long long t = 0;
+    for (int k = 0; k < kRowThreads / 32; ++k) t += s_c[k];
+    cnt[blockIdx.x] = t;
+  }
+}
+
+// sum m over the batch from the prepass' n_cnt partials (integers: any order is exact)
+__device__ __forceinline__ long long spectral_total_count(const long long* cnt, int n_cnt) {
+  __shared__ long long s_n;
+  if (threadIdx.x < 32) {
+    long long c = 0;
+    for (int k = threadIdx.x; k < n_cnt; k += 32) c += cnt[k];
+    for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
+    if (threadIdx.x == 0) s_n = c;
+  }
+  __syncthreads();
+  return s_n;
+}
+
+// pred clamped at the threshold (NaN: no clamp; NaN preds stay NaN as in torch.clamp) and whether clamp passes the
+// gradient (torch: where pred >= threshold)
+__device__ __forceinline__ float spec_clamp(float p, float thr, bool* pass) {
+  if (isnan(thr)) { *pass = true; return p; }
+  *pass = p >= thr;
+  return p < thr ? thr : p;
+}
+
+// One CTA per row b.  c = clamp(p), S = sum_j m_j c_j, pn = c / S.  row_loss[b] = sum_j w tw m L_j (not yet divided by
+// sum m); dP (nullable) = dLoss / dp, also used as the row's scratch between passes.  A row with no finite target writes
+// row_loss 0 and dP 0.
+//   SID          L_j = pn log(pn / t) + t log(t / pn) on the masked-in bins; dL/dpn = log(pn / t) + 1 - t / pn
+//   Wasserstein  L_j = |cumsum(t0)_j - cumsum(pn)_j|, t0 = t with masked bins 0, pn over every bin;
+//                dLoss/dpn_k = G_k = -sum_{j >= k} w tw m_j sign(D_j)  (a reverse scan; sign(0) = 0)
+// then dLoss/dc_k = (G_k - m_k sum_i G_i pn_i) / S, times [p_k >= threshold].
+template <bool WASS>
+__global__ void __launch_bounds__(kRowThreads)
+k_spectral_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y, int64_t ldy,
+                const float* __restrict__ w, const float* __restrict__ tw, int T, float thr,
+                const long long* __restrict__ cnt, int n_cnt, float* __restrict__ row_loss, float* __restrict__ dP,
+                int64_t lddp) {
+  const int64_t b = blockIdx.x;
+  const float* p = P + b * ldp;
+  const float* y = Y + b * ldy;
+  float* d = dP ? dP + b * lddp : nullptr;
+  const float wb = w ? w[b] : 1.f;
+  bool pass;
+  float s = 0.f, n = 0.f;
+  for (int j = threadIdx.x; j < T; j += kRowThreads)
+    if (isfinite(y[j])) { s += spec_clamp(p[j], thr, &pass); n += 1.f; }
+  const float2 sn = block_sum2(s, n);
+  if (sn.y == 0.f) {                                 // every bin masked: no loss, no gradient
+    if (threadIdx.x == 0) row_loss[b] = 0.f;
+    if (d) for (int j = threadIdx.x; j < T; j += kRowThreads) d[j] = 0.f;
+    return;
+  }
+  const float S = sn.x;
+  float l = 0.f, gpn = 0.f;
+  if constexpr (!WASS) {
+    for (int j = threadIdx.x; j < T; j += kRowThreads) {
+      const float t = y[j];
+      float g = 0.f;
+      if (isfinite(t)) {
+        const float pn = spec_clamp(p[j], thr, &pass) / S;
+        const float W = wb * (tw ? tw[j] : 1.f);
+        const float lr = logf(pn / t);
+        l = fmaf(W, pn * lr + t * logf(t / pn), l);
+        g = t == 0.f ? CUDART_NAN_F : W * (lr + 1.f - t / pn);
+        gpn = fmaf(g, pn, gpn);
+      }
+      if (d) d[j] = g;
+    }
+  } else {
+    float ct = 0.f, cp = 0.f;                        // carries of the two cumsums
+    for (int base = 0; base < T; base += kRowThreads) {
+      const int j = base + threadIdx.x;
+      const bool in = j < T;
+      const float t = in ? y[j] : 0.f;
+      const bool m = in && isfinite(t);
+      const float pn = in ? spec_clamp(p[j], thr, &pass) / S : 0.f;
+      float tt, tp;
+      const float Ct = block_scan(m ? t : 0.f, &tt) + ct;
+      const float Cp = block_scan(pn, &tp) + cp;
+      ct += tt;
+      cp += tp;
+      const float D = Ct - Cp;
+      const float W = m ? wb * (tw ? tw[j] : 1.f) : 0.f;
+      l = fmaf(W, fabsf(D), l);
+      if (d && in) d[j] = W * (D > 0.f ? 1.f : (D < 0.f ? -1.f : 0.f));
+    }
+    if (d) {
+      __syncthreads();                               // the sign terms of other threads' bins
+      float cg = 0.f;
+      for (int base = (T - 1) / kRowThreads * kRowThreads; base >= 0; base -= kRowThreads) {
+        const int j = base + (kRowThreads - 1 - threadIdx.x);       // thread order = descending bins
+        const bool in = j < T;
+        float tg;
+        const float G = -(block_scan(in ? d[j] : 0.f, &tg) + cg);
+        cg += tg;
+        if (in) {
+          d[j] = G;
+          gpn = fmaf(G, spec_clamp(p[j], thr, &pass) / S, gpn);
+        }
+      }
+    }
+  }
+  const float2 lg = block_sum2(l, gpn);              // also orders the scratch writes before the reads below
+  if (threadIdx.x == 0) row_loss[b] = lg.x;
+  if (!d) return;
+  const long long N = spectral_total_count(cnt, n_cnt);
+  const float inv_n = 1.f / (float)N;
+  for (int j = threadIdx.x; j < T; j += kRowThreads) {
+    const bool m = isfinite(y[j]);
+    spec_clamp(p[j], thr, &pass);
+    const float G = d[j];
+    d[j] = (WASS || m) && pass ? (G - (m ? lg.y : 0.f)) / S * inv_n : 0.f;
+  }
+}
+
+// loss[0] = sum_b row_loss[b] / sum m (0 when every target is masked), one block, fixed order
+__global__ void __launch_bounds__(1024)
+k_spectral_loss_finish(const float* __restrict__ row_loss, int64_t B, const long long* __restrict__ cnt, int n_cnt,
+                       float* __restrict__ loss) {
+  float l = 0.f;
+  for (int64_t b = threadIdx.x; b < B; b += blockDim.x) l += row_loss[b];
+  const float tot = block_sum2(l, 0.f).x;
+  const long long N = spectral_total_count(cnt, n_cnt);
+  if (threadIdx.x == 0) loss[0] = N > 0 ? tot / (float)N : 0.f;
+}
+
 }  // namespace head
 }  // namespace dmpnn
 
@@ -590,13 +837,28 @@ extern "C" int dmpnn_bn_bwd(const float* dY, int64_t lddy, const float* Xhat, in
   return 0;
 }
 
+extern "C" int dmpnn_regression_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                                     const float* task_weights, const uint8_t* lt_mask, const uint8_t* gt_mask, int64_t ldm,
+                                     int64_t B, int64_t T, int kind, float* loss, float* dP, int64_t lddp, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(kind >= head::kMseLoss && kind <= head::kRmseLoss, "regression_loss: unknown kind");
+  DMPNN_CHECK_ARG(B >= 0 && T > 0 && T <= INT32_MAX && loss && (B == 0 || (P && Y)), "regression_loss: bad args");
+  DMPNN_CHECK_ARG(ldp >= T && ldy >= T && (dP == nullptr || lddp >= T) && ((!lt_mask && !gt_mask) || ldm >= T),
+                  "regression_loss: row strides too small");
+  head::k_regression_loss<<<1, 1024, 0, st>>>(P, ldp, Y, ldy, weights, task_weights, lt_mask, gt_mask, ldm, B, (int)T,
+                                              kind, loss, dP, lddp);
+  DMPNN_CHECK_LAUNCH("regression_loss", 1);
+  return 0;
+}
+
 extern "C" int dmpnn_mse_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
                               const float* task_weights, int64_t B, int64_t T, float* loss, float* dP, int64_t lddp,
                               void* stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
   DMPNN_CHECK_ARG(B >= 0 && T > 0 && loss && (B == 0 || (P && Y)), "mse_loss: bad args");
   DMPNN_CHECK_ARG(ldp >= T && ldy >= T && (dP == nullptr || lddp >= T), "mse_loss: row strides too small");
-  head::k_mse_loss<<<1, 1024, 0, st>>>(P, ldp, Y, ldy, weights, task_weights, B, (int)T, loss, dP, lddp);
+  head::k_regression_loss<<<1, 1024, 0, st>>>(P, ldp, Y, ldy, weights, task_weights, nullptr, nullptr, 0, B, (int)T,
+                                              head::kMseLoss, loss, dP, lddp);
   DMPNN_CHECK_LAUNCH("mse_loss", 1);
   return 0;
 }
@@ -723,4 +985,84 @@ extern "C" int dmpnn_dirichlet_loss(const float* P, int64_t ldp, const float* Y,
   DMPNN_CHECK_ARG(C >= 1, "dirichlet_loss: bad args (C must be >= 1)");
   return uq_loss<head::kDirichlet>("dirichlet_loss: bad args or row strides too small", P, ldp, Y, ldy, weights,
                                    task_weights, B, T, C, v_kl, 0.f, loss, dP, lddp, stream);
+}
+
+extern "C" int dmpnn_spectral_transform(const float* X, int64_t ldx, int64_t B, int64_t T, int act, float* out, int64_t ldo,
+                                        void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(act == head::kSpecSoftplus || act == head::kSpecExp, "spectral_transform: unknown activation");
+  DMPNN_CHECK_ARG(B >= 0 && B <= INT32_MAX && T > 0 && T <= INT32_MAX && (B == 0 || (X && out)),
+                  "spectral_transform: bad args");
+  DMPNN_CHECK_ARG(ldx >= T && ldo >= T, "spectral_transform: row strides too small");
+  if (B == 0) return 0;
+  if (act == head::kSpecExp)
+    head::k_spectral_transform<head::kSpecExp><<<(unsigned)B, head::kRowThreads, 0, st>>>(X, ldx, (int)T, out, ldo);
+  else
+    head::k_spectral_transform<head::kSpecSoftplus><<<(unsigned)B, head::kRowThreads, 0, st>>>(X, ldx, (int)T, out, ldo);
+  DMPNN_CHECK_LAUNCH("spectral_transform", 1);
+  return 0;
+}
+
+extern "C" int dmpnn_spectral_transform_bwd(const float* X, int64_t ldx, const float* dOut, int64_t lddo, int64_t B,
+                                            int64_t T, int act, float* dX, int64_t lddx, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(act == head::kSpecSoftplus || act == head::kSpecExp, "spectral_transform_bwd: unknown activation");
+  DMPNN_CHECK_ARG(B >= 0 && B <= INT32_MAX && T > 0 && T <= INT32_MAX && (B == 0 || (X && dOut && dX)),
+                  "spectral_transform_bwd: bad args");
+  DMPNN_CHECK_ARG(ldx >= T && lddo >= T && lddx >= T, "spectral_transform_bwd: row strides too small");
+  if (B == 0) return 0;
+  if (act == head::kSpecExp)
+    head::k_spectral_transform_bwd<head::kSpecExp><<<(unsigned)B, head::kRowThreads, 0, st>>>(X, ldx, dOut, lddo, (int)T,
+                                                                                             dX, lddx);
+  else
+    head::k_spectral_transform_bwd<head::kSpecSoftplus><<<(unsigned)B, head::kRowThreads, 0, st>>>(X, ldx, dOut, lddo,
+                                                                                                  (int)T, dX, lddx);
+  DMPNN_CHECK_LAUNCH("spectral_transform_bwd", 1);
+  return 0;
+}
+
+// workspace of the two spectral losses: the count prepass' partials, then one loss partial per row
+static int64_t spectral_count_blocks(int64_t B) { return std::min<int64_t>(B, head::kCountBlocks); }
+static size_t spectral_row_offset(int64_t B) { return (size_t)spectral_count_blocks(B) * sizeof(long long); }
+
+extern "C" int dmpnn_spectral_loss_workspace_bytes(int64_t B, size_t* bytes) {
+  DMPNN_CHECK_ARG(B >= 0 && B <= INT32_MAX && bytes, "spectral_loss_workspace_bytes: bad args");
+  *bytes = spectral_row_offset(B) + (size_t)B * sizeof(float);
+  return 0;
+}
+
+template <bool WASS>
+static int spectral_loss(const char* name, const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                         const float* task_weights, int64_t B, int64_t T, float threshold, float* loss, float* dP,
+                         int64_t lddp, void* workspace, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(B >= 0 && B <= INT32_MAX && T > 0 && T <= INT32_MAX && loss && (B == 0 || (P && Y && workspace)),
+                  "%s: bad args", name);
+  DMPNN_CHECK_ARG(ldp >= T && ldy >= T && (dP == nullptr || lddp >= T), "%s: row strides too small", name);
+  DMPNN_CHECK_ARG(!std::isinf(threshold), "%s: threshold must be finite, or NaN for none", name);
+  const int n_cnt = (int)spectral_count_blocks(B);
+  long long* cnt = (long long*)workspace;
+  float* row_loss = B ? (float*)((char*)workspace + spectral_row_offset(B)) : nullptr;
+  if (B > 0) {
+    head::k_spectral_count<<<(unsigned)n_cnt, head::kRowThreads, 0, st>>>(Y, ldy, B, (int)T, cnt);
+    head::k_spectral_loss<WASS><<<(unsigned)B, head::kRowThreads, 0, st>>>(P, ldp, Y, ldy, weights, task_weights, (int)T,
+                                                                          threshold, cnt, n_cnt, row_loss, dP, lddp);
+  }
+  head::k_spectral_loss_finish<<<1, 1024, 0, st>>>(row_loss, B, cnt, n_cnt, loss);
+  DMPNN_CHECK_LAUNCH(name, B > 0 ? 3 : 1);
+  return 0;
+}
+
+extern "C" int dmpnn_sid_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                              const float* task_weights, int64_t B, int64_t T, float threshold, float* loss, float* dP,
+                              int64_t lddp, void* workspace, void* stream) {
+  return spectral_loss<false>("sid_loss", P, ldp, Y, ldy, weights, task_weights, B, T, threshold, loss, dP, lddp, workspace,
+                              stream);
+}
+
+extern "C" int dmpnn_wasserstein_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                                      const float* task_weights, int64_t B, int64_t T, float threshold, float* loss,
+                                      float* dP, int64_t lddp, void* workspace, void* stream) {
+  return spectral_loss<true>("wasserstein_loss", P, ldp, Y, ldy, weights, task_weights, B, T, threshold, loss, dP, lddp,
+                             workspace, stream);
 }

@@ -682,6 +682,60 @@ def dirichlet_loss(P: Tensor, Y: Tensor, w, tw, C: int, v_kl: float, loss: Tenso
     _lib.check(rc, "dmpnn_dirichlet_loss")
 
 
+def regression_loss(P: Tensor, Y: Tensor, w, tw, lt_mask, gt_mask, kind: int, loss: Tensor, dP: Tensor):
+    """MSE / MAE / RMSE (_lib.LOSS_*) on P, Y (B x T); lt_mask / gt_mask (B x T uint8 with Y's row stride, or None) give
+    the bounded variants."""
+    lib = _lib.load()
+    B, T = P.shape
+    ldm = T
+    for m in (lt_mask, gt_mask):
+        if m is not None:
+            assert m.dtype == torch.uint8 and m.shape == (B, T) and m.is_contiguous(), "masks: contiguous B x T uint8"
+    rc = lib.dmpnn_regression_loss(P.data_ptr(), P.stride(0) if B else T, Y.data_ptr(), Y.stride(0) if B else T, _ptr(w),
+                                   _ptr(tw), _ptr(lt_mask), _ptr(gt_mask), ldm, B, T, kind, loss.data_ptr(), _ptr(dP),
+                                   dP.stride(0) if B else T, _stream())
+    _lib.check(rc, "dmpnn_regression_loss")
+
+
+def spectral_transform(X: Tensor, act: int, out: Tensor):
+    """out (B x T) = a(a(X)) normalised per row, a = softplus or exp (_lib.SPEC_*)."""
+    lib = _lib.load()
+    B, T = X.shape
+    rc = lib.dmpnn_spectral_transform(X.data_ptr(), X.stride(0) if B else T, B, T, act, out.data_ptr(),
+                                      out.stride(0) if B else T, _stream())
+    _lib.check(rc, "dmpnn_spectral_transform")
+
+
+def spectral_transform_bwd(X: Tensor, dOut: Tensor, act: int, dX: Tensor):
+    lib = _lib.load()
+    B, T = X.shape
+    rc = lib.dmpnn_spectral_transform_bwd(X.data_ptr(), X.stride(0) if B else T, dOut.data_ptr(), dOut.stride(0) if B else T,
+                                          B, T, act, dX.data_ptr(), dX.stride(0) if B else T, _stream())
+    _lib.check(rc, "dmpnn_spectral_transform_bwd")
+
+
+def _spectral_loss(fn: str, P: Tensor, Y: Tensor, w, tw, threshold, loss: Tensor, dP: Tensor):
+    lib = _lib.load()
+    B, T = P.shape
+    n = C.c_size_t(0)
+    _lib.check(lib.dmpnn_spectral_loss_workspace_bytes(B, C.byref(n)), "dmpnn_spectral_loss_workspace_bytes")
+    ws = torch.empty(max(n.value, 1), dtype=torch.uint8, device=P.device)
+    thr = float("nan") if threshold is None else float(threshold)
+    rc = getattr(lib, fn)(P.data_ptr(), P.stride(0) if B else T, Y.data_ptr(), Y.stride(0) if B else T, _ptr(w), _ptr(tw), B,
+                          T, thr, loss.data_ptr(), _ptr(dP), dP.stride(0) if B else T, ws.data_ptr(), _stream())
+    _lib.check(rc, fn)
+
+
+def sid_loss(P: Tensor, Y: Tensor, w, tw, threshold, loss: Tensor, dP: Tensor):
+    """SID on spectra P and targets Y (B x T, NaN = masked bin); threshold None = no clamp."""
+    _spectral_loss("dmpnn_sid_loss", P, Y, w, tw, threshold, loss, dP)
+
+
+def wasserstein_loss(P: Tensor, Y: Tensor, w, tw, threshold, loss: Tensor, dP: Tensor):
+    """Wasserstein (earth mover's) distance of the cumulative spectra; arguments as sid_loss."""
+    _spectral_loss("dmpnn_wasserstein_loss", P, Y, w, tw, threshold, loss, dP)
+
+
 def column_sum(Y: Tensor, R: int, N: int, out: Tensor, *, accumulate: bool = False):
     lib = _lib.load()
     n = C.c_size_t(0)

@@ -1,10 +1,11 @@
 from .agg import (Aggregation, AggregationRegistry, AttentiveAggregation, MeanAggregation, NormAggregation,
                   SumAggregation)
 from .constrainer import ConstrainerFFN
-from .head import (EngineBatchNorm1d, EngineBinaryClassificationFFN, EngineBinaryDirichletFFN, EngineDirichletLoss,
-                   EngineEvidentialFFN, EngineEvidentialLoss, EngineLinear, EngineMPNN, EngineMulticlassClassificationFFN,
-                   EngineMulticlassDirichletFFN, EngineMveFFN, EngineMVELoss, EngineQuantileFFN, EngineQuantileLoss,
-                   EngineRegressionFFN)
+from .head import (EngineBatchNorm1d, EngineBinaryClassificationFFN, EngineBinaryDirichletFFN, EngineBoundedMAE,
+                   EngineBoundedMSE, EngineBoundedRMSE, EngineDirichletLoss, EngineEvidentialFFN, EngineEvidentialLoss,
+                   EngineLinear, EngineMAE, EngineMPNN, EngineMulticlassClassificationFFN, EngineMulticlassDirichletFFN,
+                   EngineMveFFN, EngineMVELoss, EngineQuantileFFN, EngineQuantileLoss, EngineRegressionFFN, EngineRMSE,
+                   EngineSID, EngineSpectralFFN, EngineWasserstein)
 from .message_passing import AtomMessagePassing, BondMessagePassing
 from .mol_atom_bond import MABAtomMessagePassing, MABBondMessagePassing
 from .transforms import GraphTransform, ScaleTransform, UnscaleTransform
@@ -14,4 +15,6 @@ __all__ = ["Aggregation", "AggregationRegistry", "AttentiveAggregation", "MeanAg
            "GraphTransform", "ScaleTransform", "UnscaleTransform", "EngineMPNN", "EngineRegressionFFN",
            "EngineBinaryClassificationFFN", "EngineMulticlassClassificationFFN", "EngineMveFFN", "EngineEvidentialFFN",
            "EngineQuantileFFN", "EngineBinaryDirichletFFN", "EngineMulticlassDirichletFFN", "EngineMVELoss",
-           "EngineEvidentialLoss", "EngineQuantileLoss", "EngineDirichletLoss", "EngineBatchNorm1d", "EngineLinear"]
+           "EngineEvidentialLoss", "EngineQuantileLoss", "EngineDirichletLoss", "EngineSpectralFFN", "EngineSID",
+           "EngineWasserstein", "EngineMAE", "EngineRMSE", "EngineBoundedMSE", "EngineBoundedMAE", "EngineBoundedRMSE",
+           "EngineBatchNorm1d", "EngineLinear"]

@@ -275,9 +275,13 @@ class _Criterion(nn.Module):
 
     def forward(self, preds, targets, mask=None, weights=None, lt_mask=None, gt_mask=None):
         if lt_mask is not None or gt_mask is not None:
-            raise NotImplementedError("bounded MSE is not part of the engine's head; use the reference criterion")
-        t = targets if mask is None else torch.where(mask, targets, torch.full_like(targets, float("nan")))
-        return self._loss(preds, t, weights)
+            raise NotImplementedError(f"{type(self).__name__} takes no lt_mask / gt_mask; the bounded criteria "
+                                      "(EngineBoundedMSE, EngineBoundedMAE, EngineBoundedRMSE) do")
+        return self._loss(preds, self._masked(targets, mask), weights)
+
+    @staticmethod
+    def _masked(targets, mask):
+        return targets if mask is None else torch.where(mask, targets, torch.full_like(targets, float("nan")))
 
     def _loss(self, preds, targets, weights):
         return self._loss_fn.apply(preds, targets, weights, self.task_weights)
@@ -353,6 +357,165 @@ class EngineDirichletLoss(_Criterion):
         return f"v_kl={self.v_kl}"
 
 
+def _loss_weights(weights, task_weights, b: int, T: int):
+    """Per-molecule and per-task weights as contiguous f32 vectors of exactly b and T entries (or None), as the kernels read
+    them.  A 1-entry task weight (the criteria's default `task_weights=1.0`) broadcasts, as in the reference; any other size
+    is refused."""
+    w = None if weights is None else weights.float().reshape(-1)
+    tw = None if task_weights is None else task_weights.float().reshape(-1)
+    if tw is not None and tw.numel() == 1:
+        tw = tw.expand(T)
+    if (w is not None and w.numel() != b) or (tw is not None and tw.numel() != T):
+        raise ValueError(f"weights must have {b} entries and task_weights 1 or {T}, got "
+                         f"{None if w is None else w.numel()} and {None if tw is None else tw.numel()}")
+    return (None if w is None else w.contiguous()), (None if tw is None else tw.contiguous())
+
+
+class RegressionLossFunction(torch.autograd.Function):
+    """MSE / MAE / RMSE (_lib.LOSS_*) under the MSE criterion's reduction, optionally bounded by b x T lt / gt masks: loss
+    and dLoss/dPreds in one launch (dmpnn_regression_loss)."""
+
+    @staticmethod
+    def forward(ctx, preds, targets, weights, task_weights, lt_mask, gt_mask, kind):
+        K._require_cuda(preds, targets, lt_mask, gt_mask)
+        P, Y = preds.float().contiguous(), targets.float().contiguous()
+        if P.dim() != 2 or Y.shape != P.shape:
+            raise ValueError(f"preds and targets must both be b x T, got {tuple(P.shape)} and {tuple(Y.shape)}")
+        w, tw = _loss_weights(weights, task_weights, *P.shape)
+        lt, gt = (None if m is None else m.to(torch.uint8).expand(P.shape).contiguous() for m in (lt_mask, gt_mask))
+        loss = torch.empty(1, device=P.device)
+        dP = torch.empty_like(P)
+        K.regression_loss(P, Y, w, tw, lt, gt, kind, loss, dP)
+        ctx.save_for_backward(dP)
+        ctx.pdtype = preds.dtype
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        (dP,) = ctx.saved_tensors
+        return (dP * g).to(ctx.pdtype), None, None, None, None, None, None
+
+
+class SpectralTransformFunction(torch.autograd.Function):
+    """SpectralFFN's output from the raw MLP output X (b x T): a(a(X)) normalised per row, a = softplus or exp
+    (_lib.SPEC_*), in one launch (dmpnn_spectral_transform; mirror dmpnn_spectral_transform_bwd)."""
+
+    @staticmethod
+    def forward(ctx, X, act):
+        K._require_cuda(X)
+        Xc = X.float().contiguous()
+        out = torch.empty_like(Xc)
+        K.spectral_transform(Xc, act, out)
+        ctx.save_for_backward(Xc)
+        ctx.cfg = (act, X.dtype)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        (Xc,) = ctx.saved_tensors
+        act, dt = ctx.cfg
+        dX = torch.empty_like(Xc)
+        K.spectral_transform_bwd(Xc, g.float().contiguous(), act, dX)
+        return dX.to(dt), None
+
+
+class SpectralLossFunction(torch.autograd.Function):
+    """SID or Wasserstein (engine.sid_loss / engine.wasserstein_loss) on b x T spectra under the MSE criterion's
+    reduction: loss and dLoss/dPreds from dmpnn_sid_loss / dmpnn_wasserstein_loss."""
+
+    @staticmethod
+    def forward(ctx, preds, targets, weights, task_weights, name, threshold):
+        K._require_cuda(preds, targets)
+        P, Y = preds.float().contiguous(), targets.float().contiguous()
+        if P.dim() != 2 or Y.shape != P.shape:
+            raise ValueError(f"preds and targets must both be b x T, got {tuple(P.shape)} and {tuple(Y.shape)}")
+        w, tw = _loss_weights(weights, task_weights, *P.shape)
+        loss = torch.empty(1, device=P.device)
+        dP = torch.empty_like(P)
+        getattr(K, name)(P, Y, w, tw, threshold, loss, dP)
+        ctx.save_for_backward(dP)
+        ctx.pdtype = preds.dtype
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        (dP,) = ctx.saved_tensors
+        return (dP * g).to(ctx.pdtype), None, None, None, None, None
+
+
+class _RegressionCriterion(_Criterion):
+    """MSE / MAE / RMSE (`_kind`, _lib.LOSS_*) on b x T predictions, one launch of dmpnn_regression_loss; the `_bounded`
+    ones take the batch's `lt_mask` / `gt_mask` (BoundedMixin, nn/metrics.py:142-149), the others refuse them."""
+    _kind = _lib.LOSS_MSE
+    _bounded = False
+
+    def __init__(self, task_weights=1.0):
+        super().__init__(task_weights)
+
+    def forward(self, preds, targets, mask=None, weights=None, lt_mask=None, gt_mask=None):
+        if not self._bounded:
+            return super().forward(preds, targets, mask, weights, lt_mask, gt_mask)
+        return RegressionLossFunction.apply(preds, self._masked(targets, mask), weights, self.task_weights, lt_mask, gt_mask,
+                                            self._kind)
+
+    def _loss(self, preds, targets, weights):
+        return RegressionLossFunction.apply(preds, targets, weights, self.task_weights, None, None, self._kind)
+
+
+class EngineMAE(_RegressionCriterion):
+    """chemprop's MAE (nn/metrics.py:128-132): |preds - targets|."""
+    _kind = _lib.LOSS_MAE
+
+
+class EngineRMSE(_RegressionCriterion):
+    """chemprop's RMSE (nn/metrics.py:135-139): sqrt of the MSE value, the gradient through the sqrt."""
+    _kind = _lib.LOSS_RMSE
+
+
+class EngineBoundedMSE(_RegressionCriterion):
+    """chemprop's BoundedMSE (nn/metrics.py:142-157): MSE where a prediction on the allowed side of a censored target
+    (`lt_mask` and preds < targets, or `gt_mask` and preds > targets) counts as exact."""
+    _kind = _lib.LOSS_MSE
+    _bounded = True
+
+
+class EngineBoundedMAE(_RegressionCriterion):
+    """chemprop's BoundedMAE (nn/metrics.py:160-163)."""
+    _kind = _lib.LOSS_MAE
+    _bounded = True
+
+
+class EngineBoundedRMSE(_RegressionCriterion):
+    """chemprop's BoundedRMSE (nn/metrics.py:166-169)."""
+    _kind = _lib.LOSS_RMSE
+    _bounded = True
+
+
+class EngineSID(_Criterion):
+    """chemprop's SID (nn/metrics.py:547-566) on b x T spectra: predictions clamped at `threshold` (None: not clamped),
+    normalised over the masked-in bins, symmetric KL against the targets (dmpnn_sid_loss)."""
+    _name = "sid_loss"
+
+    def __init__(self, task_weights=1.0, threshold: float | None = None):
+        super().__init__(task_weights)
+        self.threshold = threshold
+
+    def _loss(self, preds, targets, weights):
+        return SpectralLossFunction.apply(preds, targets, weights, self.task_weights, self._name, self.threshold)
+
+    def extra_repr(self) -> str:
+        return f"threshold={self.threshold}"
+
+
+class EngineWasserstein(EngineSID):
+    """chemprop's Wasserstein (nn/metrics.py:569-585): |cumsum(targets) - cumsum(normalised preds)| per bin
+    (dmpnn_wasserstein_loss).  A masked bin -- a NaN target, or one `mask` excludes -- adds 0 to the target cumsum, as in
+    the reference's `MPNN.training_step`, whose criterion sees `targets.nan_to_num(0)`.  Called directly with a `mask` and
+    finite targets at the masked bins, the reference criterion would add those targets to its cumsum instead; the engine
+    does not read them."""
+    _name = "wasserstein_loss"
+
+
 class _EngineFFNPredictor(nn.Module):
     """`_FFNPredictorBase` (chemprop/nn/predictors.py:101-157) with the reference's module tree; GEMMs on the engine.  The
     MLP has n_tasks * n_targets outputs.  `criterion` replaces the default criterion (built from `task_weights`), and
@@ -398,7 +561,7 @@ class _EngineFFNPredictor(nn.Module):
     def _mlp(self, Z: Tensor) -> Tensor:
         """`self.ffn(Z)` (nn/ffn.py:38-61: Linear, then [act, dropout, Linear] per further layer) with every activation the
         engine fuses folded into the epilogue of the GEMM before it."""
-        blocks = [list(b) for b in self.ffn]
+        blocks = [list(b) for b in self.ffn if isinstance(b, nn.Sequential)]
         X = Z
         for k, block in enumerate(blocks):
             lin = block[-1]
@@ -524,6 +687,49 @@ class EngineMulticlassDirichletFFN(EngineMulticlassClassificationFFN):
         return PredTransformFunction.apply(self._mlp(Z), _lib.PRED_DIRICHLET, self.n_classes, None, None)
 
 
+class _Exp(nn.Module):
+    """`_Exp` of chemprop/nn/predictors.py:337-339 (SpectralFFN's "exp" activation)."""
+
+    def forward(self, X: Tensor) -> Tensor:
+        return X.exp()
+
+
+class EngineSpectralFFN(_EngineFFNPredictor):
+    """`SpectralFFN` (chemprop/nn/predictors.py:342-376): the MLP's b x T output goes through the spectral activation twice
+    (the reference appends it to `ffn` as `ffn.spectral_activation` and applies it again in `forward`) and is normalised
+    to sum 1 per row (dmpnn_spectral_transform); `train_step` is `forward`.  `spectral_activation` is "softplus" (or None)
+    or "exp".  Criterion: EngineSID(task_weights, threshold)."""
+    _criterion_cls = EngineSID
+
+    def __init__(self, n_tasks: int = 1, input_dim: int = DEFAULT_HIDDEN_DIM, hidden_dim: int | Sequence[int] = 300,
+                 n_layers: int = 1, dropout: float = 0.0, activation="relu", task_weights=None,
+                 threshold: float | None = None, spectral_activation: str | None = "softplus", *, criterion=None,
+                 output_transform=None):
+        if spectral_activation not in ("softplus", "exp", None):
+            raise ValueError(f"Unknown spectral activation: {spectral_activation}. "
+                             "Expected one of 'exp', 'softplus' or None.")
+        given = criterion
+        if criterion is None:
+            criterion = EngineSID(torch.ones(n_tasks) if task_weights is None else task_weights, threshold)
+        super().__init__(n_tasks, input_dim, hidden_dim, n_layers, dropout, activation, task_weights, criterion=criterion,
+                         output_transform=output_transform)
+        # every key the reference records (criterion and output_transform even when None), and what rebuilds the default
+        # criterion
+        self.hparams.update(criterion=given, output_transform=output_transform, task_weights=task_weights,
+                            threshold=threshold, spectral_activation=spectral_activation)
+        self._act = _lib.SPEC_EXP if spectral_activation == "exp" else _lib.SPEC_SOFTPLUS
+        self.ffn.add_module("spectral_activation", _Exp() if self._act == _lib.SPEC_EXP else nn.Softplus())
+
+    @property
+    def output_dim(self) -> int:
+        return self.ffn[-2][-1].out_features
+
+    def forward(self, Z: Tensor) -> Tensor:
+        return SpectralTransformFunction.apply(self._mlp(Z), self._act)
+
+    train_step = forward
+
+
 class EngineBatchNorm1d(nn.BatchNorm1d):
     """nn.BatchNorm1d (same parameters / buffers); training mode runs dmpnn_bn_train_fwd / dmpnn_bn_bwd."""
 
@@ -546,8 +752,9 @@ class EngineMPNN(nn.Module):
     """`chemprop.models.MPNN` reduced to the path (models/model.py:66-161): message passing -> aggregation -> batch norm ->
     predictor -> criterion, all on the engine.  The predictor is EngineRegressionFFN (the default),
     EngineBinaryClassificationFFN, EngineMulticlassClassificationFFN or one of the uncertainty predictors (EngineMveFFN,
-    EngineEvidentialFFN, EngineQuantileFFN, EngineBinaryDirichletFFN, EngineMulticlassDirichletFFN).
-    `training_loss(bmg, targets, weights=None)` is `MPNN.training_step` without Lightning's logging; `forward(bmg)` gives
+    EngineEvidentialFFN, EngineQuantileFFN, EngineBinaryDirichletFFN, EngineMulticlassDirichletFFN) or EngineSpectralFFN.
+    `training_loss(bmg, targets, weights=None, lt_mask=None, gt_mask=None)` is `MPNN.training_step` without Lightning's
+    logging (the b x T boolean lt / gt masks go to the bounded criteria); `forward(bmg)` gives
     the predictions (probabilities for the classification predictors).  `X_d_transform` (a ScaleTransform, as
     models/model.py:97) scales extra molecule descriptors X_d in eval mode before they join the fingerprint."""
 
@@ -567,6 +774,9 @@ class EngineMPNN(nn.Module):
     def forward(self, bmg, V_d: Tensor | None = None, X_d: Tensor | None = None) -> Tensor:
         return self.predictor(self.fingerprint(bmg, V_d, X_d))
 
-    def training_loss(self, bmg, targets: Tensor, weights: Tensor | None = None, V_d=None, X_d=None) -> Tensor:
+    def training_loss(self, bmg, targets: Tensor, weights: Tensor | None = None, V_d=None, X_d=None, *,
+                      lt_mask: Tensor | None = None, gt_mask: Tensor | None = None) -> Tensor:
         preds = self.predictor.train_step(self.fingerprint(bmg, V_d, X_d))
-        return self.predictor.criterion(preds, targets, None, weights)      # NaN targets are the mask (model.py:140-141)
+        if lt_mask is None and gt_mask is None:
+            return self.predictor.criterion(preds, targets, None, weights)  # NaN targets are the mask (model.py:140-141)
+        return self.predictor.criterion(preds, targets, None, weights, lt_mask, gt_mask)

@@ -545,6 +545,52 @@ int dmpnn_dirichlet_loss(const float* P, int64_t ldp, const float* Y, int64_t ld
                          const float* task_weights, int64_t B, int64_t T, int64_t C, float v_kl, float* loss, float* dP,
                          int64_t lddp, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Regression-loss family and the spectral predictor (csrc/head.cu; chemprop/nn/metrics.py:128-183, 547-585,
+ * nn/predictors.py:339-376):
+ *   dmpnn_regression_loss     kind 0 MSE, 1 MAE, 2 RMSE under dmpnn_mse_loss's reduction and masking (dmpnn_mse_loss is
+ *                             kind 0 without bounds, bit for bit).  MAE: L = |P - Y|, d|e|/de = 0 at e = 0 as torch's
+ *                             abs.  RMSE: loss[0] = sqrt(the MSE value), dP = the MSE's dP / (2 loss[0]); where the loss
+ *                             is 0 (every residual exactly 0) dP = 0 (the reference's sqrt backward gives 0 * inf = NaN).
+ *                             lt_mask / gt_mask (nullable uint8, B x T, row stride ldm) give the bounded variants: where
+ *                             lt_mask is set and P < Y, or gt_mask is set and P > Y, the residual is 0 and so are the term
+ *                             and its gradient (BoundedMixin's torch.where).  One block.
+ *   dmpnn_spectral_transform  SpectralFFN's output from the raw MLP output X (B x T): y = a(a(x)) (the reference applies
+ *                             its activation twice), out = y / sum_j y_j per row over every bin.  act 0 = softplus
+ *                             (dmpnn_pred_transform's, threshold 20), 1 = exp.  T = 1 gives exactly 1.
+ *   dmpnn_spectral_transform_bwd  the mirror: dX from dOut and the forward's X.
+ *   dmpnn_sid_loss            SID on P (B x T, the spectra) and Y (B x T): c = clamp(P, min = threshold) (threshold NaN:
+ *                             none; the gradient passes where P >= threshold, as torch's clamp), pn = c / sum_j m_j c_j
+ *                             per row, L = pn log(pn / y) + y log(y / pn) on the masked-in bins.
+ *   dmpnn_wasserstein_loss    L_j = |cumsum(y0)_j - cumsum(pn)_j| with y0 = Y where finite and 0 where masked, pn (as in
+ *                             SID) over every bin, masked or not; d|D|/dD = 0 at D = 0 (a cumsum tie), as torch's abs.
+ *   Both spectral losses reduce like dmpnn_mse_loss: loss[0] = sum_{b,j} w[b] tw[j] m L / sum m, m = isfinite(Y), dP
+ *   (nullable) = dloss/dP, every entry written.  Conventions where the reference gives NaN:
+ *     - a row with every bin masked adds 0 to the loss and has dP = 0 (SID's reference: NaN gradient; Wasserstein's:
+ *       NaN loss), and every target masked gives loss[0] = 0;
+ *     - SID with a masked-in target of exactly 0 keeps the reference's NaN: loss[0] is NaN and so is that row's dP at its
+ *       masked-in bins (its masked bins stay 0).
+ *   One CTA of 256 threads per row, bins in chunks of 256 (any T); Wasserstein's cumsums are chunked block scans, forward
+ *   for the loss and in reverse for the gradient.  The 1 / sum m of the gradient comes from a count prepass on the device,
+ *   and a one-block launch sums the per-row losses: three launches, fixed summation order (bitwise repeatable), no
+ *   floating-point atomics, no host synchronisation.  workspace: dmpnn_spectral_loss_workspace_bytes(B) bytes, any
+ *   contents (every byte read is written first by the same call).
+ * ------------------------------------------------------------------------------------- */
+int dmpnn_regression_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                          const float* task_weights, const uint8_t* lt_mask, const uint8_t* gt_mask, int64_t ldm, int64_t B,
+                          int64_t T, int kind, float* loss, float* dP, int64_t lddp, void* stream);
+int dmpnn_spectral_transform(const float* X, int64_t ldx, int64_t B, int64_t T, int act, float* out, int64_t ldo,
+                             void* stream);
+int dmpnn_spectral_transform_bwd(const float* X, int64_t ldx, const float* dOut, int64_t lddo, int64_t B, int64_t T, int act,
+                                 float* dX, int64_t lddx, void* stream);
+int dmpnn_spectral_loss_workspace_bytes(int64_t B, size_t* bytes);
+int dmpnn_sid_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                   const float* task_weights, int64_t B, int64_t T, float threshold, float* loss, float* dP, int64_t lddp,
+                   void* workspace, void* stream);
+int dmpnn_wasserstein_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                           const float* task_weights, int64_t B, int64_t T, float threshold, float* loss, float* dP,
+                           int64_t lddp, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
