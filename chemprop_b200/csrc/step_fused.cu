@@ -10,9 +10,10 @@
 //               over slab by slab (box s of the next tile is loaded when the message warps have left slab s)
 //   warp 1      TMA producer: W_h stages (pre-packed smem images, cp.async.bulk): an 80-column output chunk x one
 //               k pass (slabs {0,1,2} | {3,4}), 2-stage ring of 30 KB
-//   warp 3      L2 prefetch of the backward addends (MODE_BWD_LAST)
+//   warps 2, 3  no role (warpgroup 0 runs at a reduced register budget, step_fused_kernel.cuh)
 //   warps 4-11  two warpgroups, tile rows [0, 64) / [64, 128): wgmma m64n80k16, D (registers, fp32) = A (smem, bf16)
 //               . W_h^T (smem), chunk by chunk, then the epilogue from registers: + H_0 + bias -> tau -> bf16 -> HBM
+//               (the H_0 words of the next chunk are requested before each epilogue)
 //   warps 12-19 message: thread = row e': sums the sibling rows of e' (same destination atom) out of the
 //               shared-memory tile and writes the bf16 result row into the shared-memory A operand tile;
 //               optionally also to HBM (M_out / G_out, one 32-byte sector per thread) for the W_h gradient

@@ -29,6 +29,14 @@ constexpr int kWStages = 2;
 constexpr int kThreads = 640;
 constexpr int kSWarps = 8;          // message warps (12..19)
 constexpr int kMmaThreads = 256;    // two MMA + epilogue warpgroups (warps 4..7, 8..11)
+// Registers per thread of each role (setmaxnreg at the top of its branch).  640 threads at one CTA per SM are launched with
+// 96 each; the single-lane producer warps (warpgroup 0) and the message warps (warpgroups 3, 4) hand theirs to the MMA
+// warpgroups, whose epilogue holds the next chunk's operand words next to the accumulator (up to 125 registers; at 96 it
+// spills, DESIGN.md 4.1).  The budgets fill the launch's 640 x 96: kRegsProducer + 2 kRegsMsg + 2 kRegsMma = 5 x 96.
+constexpr int kRegsProducer = 32;
+constexpr int kRegsMsg = 88;
+constexpr int kRegsMma = 136;
+static_assert(kRegsProducer + 2 * kRegsMsg + 2 * kRegsMma <= 5 * 96, "register budgets exceed the launch's 640 x 96");
 constexpr int kMaxHp = 304;
 
 struct Params {
@@ -149,90 +157,121 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, Params p) {
   const int n_items = p.n_work_dev ? __ldg(p.n_work_dev) : p.n_tiles;   // work items of this launch (uniform over the grid)
   const int npass = (p.nslab + kWHalfSlabs - 1) / kWHalfSlabs;
 
-  if (warp == 0) {
-    // ===================== TMA producer: H_prev tile -> shared memory (single buffer) =====================
-    // No L2 prefetch of the next tile's rows (nor of its H_0 rows in warp 3): both made the step slower on an H100 at
-    // h = 300 (DESIGN.md 7).  The H_0 prefetch had no barrier to pace it, so it ran through all of a CTA's tiles at the
-    // start of the launch, far more rows than L2 holds.
-    int it = 0;
-    int row_carry = (int)blockIdx.x < n_items ? __ldg(p.tile_row_ptr + blockIdx.x) : 0;   // the next tile's first row, loaded a tile ahead
-    for (int t = blockIdx.x; t < n_items; t += gridDim.x, ++it) {
-      const int row0 = row_carry;
-      const int t2 = t + gridDim.x;
-      if (t2 < n_items) row_carry = __ldg(p.tile_row_ptr + t2);
-      // slab s of this tile is loaded as soon as the message warps have left slab s of the previous tile: the load
-      // of the leading slabs overlaps the gather of the trailing ones (one shared-memory tile, no exposed latency)
-      for (int s = 0; s < p.nslab; ++s) {
-        mbar_wait_trap(bar(B_AFREE + s), (it & 1) ^ 1);
-        if (elect_one()) {
-          if (s == 0) trace_ev(p, it, 0);
-          mbar_expect_tx(bar(B_AFULL + s), kSlabBytes);
-          tma_load_2d(sA + s * kSlabBytes, &tmapH, bar(B_AFULL + s), s * 64, row0);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== TMA producer: W_h stages (pre-packed smem images) =====================
-    // a stage = the W_h rows of one 80-column output chunk for k slabs {0,1,2} or {3,4} (contiguous in the image), in the
-    // MMA warpgroups' order: chunk by chunk, both k passes of a chunk back to back
-    uint32_t ws = 0;
-    for (int t = blockIdx.x; t < n_items; t += gridDim.x) {
-      for (int c = 0; c < p.nchunks; ++c)
-        for (int half = 0; half < npass; ++half, ++ws) {
-          const int s0 = half * kWHalfSlabs;
-          const int ns = min(kWHalfSlabs, p.nslab - s0);
-          const int nc = min(kChunkN, p.hp - c * kChunkN);
-          const uint8_t* src = p.Wpk + (size_t)c * kChunkN * p.nslab * 128 + (size_t)s0 * nc * 128;
-          const uint32_t bytes = (uint32_t)(ns * nc * 128);
-          const uint32_t st = ws % kWStages, use = ws / kWStages;
-          mbar_wait_trap(bar(B_WFREE + st), (use & 1) ^ 1);
+  if (warp < 4) {
+    setmaxnreg_dec<kRegsProducer>();
+    if (warp == 0) {
+      // ===================== TMA producer: H_prev tile -> shared memory (single buffer) =====================
+      // No L2 prefetch of the next tile's rows (nor of its H_0 rows): both made the step slower on an H100 at h = 300
+      // (DESIGN.md 7).  The H_0 prefetch had no barrier to pace it, so it ran through all of a CTA's tiles at the start of
+      // the launch, far more rows than L2 holds.  Warps 2 and 3 have no role: an L2 prefetch of MODE_BWD_LAST's addends there
+      // kept ptxas from giving the MMA warpgroups more than 96 registers (their epilogue spilled).
+      int it = 0;
+      int row_carry = (int)blockIdx.x < n_items ? __ldg(p.tile_row_ptr + blockIdx.x) : 0;   // the next tile's first row, loaded a tile ahead
+      for (int t = blockIdx.x; t < n_items; t += gridDim.x, ++it) {
+        const int row0 = row_carry;
+        const int t2 = t + gridDim.x;
+        if (t2 < n_items) row_carry = __ldg(p.tile_row_ptr + t2);
+        // slab s of this tile is loaded as soon as the message warps have left slab s of the previous tile: the load
+        // of the leading slabs overlaps the gather of the trailing ones (one shared-memory tile, no exposed latency)
+        for (int s = 0; s < p.nslab; ++s) {
+          mbar_wait_trap(bar(B_AFREE + s), (it & 1) ^ 1);
           if (elect_one()) {
-            if (p.exp_flags & 4096) {              // timing experiment: no W stream at all (stale shared memory, wrong results)
-              mbar_arrive(bar(B_WFULL + st));
-            } else {
-              mbar_expect_tx(bar(B_WFULL + st), bytes);
-              bulk_load(sW + st * kWStageBytes, src, bytes, bar(B_WFULL + st));
-            }
+            if (s == 0) trace_ev(p, it, 0);
+            mbar_expect_tx(bar(B_AFULL + s), kSlabBytes);
+            tma_load_2d(sA + s * kSlabBytes, &tmapH, bar(B_AFULL + s), s * 64, row0);
           }
           __syncwarp();
         }
-    }
-  } else if (warp == 3) {
-    // ===================== L2 prefetch of the backward addends (MODE_BWD_LAST) ==========
-    for (int t = blockIdx.x; MODE == MODE_BWD_LAST && t < n_items; t += gridDim.x) {
-      if (p.add0 != nullptr) {
-        // the epilogue of this tile reads the addend rows with plain loads: pull them into L2 now (the rows of a
-        // tile are one contiguous byte range).  Nothing paces this warp: it runs ahead of the epilogue by as many tiles
-        // as it gets to
-        const int row0 = __ldg(p.tile_row_ptr + t);
-        const int nr = __ldg(p.tile_row_ptr + t + 1) - row0;
-        const int64_t lines = ((int64_t)nr * p.ld * 2 + 127) >> 7;
-        const char* b0 = reinterpret_cast<const char*>(p.add0 + (int64_t)row0 * p.ld);
-        const char* b1 = p.add1 ? reinterpret_cast<const char*>(p.add1 + (int64_t)row0 * p.ld) : nullptr;
-        for (int64_t i = lane; i < lines; i += 32) {
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(b0 + (i << 7)));
-          if (b1) asm volatile("prefetch.global.L2 [%0];" ::"l"(b1 + (i << 7)));
-        }
+      }
+    } else if (warp == 1) {
+      // ===================== TMA producer: W_h stages (pre-packed smem images) =====================
+      // a stage = the W_h rows of one 80-column output chunk for k slabs {0,1,2} or {3,4} (contiguous in the image), in the
+      // MMA warpgroups' order: chunk by chunk, both k passes of a chunk back to back
+      uint32_t ws = 0;
+      for (int t = blockIdx.x; t < n_items; t += gridDim.x) {
+        for (int c = 0; c < p.nchunks; ++c)
+          for (int half = 0; half < npass; ++half, ++ws) {
+            const int s0 = half * kWHalfSlabs;
+            const int ns = min(kWHalfSlabs, p.nslab - s0);
+            const int nc = min(kChunkN, p.hp - c * kChunkN);
+            const uint8_t* src = p.Wpk + (size_t)c * kChunkN * p.nslab * 128 + (size_t)s0 * nc * 128;
+            const uint32_t bytes = (uint32_t)(ns * nc * 128);
+            const uint32_t st = ws % kWStages, use = ws / kWStages;
+            mbar_wait_trap(bar(B_WFREE + st), (use & 1) ^ 1);
+            if (elect_one()) {
+              if (p.exp_flags & 4096) {              // timing experiment: no W stream at all (stale shared memory, wrong results)
+                mbar_arrive(bar(B_WFULL + st));
+              } else {
+                mbar_expect_tx(bar(B_WFULL + st), bytes);
+                bulk_load(sW + st * kWStageBytes, src, bytes, bar(B_WFULL + st));
+              }
+            }
+            __syncwarp();
+          }
       }
     }
-  } else if (warp >= 4 && warp < 12) {
+  } else if (warp < 12) {
+    setmaxnreg_inc<kRegsMma>();
     // ===================== MMA + epilogue: warpgroup wg owns tile rows [64 wg, 64 wg + 64) ==========
     // D[64 x 80] (registers, fp32) = A (shared memory, written by the message warps) . W_h^T (W stage) per 80-column chunk;
     // the epilogue of a chunk runs from registers right after its last k pass.  The message warps build A row r as the
     // message of edge r itself (they gather through the tile-local rev() table), so accumulator row r is the update of
-    // edge r: it needs H_0 row r (global memory, requested before the chunk's last wgmma group is waited for) and produces output row r.
+    // edge r: it needs H_0 row r (global memory, requested one chunk ahead, below) and produces output row r.
     // W rows past a chunk's last column may hold the next slab's rows or stale data: they only reach accumulator columns
     // that the epilogue never stores.
     const int wg = (warp - 4) >> 2;
     const int tt = threadIdx.x - 128 - wg * 128;
     const int rA = wg * 64 + acc_row0(tt), cl = acc_col0(tt);
     const int nj = p.hp >> 4;
+    // ---- epilogue operands of one chunk.  The packed W_h image permutes the columns of every chunk (tc::acc_out_col): in each
+    // 32-column group G this thread's accumulator blocks 4 G .. 4 G + 3 hold the 8 contiguous output columns from
+    // acc_out_col(32 G + cl, nc) on, in a 16-column tail its blocks 4 G, 4 G + 1 hold 4 (acc_run_cols).  So each row and group
+    // is one 16-byte (tail: 8-byte) load, and hv[h][b] is the operand word of accumulator block b of row rA + 8 h.
+    constexpr int kGroups = (kChunkN + 31) / 32;   // two 32-column groups and a 16-column tail
+    auto load_ops = [&](uint32_t (&hv)[2][kChunkN / 8], int row0, int nrows, int c) {
+      const int nc = min(kChunkN, p.hp - c * kChunkN);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = rA + 8 * h;
+        const __nv_bfloat16* yrow = p.H0 + (int64_t)(row0 + r) * p.ld + c * kChunkN;
+#pragma unroll
+        for (int G = 0; G < kGroups; ++G) {
+          const int run = acc_run_cols(32 * G + cl, nc);
+          uint4 v = make_uint4(0u, 0u, 0u, 0u);
+          if (MODE != MODE_BWD_COPY && r < nrows) {
+            const __nv_bfloat16* src = yrow + acc_out_col(32 * G + cl, nc);
+            if (32 * G + 32 <= kChunkN && run == 8) {
+              v = __ldg(reinterpret_cast<const uint4*>(src));
+            } else if (run == 4) {
+              const uint2 u = __ldg(reinterpret_cast<const uint2*>(src));
+              v.x = u.x; v.y = u.y;
+            }
+          }
+          const uint32_t vw[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+          for (int w = 0; w < 4; ++w)
+            if (4 * G + w < kChunkN / 8) hv[h][4 * G + w] = vw[w];
+        }
+      }
+    };
+    // The operands are requested one chunk ahead: those of chunk c + 1 (at the last chunk: chunk 0 of this CTA's next work
+    // item) before chunk c's epilogue, so that their latency hides under a whole epilogue.  hwv holds the current chunk's.
+    uint32_t hwv[2][kChunkN / 8], hwn[2][kChunkN / 8];
+    int row0 = 0, nrows = 0;
+    if ((int)blockIdx.x < n_items) {
+      row0 = __ldg(p.tile_row_ptr + blockIdx.x);
+      nrows = __ldg(p.tile_row_ptr + blockIdx.x + 1) - row0;
+      load_ops(hwv, row0, nrows, 0);
+    }
     uint32_t ws = 0;
     int it = 0;
     for (int t = blockIdx.x; t < n_items; t += gridDim.x, ++it) {
-      const int row0 = __ldg(p.tile_row_ptr + t);
-      const int nrows = __ldg(p.tile_row_ptr + t + 1) - row0;
+      const int tn = t + gridDim.x;
+      int row0n = 0, nrowsn = 0;                                         // next work item (nrowsn = 0: none)
+      if (tn < n_items) {
+        row0n = __ldg(p.tile_row_ptr + tn);
+        nrowsn = __ldg(p.tile_row_ptr + tn + 1) - row0n;
+      }
       uint32_t a_waited = 0;                                             // k passes of this tile's A already waited for
       for (int c = 0; c < p.nchunks; ++c) {
         float acc[40];
@@ -281,36 +320,8 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, Params p) {
           }
           st_prev = st;
         }
-        // ---- epilogue operands: requested now, so that their L2 latency overlaps the last wgmma group.  The packed W_h image
-        // permutes the columns of every chunk (tc::acc_out_col): in each 32-column group G this thread's accumulator blocks
-        // 4 G .. 4 G + 3 hold the 8 contiguous output columns from acc_out_col(32 G + cl, nc) on, in a 16-column tail its
-        // blocks 4 G, 4 G + 1 hold 4 (acc_run_cols).  So each row and group is one 16-byte (tail: 8-byte) load and store, and
-        // hwv[h][b] is the operand word of accumulator block b, as before.
-        constexpr int kGroups = (kChunkN + 31) / 32;   // two 32-column groups and a 16-column tail
-        uint32_t hwv[2][kChunkN / 8];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = rA + 8 * h;
-          const __nv_bfloat16* yrow = p.H0 + (int64_t)(row0 + r) * p.ld + c * kChunkN;
-#pragma unroll
-          for (int G = 0; G < kGroups; ++G) {
-            const int run = acc_run_cols(32 * G + cl, nc);
-            uint4 v = make_uint4(0u, 0u, 0u, 0u);
-            if (MODE != MODE_BWD_COPY && r < nrows) {
-              const __nv_bfloat16* src = yrow + acc_out_col(32 * G + cl, nc);
-              if (32 * G + 32 <= kChunkN && run == 8) {
-                v = __ldg(reinterpret_cast<const uint4*>(src));
-              } else if (run == 4) {
-                const uint2 u = __ldg(reinterpret_cast<const uint2*>(src));
-                v.x = u.x; v.y = u.y;
-              }
-            }
-            const uint32_t vw[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int w = 0; w < 4; ++w)
-              if (4 * G + w < kChunkN / 8) hwv[h][4 * G + w] = vw[w];
-          }
-        }
+        if (c + 1 < p.nchunks) load_ops(hwn, row0, nrows, c + 1);
+        else load_ops(hwn, row0n, nrowsn, 0);
         wgmma_wait<0>();
         acc_fence(acc);
         release(st_prev, npass - 1);
@@ -354,7 +365,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, Params p) {
                                                          : act_grad_from_out(ACT, p.act_param, bf_hi(hw));
                   float z0 = v0 * g0, z1 = v1 * g1;
                   if (MODE == MODE_BWD_LAST && p.add0 != nullptr) {
-                    // dH_0 = (this step's masked gradient) + the earlier steps' dZ rows (L2 hits: prefetched by warp 3)
+                    // dH_0 = (this step's masked gradient) + the earlier steps' dZ rows
                     if ((w & 1) == 0) {
                       aw = __ldg(reinterpret_cast<const uint2*>(p.add0 + grow * p.ld + n));
                       bw = p.add1 != nullptr ? __ldg(reinterpret_cast<const uint2*>(p.add1 + grow * p.ld + n)) : make_uint2(0u, 0u);
@@ -390,10 +401,17 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, Params p) {
             }
           }
         }
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int b = 0; b < kChunkN / 8; ++b) hwv[h][b] = hwn[h][b];
       }
       if (tt == 0) trace_ev(p, it, 8 + wg);
+      row0 = row0n;
+      nrows = nrowsn;
     }
-  } else if (warp >= 12) {
+  } else {
+    setmaxnreg_dec<kRegsMsg>();
     // ===================== message (warps 12..19): thread == tile row ==================
     // A row e' of the GEMM is M[rev(e')] = sum of the OTHER in-edge states of e's destination atom
     // (mixins.py:11-18).  Each thread reads the <= 3 sibling rows of its row from the TMA-loaded,
