@@ -78,8 +78,8 @@ class GatherLinear(torch.autograd.Function):
         # a plain (ungathered, single-source) product -- the W_h GEMM of every depth step, 2 E h^2 flop -- runs f32-accurate on
         # the tensor cores (3xTF32, csrc/gemm_x3.cu) when its dimensions allow 16-byte rows; gathered / two-source operands
         # (W_i, W_o) stay on the f32 FMA kernel, which reads them in place
-        x3 = (idx1 is None and X2c is None and R > 0 and K1 % 4 == 0 and N % 4 == 0 and 0 < K1 <= 4096 and 0 < N <= 4096
-              and X1c.data_ptr() % 16 == 0 and (resc is None or resc.data_ptr() % 16 == 0)
+        x3 = (idx1 is None and X2c is None and R > 0 and K1 % 4 == 0 and N % 4 == 0 and 0 < K1 <= K.MAX_X3_DIM
+              and 0 < N <= K.MAX_X3_DIM and X1c.data_ptr() % 16 == 0 and (resc is None or resc.data_ptr() % 16 == 0)
               and K.X3_ENABLED and K._fused_available() and _X3_STATE["ok"] is not False)
         if x3 and _X3_STATE["ok"] is None and X1c.is_cuda and torch.cuda.is_current_stream_capturing():
             x3 = False                                  # the first-use check synchronises: not inside a graph capture

@@ -23,6 +23,11 @@ HOST_META = os.environ.get("DMPNN_HOST_META", "1") != "0"      # DMPNN_HOST_META
 
 HIDDEN_ALIGN = 64  # hidden row stride padded to 64 elements: bf16 rows start on 128-byte lines (one TMA request per box row)
 
+# Kernel limits (`plan` decides from them which path a message-passing call takes)
+MAX_TC_HIDDEN = 304   # d_h of the fused depth step and of the bf16 tensor-core linear kernels
+MAX_TC_K = 448        # inner dimension K of the bf16 tensor-core linear kernels
+MAX_X3_DIM = 4096     # every dimension of the 3xTF32 GEMMs
+
 # Optional device-side timing of the depth step (bench.py's roofline): when a list, every depth step
 # appends (tag, start_event, end_event) recorded on the launching stream.
 STEP_EVENTS: list | None = None
@@ -384,7 +389,7 @@ class MPConfig:
     undirected: bool
     hidden_dtype: torch.dtype  # torch.float32 (<=1e-5 tier) or torch.bfloat16 (<=1e-2 tier)
     fused: bool = True         # use the fused wgmma depth-step kernel when applicable
-    dropout_p: float = 0.0     # > 0: training-mode dropout on the fused bf16 / ReLU path (dropout_fused_ok)
+    dropout_p: float = 0.0     # > 0: training-mode dropout on the fused bf16 / ReLU path (Plan.dropout_ok)
     mask_fn: object = None     # keep-mask source `f(like) -> {0,1} tensor like `like``; None = torch's bernoulli_
 
 
@@ -393,19 +398,6 @@ def _hidden(rows: int, hp: int, dtype, dev) -> Tensor:
 
 
 UNDIRECTED_FUSED = os.environ.get("DMPNN_UNDIRECTED_FUSED", "1") != "0"   # DMPNN_UNDIRECTED_FUSED=0: A/B switch (message + GEMM launches)
-
-
-def _fused_step_ok(cfg: MPConfig, lay: Layout, h: int) -> bool:
-    """The fused wgmma depth step applies: bf16 tier, h <= 304.  Molecules of any size: those with more than 128 directed
-    edges run as 128-row windows of the same kernel (Layout.step_tables).  `undirected=True` (base.py:202-203) runs on it too:
-    the reverse-edge average is a prologue pass that produces the step's input (bond_forward)."""
-    ok = (cfg.fused and cfg.hidden_dtype == torch.bfloat16 and h <= 304 and lay.E > 0 and (not cfg.undirected or (UNDIRECTED_FUSED and h % 4 == 0))
-          and _fused_available())
-    if not ok and cfg.fused and cfg.hidden_dtype == torch.bfloat16 and lay.E > 0:
-        _warn_once("unfused", "chemprop_b200: this batch leaves the fused depth-step kernel (" +
-                   (f"d_h = {h} > 304" if h > 304 else "undirected=True with d_h % 4 != 0" if cfg.undirected else
-                    "kernel unavailable") + "): the depth loop runs as separate message + GEMM launches")
-    return ok
 
 
 _WARNED: set = set()
@@ -426,7 +418,7 @@ def _fused_available() -> bool:
     if "ok" not in _FUSED_STATE:
         lib = _lib.load()
         n = C.c_size_t(0)
-        _FUSED_STATE["ok"] = lib.dmpnn_pack_weight_bf16_bytes(304, 304, C.byref(n)) == 0
+        _FUSED_STATE["ok"] = lib.dmpnn_pack_weight_bf16_bytes(MAX_TC_HIDDEN, MAX_TC_HIDDEN, C.byref(n)) == 0
     return _FUSED_STATE["ok"]
 
 
@@ -518,13 +510,6 @@ def wgrad_tc_multi(dYs: list, X: Tensor, R: int, N: int, K: int, dW: Tensor, *, 
 
 # ---- fp32-accurate tensor-core GEMMs (3xTF32, csrc/gemm_x3.cu) -------------------------------------------------
 X3_ENABLED = os.environ.get("DMPNN_X3", "1") != "0"          # DMPNN_X3=0: A/B switch (fp32 tier on the SIMT f32 GEMMs)
-
-
-def _x3_ok(cfg: "MPConfig", *dims: int) -> bool:
-    """fp32 tier on the tensor cores: f32 hidden states, fused kernels enabled, every GEMM dimension a multiple of 4
-    (16-byte operand rows)."""
-    return (X3_ENABLED and cfg.fused and cfg.hidden_dtype == torch.float32 and all(d % 4 == 0 and 0 < d <= 4096 for d in dims)
-            and _fused_available())
 
 
 def pack_weight_x3(W: Tensor, transpose: bool = False) -> Tensor:
@@ -834,21 +819,6 @@ def bond_step_fused(H_prev: Tensor, H0: Tensor, H_next: Tensor, h: int, Wpk: Ten
     _lib.check(rc, "dmpnn_bond_step_fused_bf16")
 
 
-def h_is_mult4(Wh: Tensor) -> bool:
-    return Wh.shape[0] % 4 == 0
-
-
-def _tc_ok(cfg: MPConfig, h: int, *Ks: int) -> bool:
-    """Tensor-core linear kernels apply: bf16 tier, fused kernels enabled, sizes inside the kernel limits."""
-    ok = (cfg.fused and cfg.hidden_dtype == torch.bfloat16 and h <= 304 and all(k <= 448 for k in Ks)
-          and _fused_available())
-    if not ok and cfg.fused and cfg.hidden_dtype == torch.bfloat16 and _fused_available():
-        _warn_once("tc_limits", f"chemprop_b200: precision='bf16' with d_h = {h}, GEMM inner dimensions {tuple(Ks)}: outside the "
-                   "tensor-core kernels' limits (d_h <= 304, d_v + d_e and d_v + d_h <= 448); the linear layers run on the f32 "
-                   "FMA pipes with bf16 storage (the fp32 tier's 3xTF32 tensor-core GEMMs take d_h up to 4096)")
-    return ok
-
-
 def _empty_hidden(rows: int, hp: int, dtype, dev) -> Tensor:
     """Uninitialised hidden buffer: only for producers that write every column below pad16(h)."""
     return torch.empty((max(rows, 1), hp), dtype=dtype, device=dev)
@@ -868,14 +838,6 @@ def _dropout_(X: Tensor, cfg: MPConfig):
     keep = 1.0 - cfg.dropout_p
     M = cfg.mask_fn(X) if cfg.mask_fn is not None else torch.empty_like(X).bernoulli_(keep)
     scale_mask_(X, M, 1.0 / keep)
-
-
-def dropout_fused_ok(cfg: MPConfig, lay: Layout, h: int, d_v: int, d_e: int) -> bool:
-    """Training-mode dropout can stay on the fused bf16 path: ReLU (tau' of the post-dropout state is the keep mask times
-    tau' of the pre-dropout one, so no mask is stored and the scale 1 / (1 - p) folds into the packed weights of the
-    mirror), directed bonds, every GEMM on the tensor-core kernels and every depth step on the fused kernel."""
-    return (cfg.act == ACT_RELU and not cfg.undirected and lay.E > 0 and h % 4 == 0 and _tc_ok(cfg, h, d_v + d_e, d_v + h)
-            and (cfg.depth == 1 or _fused_step_ok(cfg, lay, h)))
 
 
 def bond_step_bwd_fused(dZ: Tensor, Yact: Tensor | None, dOut: Tensor, h: int, WpkT: Tensor, lay: Layout, act: int,
@@ -920,19 +882,6 @@ def atom_tables(lay: Layout):
     return lay._atom_work
 
 
-def _atom_fused_ok(cfg: MPConfig, lay: Layout, h: int, d_v: int, d_e: int) -> bool:
-    """The fused atom step applies: bf16 tier on the tensor-core kernels, directed, depth > 1, no training dropout, and every
-    molecule of the batch has <= 128 atoms (an atom tile is a run of whole molecules: max_tile_atoms of the layout exceeds
-    128 only for a single oversized molecule)."""
-    ok = (ATOM_FUSED_ENABLED and cfg.depth > 1 and not cfg.undirected and cfg.dropout_p == 0 and lay.V > 0 and lay.E > 0
-          and _atom_tc_ok(cfg, h, d_v, d_e) and lay.max_tile_atoms <= ATOM_TILE_ATOMS)
-    if not ok and ATOM_FUSED_ENABLED and cfg.depth > 1 and lay.E > 0 and _atom_tc_ok(cfg, h, d_v, d_e):
-        _warn_once("atom_unfused", "chemprop_b200: this batch leaves the fused atom depth step (" +
-                   ("undirected=True" if cfg.undirected else "training dropout" if cfg.dropout_p > 0 else
-                    "a molecule with more than 128 atoms") + "): neighbour sum and GEMM run as separate launches")
-    return ok
-
-
 def atom_step_fused(H_prev: Tensor, H0: Tensor, H_next: Tensor, h: int, Wpk: Tensor, bias: Tensor | None, lay: Layout,
                     act: int, act_param: float, first_step: bool, N_out: Tensor | None = None):
     """H_next[v] = act(H0[v] + bias + W . sum_{e in in(v)} g(H_prev[src(e)])) in one launch (dmpnn_atom_step_fused_bf16)."""
@@ -964,7 +913,7 @@ def _readout_pad(d_v: int, h: int) -> int:
     for the vectorised segment sum that writes M_v in place; d_v = 106 of the reaction graphs left it on the scalar kernel:
     1.2 ms per step at C4), unless that would exceed the GEMM's K limit."""
     dvp = (d_v + 7) // 8 * 8
-    return dvp if dvp + h <= 448 else d_v
+    return dvp if dvp + h <= MAX_TC_K else d_v
 
 
 def _wo_padded(Wo: Tensor, d_v: int, dvp: int) -> Tensor:
@@ -991,7 +940,7 @@ def _readout_operand(lay: Layout, V: Tensor, Hprev: Tensor, first: bool, h: int,
     concat_bf16(V, V.shape[1], XO, lay.V, width=dvp)
     segment_sum(Hprev, lay.rowptr, lay.V, h, XO[:, dvp:dvp + h], idx=idx, act=(cfg.act if first else ACT_NONE),
                 act_param=cfg.act_param, pad_to=hc)
-    ones_col = dvp + hc if ones and dvp + hc + 1 <= 448 else None
+    ones_col = dvp + hc if ones and dvp + hc + 1 <= MAX_TC_K else None
     if ones_col is not None:
         XO[:, ones_col].fill_(1.0)
     return XO, ones_col
@@ -1015,11 +964,93 @@ def _readout_grads(dY: Tensor, saved: dict, nV: int, h: int, d_v: int, bias: boo
     return dWo, dbo
 
 
+TC, X3, SIMT = "tc", "x3", "simt"     # GEMM families: bf16 tensor cores, 3xTF32 tensor cores, f32 FMA pipes
+
+
+@dataclass(frozen=True)
+class Plan:
+    """How one message-passing call runs (see `plan`)."""
+    gemm: str | None           # TC, X3 or SIMT
+    fused: bool                # the depth loop runs on the fused step
+    forward: object            # (lay, V, E, W_i, b_i, W_h, b_h, W_o, b_o, cfg, plan, ...) -> (H_v, saved)
+    mirror: object             # (lay, V, E, W_i, W_h, W_o, cfg, plan, saved, gH_v, need_bias, ...) -> six gradients
+    dropout_ok: bool = False   # training-mode dropout can stay on this path (bond kinds)
+    reason: str | None = None  # mol-atom-bond kinds: why the bf16 path does not apply (None: it does)
+
+
+def plan(kind: str, cfg: MPConfig, lay: Layout | None, h: int, d_v: int, d_e: int) -> Plan:
+    """The execution path of one message-passing call.  `kind`: "bond" / "atom" (Bond / AtomMPFunction and the export op's
+    bonds), "mab_bond" / "mab_atom" (MABMPFunction), "export_atom" (the export op's atoms: never on the fused atom step).
+    The only place that knows the kernels' limits, and the only one that warns, once per process and reason, when a bf16
+    call leaves a fast path.  `lay` None (mol-atom-bond kinds): only `reason` is filled in, the eligibility of a module
+    before it sees a batch."""
+    reason = None
+    if kind in ("mab_bond", "mab_atom"):
+        Ks = (d_v + d_e, d_v + h, d_e + h) if kind == "mab_bond" else (d_v, h + d_e, d_v + h, d_e + h)   # + W_eo's K
+        reason = (f"d_h = {h} > {MAX_TC_HIDDEN}" if h > MAX_TC_HIDDEN else f"d_h = {h} not a multiple of 4" if h % 4 != 0 else
+                  "d_e = 0" if d_e == 0 else f"GEMM inner dimensions {Ks} above {MAX_TC_K}" if max(Ks) > MAX_TC_K else
+                  "tensor-core kernels unavailable" if not _fused_available() else None)
+        if lay is None:
+            return Plan(None, False, None, None, reason=reason)
+    bond = kind in ("bond", "mab_bond")
+    bf16 = cfg.fused and cfg.hidden_dtype == torch.bfloat16
+    Ks = (d_v + d_e, d_v + h) if bond else (d_v, h + d_e, d_v + h)
+    tc = bf16 and h <= MAX_TC_HIDDEN and max(Ks) <= MAX_TC_K and _fused_available()
+    # Training-mode dropout stays on the fused bf16 path (dropout_ok) for ReLU on directed bonds -- tau' of the post-dropout
+    # state is the keep mask times tau' of the pre-dropout one, so no mask is stored and 1 / (1 - p) folds into the mirror's
+    # packed weights -- with every GEMM on the tensor cores and every depth step fused.  Of a bond call with dropout only the
+    # GEMM limits are warned about, and only when they alone keep it off that path (it then runs on the composed tier).
+    drop_shape = cfg.act == ACT_RELU and not cfg.undirected and lay.E > 0 and h % 4 == 0
+    if not tc and bf16 and not (bond and cfg.dropout_p > 0 and not drop_shape) and _fused_available():
+        _warn_once("tc_limits", f"chemprop_b200: precision='bf16' with d_h = {h}, GEMM inner dimensions {Ks}: outside the "
+                   f"tensor-core kernels' limits (d_h <= {MAX_TC_HIDDEN}, d_v + d_e and d_v + d_h <= {MAX_TC_K}); the linear "
+                   "layers run on the f32 FMA pipes with bf16 storage (the fp32 tier's 3xTF32 tensor-core GEMMs take d_h up "
+                   f"to {MAX_X3_DIM})")
+    if bond:
+        # fp32 tier on the tensor cores: every GEMM dimension a multiple of 4 (16-byte operand rows), atoms to run on
+        x3 = (X3_ENABLED and cfg.fused and cfg.hidden_dtype == torch.float32 and lay.V > 0
+              and all(d % 4 == 0 and 0 < d <= MAX_X3_DIM for d in (h, d_v + h)) and _fused_available())
+        # the fused depth step: molecules of any size (those with more than 128 directed edges run as 128-row windows,
+        # Layout.step_tables); undirected bonds too, the reverse-edge average being a prologue pass (bond_forward)
+        step = (bf16 and h <= MAX_TC_HIDDEN and lay.E > 0 and (not cfg.undirected or (UNDIRECTED_FUSED and h % 4 == 0))
+                and _fused_available())
+        if cfg.depth > 1 and not step and bf16 and lay.E > 0 and cfg.dropout_p == 0:
+            why = (f"d_h = {h} > {MAX_TC_HIDDEN}" if h > MAX_TC_HIDDEN else
+                   "undirected=True with d_h % 4 != 0" if cfg.undirected else "kernel unavailable")
+            _warn_once("unfused", f"chemprop_b200: this batch leaves the fused depth-step kernel ({why}): the depth loop runs "
+                       "as separate message + GEMM launches")
+        fused = cfg.depth > 1 and step
+        # the tensor-core mirror needs the fused forward's saved M^1 and X_0: directed, edges, d_h % 4 == 0; otherwise the
+        # generic mirror (which recomputes the M^t the fused forward did not keep)
+        tc_mirror = kind == "mab_bond" or (tc and not cfg.undirected and lay.E > 0 and h % 4 == 0)
+        return Plan(TC if tc else X3 if x3 else SIMT, fused, bond_forward, bond_backward_tc if tc_mirror else bond_backward,
+                    dropout_ok=drop_shape and tc and (cfg.depth == 1 or fused), reason=reason)
+    # atoms: the tensor-core path needs d_h % 4 == 0 and atoms to run on; a mol-atom-bond call is on it by `reason`
+    atom_tc = tc and h % 4 == 0
+    on_tc = kind == "mab_atom" or (atom_tc and lay.V > 0)
+    fused = False
+    if on_tc and kind != "export_atom":
+        # the fused atom step: directed, depth > 1, no training dropout, and every molecule within one atom tile (a tile is a
+        # run of whole molecules: max_tile_atoms exceeds the tile only for a single oversized molecule)
+        fused = (ATOM_FUSED_ENABLED and cfg.depth > 1 and not cfg.undirected and cfg.dropout_p == 0 and lay.V > 0 and lay.E > 0
+                 and atom_tc and lay.max_tile_atoms <= ATOM_TILE_ATOMS)
+        if not fused and ATOM_FUSED_ENABLED and cfg.depth > 1 and lay.E > 0 and atom_tc:
+            why = ("undirected=True" if cfg.undirected else "training dropout" if cfg.dropout_p > 0 else
+                   f"a molecule with more than {ATOM_TILE_ATOMS} atoms")
+            _warn_once("atom_unfused", f"chemprop_b200: this batch leaves the fused atom depth step ({why}): neighbour sum and "
+                       "GEMM run as separate launches")
+    if fused:
+        return Plan(TC, True, atom_forward_fused, atom_backward_fused, reason=reason)
+    if on_tc:
+        return Plan(TC, False, atom_forward_tc, atom_backward_tc, reason=reason)
+    return Plan(SIMT, False, atom_forward, atom_backward, reason=reason)
+
+
 def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor | None, bo,
-                 cfg: MPConfig, for_backward: bool = False, readout_f32: bool = False):
+                 cfg: MPConfig, path: Plan, for_backward: bool = False, readout_f32: bool = False):
     """BondMessagePassing.forward up to W_o (chemprop/nn/message_passing/base.py:196-212 with
-    mixins.py:8-18 and base.py:135-141, 180-182).  Returns (H_v, saved-for-backward).  `Wo` None: the depth loop only
-    (H_v None); `readout_f32` (tensor-core path): the W_o epilogue stores H_v in f32."""
+    mixins.py:8-18 and base.py:135-141, 180-182) on `path`.  Returns (H_v, saved-for-backward).  `Wo` None: the
+    depth loop only (H_v None); `readout_f32` (tensor-core path): the W_o epilogue stores H_v in f32."""
     dev = V.device
     h = Wh.shape[0]
     hp = pad_hidden(h)
@@ -1027,7 +1058,7 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
     T = cfg.hidden_dtype
     nE, nV = lay.E, lay.V
     a, ap = cfg.act, cfg.act_param
-    tc = _tc_ok(cfg, h, d_v + d_e, d_v + h)
+    tc, x3 = path.gemm == TC, path.gemm == X3
     X0 = X0f = None
     # H_0 = W_i([V[src] || E])   (mixins.py:8-9); rows in dst-sorted order
     if tc and nE > 0:
@@ -1036,7 +1067,7 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
         concat_bf16(V, d_v, X0, nE, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm)
         H0 = _empty_hidden(nE, hp, T, dev)
         linear_tc(X0, d_v + d_e, pack_weight_tc(Wi), h, H0, bias=bi, R=nE)
-    elif _x3_ok(cfg, h, d_v + h) and nE > 0:
+    elif x3 and nE > 0:
         # fp32 tier on the tensor cores: [V[src] || E] materialised once in f32 (zero-padded to a multiple of 4 columns),
         # W_i as a 3xTF32 GEMM; the same operand serves the W_i gradient
         kx4 = (d_v + d_e + 3) // 4 * 4
@@ -1049,9 +1080,9 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
         linear_fwd(V, d_v, Wi, H0, h, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm, bias=bi, R=nE, pad_to=hp)
     Hs, Ms, Hbars = [], [], []
     Hprev, first = H0, True  # H^0 = tau(H_0) is applied on load (base.py:200)
-    use_fused = cfg.depth > 1 and _fused_step_ok(cfg, lay, h)
+    use_fused = path.fused
     Wpk = pack_weight_bf16(Wh) if use_fused else None
-    x3 = _x3_ok(cfg, h, d_v + h)          # fp32 tier: W_h / W_o GEMMs as 3xTF32 on the tensor cores (f32-accurate)
+    # fp32 tier with x3: W_h / W_o GEMMs as 3xTF32 on the tensor cores (f32-accurate)
     Wh_x3 = pack_weight_x3(Wh) if (x3 and cfg.depth > 1 and nE > 0) else None
     # bf16 tier off the fused kernel (undirected=True): the W_h GEMM still runs on the tensor cores (k_linear_tc, H_0 residual,
     # bias and tau in its epilogue -- the form AtomMessagePassing's unfused step uses), not on the f32 FMA pipes
@@ -1080,7 +1111,7 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             Ms.append(M1)
         else:
             if cfg.dropout_p > 0:
-                raise DmpnnError("dropout on the monolithic tier needs the fused depth step (see dropout_fused_ok)")
+                raise DmpnnError("dropout on the monolithic tier needs the fused depth step (see Plan.dropout_ok)")
             src_in, fa = Hprev, (a if first else ACT_NONE)
             if cfg.undirected:  # H = (H + H[rev]) / 2   (base.py:202-203)
                 Hbar = _hidden(nE, hp, T, dev)
@@ -1116,8 +1147,8 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             Hv = Hvp[:nV, :h]
     elif Wo is not None:
         if cfg.dropout_p > 0:
-            raise DmpnnError("dropout on the monolithic tier needs the tensor-core path (see dropout_fused_ok)")
-        if x3 and nV > 0:
+            raise DmpnnError("dropout on the monolithic tier needs the tensor-core path (see Plan.dropout_ok)")
+        if x3:
             # [V || M_v] assembled once in f32 (torch.cat of base.py:180): V copied in, M_v written in place by the segment sum
             XO = torch.empty((nV, d_v + h), dtype=T, device=dev)
             XO[:, :d_v].copy_(V)
@@ -1132,14 +1163,13 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             # H_v = tau(W_o([V || M_v]))   (base.py:180-182)
             Hv = torch.empty((nV, h), dtype=T, device=dev)
             linear_fwd(V, d_v, Wo, Hv, h, X2=Mv, K2=h, bias=bo, act=a, act_param=ap, R=nV, pad_to=h)
-    saved = dict(H0=H0, Hs=Hs, Ms=Ms, Hbars=Hbars, Mv=Mv, Hv=Hv, X0=X0, XO=XO, tc=tc, x3=x3, X0f=X0f, dvp=d_v,
-                 ones_col=ones_col)
+    saved = dict(H0=H0, Hs=Hs, Ms=Ms, Hbars=Hbars, Mv=Mv, Hv=Hv, X0=X0, XO=XO, X0f=X0f, dvp=d_v, ones_col=ones_col)
     return Hv, saved
 
 
-def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
+def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig, path: Plan,
                   saved: dict, gHv: Tensor, need_bias: tuple[bool, bool, bool]):
-    """Hand-written autograd mirror (SURVEY.md 8a-7) of bond_forward.  Returns
+    """Hand-written autograd mirror (SURVEY.md 8a-7) of bond_forward on `path`.  Returns
     (dWi, dbi, dWh, dbh, dWo, dbo)."""
     dev = V.device
     h = Wh.shape[0]
@@ -1156,8 +1186,7 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
     dbi = torch.zeros(h, **f32) if need_bias[0] else None
     dbh = torch.zeros(h, **f32) if need_bias[1] else None
     dbo = torch.zeros(h, **f32) if need_bias[2] else None
-    tc = bool(saved.get("tc"))
-    x3 = bool(saved.get("x3")) and saved.get("XO") is not None
+    tc, x3 = path.gemm == TC, path.gemm == X3
     if gHv.stride(1) != 1:
         gHv = gHv.contiguous()
     # readout: dY = g * tau'(Y); dW_o = dY^T [V || M_v]; dM_v = dY . W_o[:, d_v:]
@@ -1195,7 +1224,7 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
             dZ = _hidden(nE, hp, T, dev)
             act_bwd(dMv, Hs[-1], nE, h, act=a, act_param=ap, gidx=lay.dst_row, dZ=dZ, acc=dH0)
             # undirected steps that ran on the fused kernel (they saved no M^t): their mirror on the fused kernel too
-            fused_undirected = cfg.undirected and tc and Ms[0] is None
+            fused_undirected = cfg.undirected and tc and path.fused
             WhT_f = pack_weight_bf16(Wh.t().contiguous()) if fused_undirected else None
             for t in range(cfg.depth - 1, 0, -1):
                 # inputs of step t: Hin = H^{t-1} (or tau(H_0) when t == 1)
@@ -1250,13 +1279,13 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
                 else:
                     dZ = _hidden(nE, hp, T, dev)
                     act_bwd(dHin, Hin, nE, h, act=a, act_param=ap, dZ=dZ, acc=dH0)
-        if tc and saved.get("X0") is not None:
+        if tc:
             dH0b = torch.empty((nE, hp), dtype=T, device=dev)
             concat_bf16(dH0, h, dH0b, nE)                      # f32 accumulator -> bf16 operand
             wgrad_tc(dH0b, saved["X0"], nE, h, d_v + d_e, dWi)
             if dbi is not None:
                 column_sum(dH0, nE, h, dbi)
-        elif x3 and saved.get("X0f") is not None:
+        elif x3:
             X0f = saved["X0f"]
             dWi4 = torch.empty((h, X0f.shape[1]), dtype=torch.float32, device=dev)
             wgrad_x3(dH0, X0f, nE, h, X0f.shape[1], dWi4)
@@ -1268,7 +1297,7 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
     return dWi, dbi, dWh, dbh, dWo, dbo
 
 
-def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
+def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig, path: Plan,
                      saved: dict, gHv: Tensor | None, need_bias: tuple[bool, bool, bool], entry=None):
     """bf16-tier autograd mirror of bond_forward on the fused depth step (directed bonds).  Differences from the generic
     mirror: every GEMM is on the tensor cores (wgmma); each depth step's mirror is one launch of the fused kernel (_fused_mirror);
@@ -1295,7 +1324,7 @@ def bond_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
     dWo = dbo = None
     dbi = torch.zeros(h, **f32) if need_bias[0] else None
     dbh = torch.zeros(h, **f32) if need_bias[1] else None
-    # Training-mode dropout (cfg.dropout_p > 0; ReLU only, dropout_fused_ok): a gradient that crosses a dropout site is
+    # Training-mode dropout (cfg.dropout_p > 0; ReLU only, Plan.dropout_ok): a gradient that crosses a dropout site is
     # multiplied by the keep mask and by s = 1 / (1 - p).  With ReLU the mask is already in tau' of the stored POST-dropout
     # state ([H_post > 0] = mask * [H_pre > 0]), and s, a scalar, folds into the packed weight of the GEMM that produces
     # the gradient arriving at the site (or, for W_o's own gradient, into the result).
@@ -1389,48 +1418,54 @@ def _refuse_feature_grads(ctx):
             "(d/dV, d/dE are not implemented); detach the features, or use the reference module for input attribution")
 
 
+def _mp_inputs(ctx, V: Tensor, E: Tensor, params: tuple) -> tuple:
+    """Start of every message-passing Function's forward: CUDA tensors only, no feature gradients, and the features and the
+    (weight, bias) pairs of `params` (None stays None) as f32 contiguous tensors detached from autograd.  Records on `ctx`
+    which biases are present and the dtype of each parameter's gradient (its weight's)."""
+    _require_cuda(V, E, *params[0::2])
+    _refuse_feature_grads(ctx)
+    ctx.has_bias = tuple(b is not None for b in params[1::2])
+    ctx.gdtypes = tuple(None if w is None else w.dtype for w in params[0::2] for _ in range(2))
+    f32 = lambda t: None if t is None else t.detach().contiguous().float()  # noqa: E731
+    return V.contiguous().float(), E.contiguous().float(), [f32(t) for t in params]
+
+
+def _mp_save(ctx, lay: Layout, cfg: MPConfig, path: Plan, V: Tensor, E: Tensor, W: tuple, saved: dict, Hv: Tensor | None):
+    """What the mirror needs.  `Hv` is the tensor autograd turns into this node's output: keeping THAT object in ctx.saved
+    would be a reference cycle (node -> saved -> Hv -> grad_fn = node) and the step's activations would live until Python's
+    cyclic GC runs (GBs per step, cudaMalloc on every step); a detached alias shares the storage without the back edge."""
+    saved["Hv"] = None if Hv is None else Hv.detach()
+    ctx.lay, ctx.cfg, ctx.plan, ctx.saved, ctx.VE, ctx.W = lay, cfg, path, saved, (V, E), W
+
+
+def _mp_grads(ctx, grads: tuple, n_after: int) -> tuple:
+    """backward's return: None for V and E, the parameter gradients in their weights' dtypes, None for the `n_after`
+    non-tensor inputs.  ctx.saved stays until autograd frees the node: a second backward (retain_graph=True) works like
+    torch's own."""
+    cast = tuple(None if (g is None or d is None) else g.to(d) for g, d in zip(grads, ctx.gdtypes))
+    return (None, None) + cast + (None,) * n_after
+
+
 class BondMPFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, V, E, Wi, bi, Wh, bh, Wo, bo, lay, cfg):
-        _require_cuda(V, E, Wi, Wh, Wo)
-        _refuse_feature_grads(ctx)
-        V = V.contiguous().float()
-        E = E.contiguous().float()
-        Wi_, Wh_, Wo_ = Wi.detach().contiguous().float(), Wh.detach().contiguous().float(), Wo.detach().contiguous().float()
-        bi_ = None if bi is None else bi.detach().contiguous().float()
-        bh_ = None if bh is None else bh.detach().contiguous().float()
-        bo_ = None if bo is None else bo.detach().contiguous().float()
-        Hv, saved = bond_forward(lay, V, E, Wi_, bi_, Wh_, bh_, Wo_, bo_, cfg, for_backward=any(ctx.needs_input_grad))
-        # `Hv` is the tensor autograd turns into this node's output: keeping THAT object in ctx.saved would be a reference
-        # cycle (node -> saved -> Hv -> grad_fn = node) and the step's activations would live until Python's cyclic GC
-        # runs (GBs per step, cudaMalloc on every step); a detached alias shares the storage without the back edge
-        saved["Hv"] = Hv.detach()
-        ctx.lay, ctx.cfg, ctx.saved = lay, cfg, saved
-        ctx.VE = (V, E)
-        ctx.W = (Wi_, Wh_, Wo_)
-        ctx.has_bias = (bi is not None, bh is not None, bo is not None)
-        ctx.wdtypes = (Wi.dtype, Wh.dtype, Wo.dtype)
+        V, E, (Wi, bi, Wh, bh, Wo, bo) = _mp_inputs(ctx, V, E, (Wi, bi, Wh, bh, Wo, bo))
+        p = plan("bond", cfg, lay, Wh.shape[0], V.shape[1], E.shape[1])
+        Hv, saved = p.forward(lay, V, E, Wi, bi, Wh, bh, Wo, bo, cfg, p, for_backward=any(ctx.needs_input_grad))
+        _mp_save(ctx, lay, cfg, p, V, E, (Wi, Wh, Wo), saved, Hv)
         return Hv
 
     @staticmethod
     def backward(ctx, gHv):
-        V, E = ctx.VE
-        Wi, Wh, Wo = ctx.W
-        bwd = bond_backward_tc if (ctx.saved.get("tc") and not ctx.cfg.undirected and ctx.saved.get("X0") is not None
-                                   and h_is_mult4(Wh)) else bond_backward
-        dWi, dbi, dWh, dbh, dWo, dbo = bwd(ctx.lay, V, E, Wi, Wh, Wo, ctx.cfg, ctx.saved, gHv, ctx.has_bias)
-        # ctx.saved stays until autograd frees the node: a second backward (retain_graph=True) works like torch's own
-        d0, d1, d2 = ctx.wdtypes
-        cast = lambda g, d: None if g is None else g.to(d)
-        return (None, None, cast(dWi, d0), cast(dbi, d0), cast(dWh, d1), cast(dbh, d1), cast(dWo, d2),
-                cast(dbo, d2), None, None)
+        grads = ctx.plan.mirror(ctx.lay, *ctx.VE, *ctx.W, ctx.cfg, ctx.plan, ctx.saved, gHv, ctx.has_bias)
+        return _mp_grads(ctx, grads, 2)
 
 
 # ----------------------------------------------------------------------------------------------
 # atom message passing (atom-granular: every edge row depends only on its source atom)
 # ----------------------------------------------------------------------------------------------
 def atom_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor, bo,
-                 cfg: MPConfig):
+                 cfg: MPConfig, path: Plan):
     """AtomMessagePassing.forward up to W_o (base.py:196-212 with mixins.py:22-30), restated on atoms:
     the reference's H[e] equals Ha[src(e)], so M[e] = [sum_{u in N(src e)} Ha[u] || sum_in E]."""
     dev = V.device
@@ -1465,7 +1500,7 @@ def atom_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
     return Hv, dict(H0=H0, Hs=Hs, Ns=Ns, SE=SE, Mv=Mv, Hv=Hv)
 
 
-def atom_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
+def atom_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig, path: Plan,
                   saved: dict, gHv: Tensor, need_bias):
     dev = V.device
     h = Wi.shape[0]
@@ -1508,10 +1543,6 @@ def atom_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
     return dWi, dbi, dWh, dbh, dWo, dbo
 
 
-def _atom_tc_ok(cfg: MPConfig, h: int, d_v: int, d_e: int) -> bool:
-    return _tc_ok(cfg, h, d_v, h + d_e, d_v + h) and h % 4 == 0
-
-
 def _atom_readout_tc(lay: Layout, V: Tensor, Hprev: Tensor, first: bool, h: int, Wo: Tensor, bo, cfg: MPConfig, rows: int,
                      with_ones: bool, readout_f32: bool):
     """H_v = tau(W_o([V || M_v])) of the atom tiers (base.py:180-182, 208-211): returns (H_v, XO, dvp, ones_col).  `with_ones`:
@@ -1533,7 +1564,7 @@ def _atom_readout_tc(lay: Layout, V: Tensor, Hprev: Tensor, first: bool, h: int,
 
 
 def atom_forward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor, bo, cfg: MPConfig,
-                    readout_f32: bool = False):
+                    path: Plan, readout_f32: bool = False):
     """bf16 tier of atom_forward on the tensor cores: every GEMM is dmpnn_linear_tc_bf16 (the H_0 residual of
     base.py:138 is added in its epilogue), the neighbour sums write straight into the GEMM's A operand.  `Wo` None: no
     read-out; `readout_f32`: H_v stored in f32."""
@@ -1574,10 +1605,10 @@ def atom_forward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tenso
     Hv = XO = dvp = None
     if Wo is not None:
         Hv, XO, dvp, _ = _atom_readout_tc(lay, V, Hprev, first, h, Wo, bo, cfg, rows, False, readout_f32)
-    return Hv, dict(H0=H0, Hs=Hs, XAs=XAs, XO=XO, Xv=Xv, Hv=Hv, tc=True, dvp=dvp, ones_col=None)
+    return Hv, dict(H0=H0, Hs=Hs, XAs=XAs, XO=XO, Xv=Xv, Hv=Hv, dvp=dvp, ones_col=None)
 
 
-def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
+def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig, path: Plan,
                      saved: dict, gHv: Tensor | None, need_bias, entry=None):
     """Autograd mirror of atom_forward_tc (wgmma GEMMs; dH_0 is kept as separate terms, one W_i GEMM each).  `gHv` None:
     no read-out.  `entry(dHa, Y, from_preact, out)` (the mol-atom-bond edge head) replaces the first tau' pass
@@ -1642,7 +1673,7 @@ def atom_backward_tc(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, 
 
 
 def atom_forward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, bh, Wo: Tensor, bo, cfg: MPConfig,
-                       readout_f32: bool = False):
+                       path: Plan, readout_f32: bool = False):
     """bf16 tier of atom_forward with ONE launch per depth step (dmpnn_atom_step_fused_bf16).  The reference's update
     (base.py:135-141) on atoms is tau(H_0 + b_h + W_h . [N^t || SE]) with N^t the neighbour sum of the previous state and SE the
     loop-invariant sum of the incoming bond features: W_h[:, h:] . SE + b_h is added to H_0 ONCE (a K = d_e GEMM with H_0 as
@@ -1688,10 +1719,10 @@ def atom_forward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Te
     Hv = XO = dvp = ones_col = None
     if Wo is not None:          # db_o rides on dW_o's GEMM (ones column)
         Hv, XO, dvp, ones_col = _atom_readout_tc(lay, V, Hprev, first, h, Wo, bo, cfg, rows, True, readout_f32)
-    return Hv, dict(H0=H0, Hs=Hs, N1=N1, SEb=SEb, XO=XO, Xv=Xv, Hv=Hv, tc=True, fused=True, dvp=dvp, ones_col=ones_col)
+    return Hv, dict(H0=H0, Hs=Hs, N1=N1, SEb=SEb, XO=XO, Xv=Xv, Hv=Hv, dvp=dvp, ones_col=ones_col)
 
 
-def atom_backward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig,
+def atom_backward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo: Tensor, cfg: MPConfig, path: Plan,
                         saved: dict, gHv: Tensor | None, need_bias, entry=None):
     """Autograd mirror of atom_forward_fused.  With A the (symmetric) atom adjacency, N^t = A H^{t-1}:
     dH^{t-1} = ((A dZ^t) . W_h[:, :h]) * tau'(H^{t-1}) -- the mirror mode of the fused kernel, whose gathered operand
@@ -1760,63 +1791,22 @@ def atom_backward_fused(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tenso
 class AtomMPFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, V, E, Wi, bi, Wh, bh, Wo, bo, lay, cfg):
-        _require_cuda(V, E, Wi, Wh, Wo)
-        _refuse_feature_grads(ctx)
-        V = V.contiguous().float()
-        E = E.contiguous().float()
-        Wi_, Wh_, Wo_ = Wi.detach().contiguous().float(), Wh.detach().contiguous().float(), Wo.detach().contiguous().float()
-        bi_ = None if bi is None else bi.detach().contiguous().float()
-        bh_ = None if bh is None else bh.detach().contiguous().float()
-        bo_ = None if bo is None else bo.detach().contiguous().float()
-        fwd = atom_forward_tc if (_atom_tc_ok(cfg, Wi_.shape[0], V.shape[1], E.shape[1]) and lay.V > 0) else atom_forward
-        if fwd is atom_forward_tc and _atom_fused_ok(cfg, lay, Wi_.shape[0], V.shape[1], E.shape[1]):
-            fwd = atom_forward_fused
-        Hv, saved = fwd(lay, V, E, Wi_, bi_, Wh_, bh_, Wo_, bo_, cfg)
-        # `Hv` is the tensor autograd turns into this node's output: keeping THAT object in ctx.saved would be a reference
-        # cycle (node -> saved -> Hv -> grad_fn = node) and the step's activations would live until Python's cyclic GC
-        # runs (GBs per step, cudaMalloc on every step); a detached alias shares the storage without the back edge
-        saved["Hv"] = Hv.detach()
-        ctx.lay, ctx.cfg, ctx.saved = lay, cfg, saved
-        ctx.VE = (V, E)
-        ctx.W = (Wi_, Wh_, Wo_)
-        ctx.has_bias = (bi is not None, bh is not None, bo is not None)
-        ctx.wdtypes = (Wi.dtype, Wh.dtype, Wo.dtype)
+        V, E, (Wi, bi, Wh, bh, Wo, bo) = _mp_inputs(ctx, V, E, (Wi, bi, Wh, bh, Wo, bo))
+        p = plan("atom", cfg, lay, Wi.shape[0], V.shape[1], E.shape[1])
+        Hv, saved = p.forward(lay, V, E, Wi, bi, Wh, bh, Wo, bo, cfg, p)
+        _mp_save(ctx, lay, cfg, p, V, E, (Wi, Wh, Wo), saved, Hv)
         return Hv
 
     @staticmethod
     def backward(ctx, gHv):
-        V, E = ctx.VE
-        Wi, Wh, Wo = ctx.W
-        bwd = atom_backward_fused if ctx.saved.get("fused") else atom_backward_tc if ctx.saved.get("tc") else atom_backward
-        dWi, dbi, dWh, dbh, dWo, dbo = bwd(ctx.lay, V, E, Wi, Wh, Wo, ctx.cfg, ctx.saved, gHv, ctx.has_bias)
-        # ctx.saved stays until autograd frees the node: a second backward (retain_graph=True) works like torch's own
-        d0, d1, d2 = ctx.wdtypes
-        cast = lambda g, d: None if g is None else g.to(d)
-        return (None, None, cast(dWi, d0), cast(dbi, d0), cast(dWh, d1), cast(dbh, d1), cast(dWo, d2),
-                cast(dbo, d2), None, None)
+        grads = ctx.plan.mirror(ctx.lay, *ctx.VE, *ctx.W, ctx.cfg, ctx.plan, ctx.saved, gHv, ctx.has_bias)
+        return _mp_grads(ctx, grads, 2)
 
 
 # ----------------------------------------------------------------------------------------------
 # mol-atom-bond message passing on the bf16 tier (chemprop/nn/message_passing/mol_atom_bond.py): the depth loop and the
 # W_vo read-out of Bond / AtomMPFunction, plus the per-edge head H_e = tau(W_eo([E || H^{T-1}])) in the caller's edge order
 # ----------------------------------------------------------------------------------------------
-def mab_bf16_limits(kind: str, h: int, d_v: int, d_e: int) -> str | None:
-    """None when every GEMM of the bf16 mol-atom-bond path fits the tensor-core kernels (the limits of _tc_ok / _atom_tc_ok
-    plus K = d_e + d_h for W_eo), else the reason it does not."""
-    Ks = (d_v + d_e, d_v + h, d_e + h) if kind == "bond" else (d_v, h + d_e, d_v + h, d_e + h)
-    if h > 304:
-        return f"d_h = {h} > 304"
-    if h % 4 != 0:
-        return f"d_h = {h} not a multiple of 4"
-    if d_e == 0:
-        return "d_e = 0"
-    if any(k > 448 for k in Ks):
-        return f"GEMM inner dimensions {Ks} above 448"
-    if not _fused_available():
-        return "tensor-core kernels unavailable"
-    return None
-
-
 def mab_tables(lay: Layout):
     """(dst atom of caller edge e, src atom of caller edge e, caller edge of the reverse of dst-sorted row r) as int32, built
     once per batch: the residual map of the bond kind's mirror, the gather of the atom kind's edge operand, and the
@@ -1841,26 +1831,21 @@ class MABMPFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, V, E, Wi, bi, Wh, bh, Wvo, bvo, Weo, beo, lay, cfg, kind):
-        _require_cuda(V, E, Wi, Wh)
-        _refuse_feature_grads(ctx)
-        V = V.contiguous().float()
-        E = E.contiguous().float()
-        f = lambda w: None if w is None else w.detach().contiguous().float()  # noqa: E731
-        Wi_, bi_, Wh_, bh_, Wvo_, bvo_, Weo_, beo_ = (f(w) for w in (Wi, bi, Wh, bh, Wvo, bvo, Weo, beo))
+        V, E, (Wi_, bi_, Wh_, bh_, Wvo_, bvo_, Weo_, beo_) = _mp_inputs(ctx, V, E, (Wi, bi, Wh, bh, Wvo, bvo, Weo, beo))
         h = Wh_.shape[0]
         d_v, d_e = V.shape[1], E.shape[1]
         nE, nV = lay.E, lay.V
         dev, T = V.device, cfg.hidden_dtype
         a, ap = cfg.act, cfg.act_param
+        p = plan("mab_" + kind, cfg, lay, h, d_v, d_e)
         if kind == "bond":
-            Hv, saved = bond_forward(lay, V, E, Wi_, bi_, Wh_, bh_, Wvo_, bvo_, cfg, for_backward=any(ctx.needs_input_grad),
-                                     readout_f32=True)
+            Hv, saved = p.forward(lay, V, E, Wi_, bi_, Wh_, bh_, Wvo_, bvo_, cfg, p, for_backward=any(ctx.needs_input_grad),
+                                  readout_f32=True)
             src_idx = lay.inv_perm
             if Weo_ is not None and nE > 0:
                 mab_tables(lay)            # built here, on the forward's stream, for the backward's residual map
         else:
-            fwd = atom_forward_fused if _atom_fused_ok(cfg, lay, h, d_v, d_e) else atom_forward_tc
-            Hv, saved = fwd(lay, V, E, Wi_, bi_, Wh_, bh_, Wvo_, bvo_, cfg, readout_f32=True)
+            Hv, saved = p.forward(lay, V, E, Wi_, bi_, Wh_, bh_, Wvo_, bvo_, cfg, p, readout_f32=True)
             src_idx = mab_tables(lay)[1] if nE > 0 else None
         He = Xe = None
         if Weo_ is not None:
@@ -1877,14 +1862,9 @@ class MABMPFunction(torch.autograd.Function):
                 Xe = torch.empty((nE, (d_e + h + 15) // 16 * 16), dtype=T, device=dev)
                 concat_bf16(E, d_e, Xe, nE, X2=Hfin, K2=h, idx2=src_idx)
                 linear_tc_rows(Xe, d_e + h, pack_weight_tc(Weo_), h, He, R=nE, bias=beo_, act=a, act_param=ap)
-        if Hv is not None:
-            saved["Hv"] = Hv.detach()          # see BondMPFunction.forward: no reference cycle through the output
-        ctx.lay, ctx.cfg, ctx.saved, ctx.kind = lay, cfg, saved, kind
-        ctx.VE = (V, E)
-        ctx.W = (Wi_, Wh_, Wvo_, Weo_)
+        _mp_save(ctx, lay, cfg, p, V, E, (Wi_, Wh_, Wvo_, Weo_), saved, Hv)
+        ctx.kind = kind
         ctx.edge = (Xe, None if He is None else He.detach())
-        ctx.has_bias = (bi is not None, bh is not None, bvo is not None, beo is not None)
-        ctx.wdtypes = tuple(None if w is None else w.dtype for w in (Wi, Wh, Wvo, Weo))
         empty = torch.empty((0, h), dtype=torch.float32, device=dev)
         return (Hv if Hv is not None else empty), (He if He is not None else empty)
 
@@ -1938,15 +1918,10 @@ class MABMPFunction(torch.autograd.Function):
             z = lambda w, b: (torch.zeros_like(w), torch.zeros(w.shape[0], **f32) if b else None)  # noqa: E731
             (dWi, dbi), (dWh, dbh) = z(Wi, nb[0]), z(Wh, nb[1])
             dWvo = dbvo = None
-        elif kind == "bond":
-            dWi, dbi, dWh, dbh, dWvo, dbvo = bond_backward_tc(lay, V, E, Wi, Wh, Wvo, cfg, ctx.saved, gv, nb, entry=entry)
         else:
-            bwd = atom_backward_fused if ctx.saved.get("fused") else atom_backward_tc
-            dWi, dbi, dWh, dbh, dWvo, dbvo = bwd(lay, V, E, Wi, Wh, Wvo, cfg, ctx.saved, gv, nb, entry=entry)
-        d0, d1, d2, d3 = ctx.wdtypes
-        cast = lambda g, d: None if (g is None or d is None) else g.to(d)  # noqa: E731
-        return (None, None, cast(dWi, d0), cast(dbi, d0), cast(dWh, d1), cast(dbh, d1), cast(dWvo, d2), cast(dbvo, d2),
-                cast(dWeo, d3), cast(dbeo, d3), None, None, None)
+            dWi, dbi, dWh, dbh, dWvo, dbvo = ctx.plan.mirror(lay, V, E, Wi, Wh, Wvo, cfg, ctx.plan, ctx.saved, gv, nb,
+                                                             entry=entry)
+        return _mp_grads(ctx, (dWi, dbi, dWh, dbh, dWvo, dbvo, dWeo, dbeo), 3)
 
 
 # ----------------------------------------------------------------------------------------------

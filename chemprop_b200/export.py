@@ -42,13 +42,11 @@ def mp_forward(V: Tensor, E: Tensor, edge_index: Tensor, rev_edge_index: Tensor,
                           hidden_dtype=torch.bfloat16 if bf16 else torch.float32, fused=bool(fused))
     f = lambda t: None if t is None else t.detach().contiguous().float()  # noqa: E731
     Vf, Ef = V.contiguous().float(), E.contiguous().float()
+    # the atom forward here is atom_forward_tc or atom_forward, never the fused atom step: that step rounds to bf16 at other
+    # points, so moving exported atom models onto it would change their results
+    p = engine.plan("bond" if kind == KIND_BOND else "export_atom", cfg, lay, W_i.shape[0], Vf.shape[1], Ef.shape[1])
     with torch.no_grad():
-        if kind == KIND_BOND:
-            Hv, _ = engine.bond_forward(lay, Vf, Ef, f(W_i), f(b_i), f(W_h), f(b_h), f(W_o), f(b_o), cfg)
-        else:
-            tc = engine._atom_tc_ok(cfg, W_i.shape[0], Vf.shape[1], Ef.shape[1]) and lay.V > 0
-            fwd = engine.atom_forward_tc if tc else engine.atom_forward
-            Hv, _ = fwd(lay, Vf, Ef, f(W_i), f(b_i), f(W_h), f(b_h), f(W_o), f(b_o), cfg)
+        Hv, _ = p.forward(lay, Vf, Ef, f(W_i), f(b_i), f(W_h), f(b_h), f(W_o), f(b_o), cfg, p)
     return Hv.clone(memory_format=torch.contiguous_format)
 
 

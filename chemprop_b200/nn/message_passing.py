@@ -20,7 +20,7 @@ import torch
 from torch import Tensor, nn
 
 from .. import _lib, composed
-from ..engine import AtomMPFunction, BondMPFunction, MPConfig, _warn_once, dropout_fused_ok, get_layout
+from ..engine import AtomMPFunction, BondMPFunction, MPConfig, _warn_once, get_layout, plan
 from ..exceptions import InvalidShapeError
 
 try:                                   # custom-op registration for torch.export (inference); optional
@@ -206,10 +206,13 @@ class BondMessagePassing(_MessagePassingBase):
     _composed_forward = staticmethod(composed.bond_forward)
 
     def _dropout_on_fused_path(self, lay) -> bool:
+        if not (self.precision == "bf16" and 0.0 < self.dropout.p < 1.0 and is_fused_activation(self.tau)):
+            return False
         h = self.W_h.out_features
         d_v = self.W_o.in_features - h
-        return (self.precision == "bf16" and 0.0 < self.dropout.p < 1.0 and is_fused_activation(self.tau)
-                and dropout_fused_ok(self._config(), lay, h, d_v, self.W_i.in_features - d_v))
+        cfg = self._config()
+        cfg.dropout_p = float(self.dropout.p)
+        return plan("bond", cfg, lay, h, d_v, self.W_i.in_features - d_v).dropout_ok
 
     def setup(self, d_v=DEFAULT_ATOM_FDIM, d_e=DEFAULT_BOND_FDIM, d_h=DEFAULT_HIDDEN_DIM, d_vd=None, bias=False):
         W_i = nn.Linear(d_v + d_e, d_h, bias)

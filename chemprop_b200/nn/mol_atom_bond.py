@@ -10,8 +10,9 @@ Per-edge outputs are handed back in the caller's edge order.  CUDA only, like th
   * "bf16": engine.MABMPFunction -- bf16 hidden states, the fused depth step of the bf16 tier, the W_vo read-out and the
     per-edge W_eo head as tensor-core GEMMs with bias, tau and an f32 store in their epilogues; within 1e-2.  It applies
     when the activation is fused (ReLU, LeakyReLU, Tanh, ELU), `undirected=False`, no training-mode dropout, and the GEMM
-    sizes fit the tensor-core kernels (d_h <= 304 and a multiple of 4, every inner dimension -- d_e + d_h for W_eo
-    included -- <= 448).  Anything else runs on the composed tier, with a one-time RuntimeWarning naming the reason.
+    sizes fit the tensor-core kernels (d_h <= engine.MAX_TC_HIDDEN and a multiple of 4, every inner dimension -- d_e + d_h
+    for W_eo included -- <= engine.MAX_TC_K).  Anything else runs on the composed tier, with a one-time RuntimeWarning
+    naming the reason.
     No host synchronisation on the path: a training step captures into CudaGraphStep.
 Both tiers return f32 `H_v` / `H_e`: every consumer (atom / bond predictors, W_vd / W_ed, MolAtomBondMPNN) holds f32
 parameters.
@@ -22,7 +23,7 @@ import torch
 from torch import Tensor, nn
 
 from .. import composed
-from ..engine import MABMPFunction, MPConfig, _warn_once, get_layout, mab_bf16_limits
+from ..engine import MABMPFunction, MPConfig, _warn_once, get_layout, plan
 from ..exceptions import InvalidShapeError
 from .message_passing import (DEFAULT_ATOM_FDIM, DEFAULT_BOND_FDIM, DEFAULT_HIDDEN_DIM, activation_name,
                               engine_activation, get_activation_function, is_fused_activation)
@@ -81,7 +82,8 @@ class _MABMessagePassingBase(nn.Module):
             return "undirected=True"
         if self.training and self.dropout.p > 0:
             return "training-mode dropout"
-        return mab_bf16_limits(self._kind, self.W_h.out_features, self.hparams["d_v"], self.hparams["d_e"])
+        return plan("mab_" + self._kind, self._config(), None, self.W_h.out_features, self.hparams["d_v"],
+                    self.hparams["d_e"]).reason
 
     def uses_composed_tier(self) -> bool:
         return self.precision != "bf16" or self.composed_reason() is not None

@@ -272,7 +272,7 @@ def check_attentive(device: str, atol: float = 2e-6):
 
 
 def fused_dropout_vs_oracle(device: str, depth: int = 3, bias: bool = True, d_h: int = 64, n_mols: int = 60, p: float = 0.3):
-    """Training-mode dropout on the fused bf16 / ReLU path (engine.dropout_fused_ok) vs the oracle fed with the very keep
+    """Training-mode dropout on the fused bf16 / ReLU path (engine.Plan.dropout_ok) vs the oracle fed with the very keep
     masks the run drew (mapped from the engine's row order to the caller's edge order): hidden states within the bf16
     bound, gradients within a bound that a wrong 1 / (1 - p) factor anywhere in the mirror would break."""
     from chemprop_b200.data import BatchMolGraph, make_molecules
