@@ -102,6 +102,15 @@ SIGNATURES = {
     "dmpnn_spectral_loss_workspace_bytes": (C.c_int, [_i64, C.POINTER(_sz)]),
     "dmpnn_sid_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _i64, _vp, _vp]),
     "dmpnn_wasserstein_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _i64, _vp, _vp]),
+    "dmpnn_edge_pair_mean": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp]),
+    "dmpnn_edge_pair_mean_bwd": (C.c_int, [_vp, _i64, _i64, _i64, _vp, _i64, _vp]),
+    "dmpnn_regression_loss_rows_workspace_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
+    "dmpnn_regression_loss_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp, _i64,
+                                             _vp, _vp]),
+    "dmpnn_bce_loss_rows_workspace_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
+    "dmpnn_bce_loss_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i64, _vp, _vp]),
+    "dmpnn_ce_loss_rows_workspace_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
+    "dmpnn_ce_loss_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp]),
 }
 
 # dmpnn_pred_transform kinds (include/dmpnn.h)

@@ -721,6 +721,68 @@ def wasserstein_loss(P: Tensor, Y: Tensor, w, tw, threshold, loss: Tensor, dP: T
     _spectral_loss("dmpnn_wasserstein_loss", P, Y, w, tw, threshold, loss, dP)
 
 
+# ---- atom- and bond-level heads (csrc/row_head.cu) ----------------------------------------------------------------
+def edge_pair_mean(P: Tensor, rev: Tensor, out: Tensor):
+    """out (E/2 x C) = (P[2i] + P[2i+1]) / 2 of P (E x C), NaN rows where rev[2i] != 2i+1 (rev: int32, E)."""
+    lib = _lib.load()
+    E, Cc = P.shape
+    rc = lib.dmpnn_edge_pair_mean(P.data_ptr(), P.stride(0) if E else Cc, rev.data_ptr(), E, Cc, out.data_ptr(),
+                                  out.stride(0) if E else Cc, _stream())
+    _lib.check(rc, "dmpnn_edge_pair_mean")
+
+
+def edge_pair_mean_bwd(G: Tensor, dP: Tensor):
+    """dP (E x C): rows 2i and 2i+1 both G[i] / 2."""
+    lib = _lib.load()
+    E, Cc = dP.shape
+    rc = lib.dmpnn_edge_pair_mean_bwd(G.data_ptr(), G.stride(0) if E else Cc, E, Cc, dP.data_ptr(), dP.stride(0) if E else Cc,
+                                      _stream())
+    _lib.check(rc, "dmpnn_edge_pair_mean_bwd")
+
+
+def _rows_workspace(fn: str, B: int, T: int, dev) -> Tensor:
+    lib = _lib.load()
+    n = C.c_size_t(0)
+    _lib.check(getattr(lib, fn + "_workspace_bytes")(B, T, C.byref(n)), fn + "_workspace_bytes")
+    return torch.empty(max(n.value, 1), dtype=torch.uint8, device=dev)
+
+
+def regression_loss_rows(P: Tensor, Y: Tensor, w, tw, lt_mask, gt_mask, kind: int, loss: Tensor, dP: Tensor):
+    """regression_loss over the whole grid (dmpnn_regression_loss_rows): same arguments and results, for V or E rows."""
+    lib = _lib.load()
+    B, T = P.shape
+    for m in (lt_mask, gt_mask):
+        if m is not None:
+            assert m.dtype == torch.uint8 and m.shape == (B, T) and m.is_contiguous(), "masks: contiguous B x T uint8"
+    ws = _rows_workspace("dmpnn_regression_loss_rows", B, T, P.device)
+    rc = lib.dmpnn_regression_loss_rows(P.data_ptr(), P.stride(0) if B else T, Y.data_ptr(), Y.stride(0) if B else T,
+                                        _ptr(w), _ptr(tw), _ptr(lt_mask), _ptr(gt_mask), T, B, T, kind, loss.data_ptr(),
+                                        _ptr(dP), dP.stride(0) if B else T, ws.data_ptr(), _stream())
+    _lib.check(rc, "dmpnn_regression_loss_rows")
+
+
+def bce_loss_rows(P: Tensor, Y: Tensor, w, tw, loss: Tensor, dP: Tensor):
+    """bce_loss over the whole grid (dmpnn_bce_loss_rows)."""
+    lib = _lib.load()
+    B, T = P.shape
+    ws = _rows_workspace("dmpnn_bce_loss_rows", B, T, P.device)
+    rc = lib.dmpnn_bce_loss_rows(P.data_ptr(), P.stride(0) if B else T, Y.data_ptr(), Y.stride(0) if B else T, _ptr(w),
+                                 _ptr(tw), B, T, loss.data_ptr(), _ptr(dP), dP.stride(0) if B else T, ws.data_ptr(), _stream())
+    _lib.check(rc, "dmpnn_bce_loss_rows")
+
+
+def ce_loss_rows(P: Tensor, Y: Tensor, w, tw, C_: int, loss: Tensor, dP: Tensor):
+    """ce_loss over the whole grid (dmpnn_ce_loss_rows); P: B x (T*C) logits, Y: B x T class labels."""
+    lib = _lib.load()
+    B, TC = P.shape
+    T = Y.shape[1]
+    ws = _rows_workspace("dmpnn_ce_loss_rows", B, T, P.device)
+    rc = lib.dmpnn_ce_loss_rows(P.data_ptr(), P.stride(0) if B else TC, Y.data_ptr(), Y.stride(0) if B else T, _ptr(w),
+                                _ptr(tw), B, T, C_, loss.data_ptr(), _ptr(dP), dP.stride(0) if B else TC, ws.data_ptr(),
+                                _stream())
+    _lib.check(rc, "dmpnn_ce_loss_rows")
+
+
 def column_sum(Y: Tensor, R: int, N: int, out: Tensor, *, accumulate: bool = False):
     lib = _lib.load()
     n = C.c_size_t(0)

@@ -8,6 +8,7 @@ from .head import (EngineBatchNorm1d, EngineBinaryClassificationFFN, EngineBinar
                    EngineSID, EngineSpectralFFN, EngineWasserstein)
 from .message_passing import AtomMessagePassing, BondMessagePassing
 from .mol_atom_bond import MABAtomMessagePassing, MABBondMessagePassing
+from .mol_atom_bond_model import EngineMolAtomBondMPNN
 from .transforms import GraphTransform, ScaleTransform, UnscaleTransform
 
 __all__ = ["Aggregation", "AggregationRegistry", "AttentiveAggregation", "MeanAggregation", "NormAggregation", "SumAggregation",
@@ -17,4 +18,4 @@ __all__ = ["Aggregation", "AggregationRegistry", "AttentiveAggregation", "MeanAg
            "EngineQuantileFFN", "EngineBinaryDirichletFFN", "EngineMulticlassDirichletFFN", "EngineMVELoss",
            "EngineEvidentialLoss", "EngineQuantileLoss", "EngineDirichletLoss", "EngineSpectralFFN", "EngineSID",
            "EngineWasserstein", "EngineMAE", "EngineRMSE", "EngineBoundedMSE", "EngineBoundedMAE", "EngineBoundedRMSE",
-           "EngineBatchNorm1d", "EngineLinear"]
+           "EngineBatchNorm1d", "EngineLinear", "EngineMolAtomBondMPNN"]

@@ -122,10 +122,77 @@ class LinearActFunction(torch.autograd.Function):
         return dX, dW.to(wdt), (None if db is None else db.to(bdt)), None, None
 
 
+class EdgePairOperand:
+    """The bond-level fingerprint `[H_e || H_e[rev]]` of chemprop's MolAtomBondMPNN (E x 2h) without the E x 2h buffer:
+    H (E x h) and the int32 reverse-edge index.  EngineLinear consumes it through PairLinearFunction; `materialize()` gives
+    the concatenation for code that needs a tensor."""
+
+    def __init__(self, H: Tensor, rev: Tensor):
+        self.H, self.rev = H, rev
+
+    @property
+    def shape(self) -> torch.Size:
+        return torch.Size((self.H.shape[0], 2 * self.H.shape[1]))
+
+    def dim(self) -> int:
+        return 2
+
+    def __len__(self) -> int:
+        return self.H.shape[0]
+
+    def materialize(self) -> Tensor:
+        return torch.cat((self.H, self.H[self.rev.long()]), dim=1)
+
+
+class PairLinearFunction(torch.autograd.Function):
+    """Y = act([H || H[rev]] . W^T + b) with the second half of the operand gathered by the GEMM (dmpnn_linear_fwd,
+    X2 = H, idx2 = rev); mirror: dW / db from the same gathered operand (dmpnn_linear_wgrad), and
+    dH = [dZ || dZ[rev]] . [W_a^T | W_b^T] in one dmpnn_linear_fwd (W = [W_a | W_b]; rev is an involution)."""
+
+    @staticmethod
+    def forward(ctx, H, rev, W, b, act, act_param):
+        K._require_cuda(H, W)
+        Hc, Wc = H.float().contiguous(), W.detach().float().contiguous()
+        bc = None if b is None else b.detach().float().contiguous()
+        E, h = Hc.shape
+        N = Wc.shape[0]
+        if Wc.shape[1] != 2 * h:
+            raise ValueError(f"the bond-level fingerprint has {2 * h} columns, the layer takes {Wc.shape[1]}")
+        Y = torch.empty((E, N), dtype=torch.float32, device=H.device)
+        if E > 0:
+            K.linear_fwd(Hc, h, Wc, Y, N, X2=Hc, K2=h, idx2=rev, bias=bc, act=act, act_param=act_param, R=E, pad_to=N)
+        ctx.save_for_backward(Hc, rev, Wc, Y)
+        ctx.cfg = (act, act_param, b is not None, W.dtype, None if b is None else b.dtype, H.dtype)
+        return Y
+
+    @staticmethod
+    def backward(ctx, dY):
+        Hc, rev, Wc, Y = ctx.saved_tensors
+        act, ap, has_b, wdt, bdt, hdt = ctx.cfg
+        E, h = Hc.shape
+        N = Wc.shape[0]
+        dZ = dY.float().contiguous()
+        if act != _lib.ACT_NONE and E > 0:
+            dZ = torch.empty_like(dZ)
+            K.act_bwd(dY.float().contiguous(), Y, E, N, act=act, act_param=ap, dZ=dZ)
+        dW = torch.zeros_like(Wc)
+        db = torch.zeros(N, dtype=torch.float32, device=Wc.device) if has_b else None
+        dH = torch.zeros_like(Hc) if ctx.needs_input_grad[0] else None
+        if E > 0:
+            K.linear_wgrad(dZ, Hc, h, dW, N, X2=Hc, K2=h, idx2=rev, dbias=db, R=E)
+            if dH is not None:
+                WT = torch.cat((Wc[:, :h].t(), Wc[:, h:].t()), dim=1).contiguous()     # h x 2N
+                K.linear_fwd(dZ, N, WT, dH, h, X2=dZ, K2=N, idx2=rev, R=E, pad_to=h)
+        return (None if dH is None else dH.to(hdt)), None, dW.to(wdt), (None if db is None else db.to(bdt)), None, None
+
+
 class EngineLinear(nn.Linear):
-    """nn.Linear (same parameters / state-dict keys) executed by dmpnn_linear_fwd / dmpnn_linear_wgrad (f32)."""
+    """nn.Linear (same parameters / state-dict keys) executed by dmpnn_linear_fwd / dmpnn_linear_wgrad (f32).  An
+    EdgePairOperand input runs PairLinearFunction: the pair concatenation is gathered, never stored."""
 
     def forward(self, x: Tensor, act: int = _lib.ACT_NONE, act_param: float = 0.0) -> Tensor:
+        if isinstance(x, EdgePairOperand):
+            return PairLinearFunction.apply(x.H, x.rev, self.weight, self.bias, act, act_param)
         return LinearActFunction.apply(x, self.weight, self.bias, act, act_param)
 
 

@@ -1,0 +1,254 @@
+"""`EngineMolAtomBondMPNN`: chemprop's `MolAtomBondMPNN` (chemprop/models/mol_atom_bond.py) without Lightning, on the
+engine -- what follows the MAB message passing: three batch norms (molecule, atom and edge fingerprints), the bond
+fingerprint `[H_e || H_e[rev]]`, molecule-, atom- and bond-level predictors, the bond predictor's average over each
+reverse-edge pair, atom and bond constraints, and the sum of the per-level criteria.
+
+- The bond fingerprint is an EdgePairOperand: the bond predictor's first layer gathers `H_e[rev]` inside its GEMM
+  (PairLinearFunction), so the E x 2h concatenation is never stored, and its mirror sends the gradient back into H_e.
+- The pair mean `(P[2i] + P[2i+1]) / 2` is dmpnn_edge_pair_mean (NaN rows where edge 2i+1 is not the reverse of edge 2i),
+  applied by the model to the bond predictor's output and, through `_EdgePairMeanMLP`, to the bond constrainer's MLP
+  output, as the reference's wrappers do.
+- Atom- and bond-level criteria: MSE, MAE, RMSE and their bounded variants, BCE and cross-entropy run on the row-parallel
+  kernels (dmpnn_regression_loss_rows, dmpnn_bce_loss_rows, dmpnn_ce_loss_rows); any other engine criterion runs on its
+  own kernel.  The molecule level calls its predictor's criterion, as EngineMPNN does.
+- No host synchronisation without constraints: a constraint-free training step captures into CudaGraphStep.
+  ConstrainerFFN reads which constraint columns are set on the host (`has.any()`), so steps with constraints are eager
+  only.
+
+Module tree and state-dict keys are the reference's (`bns.*`, `{mol,atom,bond}_predictor.*`, `{atom,bond}_constrainer.*`):
+a reference `MolAtomBondMPNN` state dict without its `metricss.*` entries loads with `strict=True`."""
+from __future__ import annotations
+
+import torch
+from torch import Tensor, nn
+
+from .. import _lib
+from .. import engine as K
+from .head import (EdgePairOperand, PairLinearFunction, _BCECriterion, _Criterion, _CrossEntropyCriterion, _loss_weights,
+                   _RegressionCriterion, EngineBatchNorm1d)
+
+_LEVELS = ("mol", "atom", "bond")
+
+
+class EdgePairMeanFunction(torch.autograd.Function):
+    """P (E x ...) -> (P[2i] + P[2i+1]) / 2 (E/2 x ...) in one launch (dmpnn_edge_pair_mean; mirror
+    dmpnn_edge_pair_mean_bwd).  An odd E is refused."""
+
+    @staticmethod
+    def forward(ctx, P, rev):
+        K._require_cuda(P, rev)
+        E = P.shape[0]
+        if E % 2:
+            raise ValueError(f"the reverse-edge pair mean needs an even number of directed edges, got {E}")
+        X = P.float().reshape(E, -1).contiguous()
+        out = torch.empty((E // 2, X.shape[1]), dtype=torch.float32, device=P.device)
+        if E > 0 and X.shape[1] > 0:
+            K.edge_pair_mean(X, rev, out)
+        ctx.cfg = (tuple(P.shape), P.dtype)
+        return out.view(E // 2, *P.shape[1:])
+
+    @staticmethod
+    def backward(ctx, g):
+        shape, dt = ctx.cfg
+        E = shape[0]
+        G = g.float().reshape(E // 2, -1).contiguous()
+        dP = torch.empty((E, G.shape[1]), dtype=torch.float32, device=g.device)
+        if E > 0 and G.shape[1] > 0:
+            K.edge_pair_mean_bwd(G, dP)
+        return dP.view(shape).to(dt), None
+
+
+class RowLossFunction(torch.autograd.Function):
+    """The atom- and bond-level criteria on R x T predictions (R x T x C logits for cross-entropy): loss and dLoss/dPreds
+    from the row-parallel kernels -- `which` "regression" (kind _lib.LOSS_*, optional lt / gt masks), "bce" or "ce"."""
+
+    @staticmethod
+    def forward(ctx, preds, targets, weights, task_weights, lt_mask, gt_mask, kind, which):
+        K._require_cuda(preds, targets, lt_mask, gt_mask)
+        R = preds.shape[0]
+        P = preds.float().reshape(R, -1).contiguous()
+        Y = targets.float().reshape(R, -1).contiguous()
+        T = Y.shape[1]
+        if (which == "ce" and (preds.dim() != 3 or preds.shape[1] != T)) or (which != "ce" and P.shape != Y.shape):
+            raise ValueError(f"predictions {tuple(preds.shape)} do not match targets {tuple(targets.shape)}")
+        w, tw = _loss_weights(weights, task_weights, R, T)
+        loss = torch.empty(1, device=P.device)
+        dP = torch.empty_like(P)
+        if which == "regression":
+            lt, gt = (None if m is None else m.to(torch.uint8).reshape(R, -1).expand(R, T).contiguous()
+                      for m in (lt_mask, gt_mask))
+            K.regression_loss_rows(P, Y, w, tw, lt, gt, kind, loss, dP)
+        elif which == "bce":
+            K.bce_loss_rows(P, Y, w, tw, loss, dP)
+        else:
+            K.ce_loss_rows(P, Y, w, tw, preds.shape[2], loss, dP)
+        ctx.save_for_backward(dP.view(preds.shape))
+        ctx.pdtype = preds.dtype
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        (dP,) = ctx.saved_tensors
+        return (dP * g).to(ctx.pdtype), None, None, None, None, None, None, None
+
+
+def row_criterion_loss(criterion: nn.Module, preds: Tensor, targets: Tensor, weights: Tensor | None = None,
+                       lt_mask: Tensor | None = None, gt_mask: Tensor | None = None) -> Tensor:
+    """`criterion(preds, targets, isfinite(targets), weights, lt_mask, gt_mask)` over atom or bond rows: the MSE / MAE /
+    RMSE family (bounded or not), BCE and cross-entropy on the row-parallel kernels, any other criterion on its own."""
+    bounded = getattr(criterion, "_bounded", False)
+    masks = lt_mask is not None or gt_mask is not None
+    which = None
+    if type(criterion) is _Criterion or isinstance(criterion, _RegressionCriterion):
+        which = "regression"
+    elif type(criterion) is _BCECriterion:
+        which = "bce"
+    elif type(criterion) is _CrossEntropyCriterion:
+        which = "ce"
+    if which is None:
+        return criterion(preds, targets, None, weights, lt_mask, gt_mask) if masks else criterion(preds, targets, None, weights)
+    if masks and not bounded:
+        raise NotImplementedError(f"{type(criterion).__name__} takes no lt_mask / gt_mask; the bounded criteria "
+                                  "(EngineBoundedMSE, EngineBoundedMAE, EngineBoundedRMSE) do")
+    kind = getattr(criterion, "_kind", _lib.LOSS_MSE)
+    return RowLossFunction.apply(preds, targets, weights, criterion.task_weights, lt_mask, gt_mask, kind, which)
+
+
+class _EdgePairMeanMLP(nn.Sequential):
+    """The bond constrainer's MLP (`ConstrainerFFN.ffn`, same children and state-dict keys) followed by the reverse-edge
+    pair mean, as the reference wraps `bond_constrainer.ffn.forward`.  It takes the model's EdgePairOperand: the first
+    Linear gathers H_e[rev] in its GEMM (PairLinearFunction), the remaining blocks run as ConstrainerFFN runs them."""
+
+    def forward(self, x):
+        if not isinstance(x, EdgePairOperand):
+            raise TypeError("the bond constrainer of EngineMolAtomBondMPNN takes the model's bond-level fingerprint "
+                            "(an EdgePairOperand)")
+        first = self[0]
+        lin = first[-1]
+        X = PairLinearFunction.apply(x.H, x.rev, lin.weight, lin.bias, _lib.ACT_NONE, 0.0)
+        for block in list(self)[1:]:
+            X = block(X)
+        return EdgePairMeanFunction.apply(X, x.rev)
+
+
+class EngineMolAtomBondMPNN(nn.Module):
+    """chemprop's `MolAtomBondMPNN` (models/mol_atom_bond.py) reduced to its path, on the engine: MAB message passing ->
+    (aggregation) -> three batch norms -> molecule-, atom- and bond-level predictors (any Engine*FFN) -> constraints ->
+    the sum of the per-level criteria.
+
+    - `fingerprint(bmg, V_d, E_d, X_d) -> (H_g, H_v, H_e)`, H_e an EdgePairOperand standing for `[H_e || H_e[rev]]`.
+    - `forward(bmg, V_d, E_d, X_d, constraints=None)`: the list of the three predictions (None for an absent level), the
+      bond level averaged over each reverse-edge pair, with the constrainers applied as the reference does (to
+      `preds[..., 0]` for multi-target predictors).
+    - `training_loss(bmg, targetss, weightss, V_d, E_d, X_d, lt_masks=None, gt_masks=None, constraints=None)`:
+      `MolAtomBondMPNN.training_step` without logging.  NaN targets are masked.  Without constraints the step never
+      synchronises with the host and captures into CudaGraphStep; with constraints it is eager only (ConstrainerFFN
+      reads the set constraint columns on the host).
+
+    A bond constrainer gets its MLP wrapped in `_EdgePairMeanMLP` (same children, same state-dict keys), which averages the
+    MLP output over each reverse-edge pair as the reference's wrapper does; that constrainer then takes this model's bond
+    fingerprint only.  The molecule index of each bond is derived on the device, `batch[edge_index[0, ::2]]`."""
+
+    def __init__(self, message_passing: nn.Module, agg: nn.Module | None = None, mol_predictor: nn.Module | None = None,
+                 atom_predictor: nn.Module | None = None, bond_predictor: nn.Module | None = None,
+                 atom_constrainer: nn.Module | None = None, bond_constrainer: nn.Module | None = None,
+                 batch_norm: bool = False, X_d_transform: nn.Module | None = None):
+        if all(p is None for p in (mol_predictor, atom_predictor, bond_predictor)):
+            raise ValueError("At least one of mol_predictor, atom_predictor, or bond_predictor must be provided.")
+        if mol_predictor is not None and agg is None:
+            raise ValueError("If mol_predictor is provided, agg must also be provided.")
+        super().__init__()
+        self.message_passing = message_passing
+        self.agg = agg
+        self.mol_predictor = mol_predictor
+        self.atom_predictor = atom_predictor
+        self.atom_constrainer = atom_constrainer
+        self.bond_predictor = bond_predictor
+        if bond_constrainer is not None and not isinstance(bond_constrainer.ffn, _EdgePairMeanMLP):
+            bond_constrainer.ffn = _EdgePairMeanMLP(*bond_constrainer.ffn)
+        self.bond_constrainer = bond_constrainer
+        fp_dims = [message_passing.output_dims[0]] * 2 + [message_passing.output_dims[1]]
+        self.bns = nn.ModuleList([EngineBatchNorm1d(d) if batch_norm and p is not None else nn.Identity()
+                                  for d, p in zip(fp_dims, self.predictors)])
+        self.X_d_transform = X_d_transform if X_d_transform is not None else nn.Identity()
+
+    @property
+    def predictors(self) -> tuple:
+        return self.mol_predictor, self.atom_predictor, self.bond_predictor
+
+    @property
+    def criterions(self) -> tuple:
+        return tuple(None if p is None else p.criterion for p in self.predictors)
+
+    @property
+    def n_taskss(self) -> tuple:
+        return tuple(None if p is None else p.n_tasks for p in self.predictors)
+
+    def fingerprint(self, bmg, V_d: Tensor | None = None, E_d: Tensor | None = None, X_d: Tensor | None = None):
+        H_v, H_e = self.message_passing(bmg, V_d, E_d)
+        H_g = self.agg(H_v, bmg.batch) if self.agg is not None else None
+        H_g = self.bns[0](H_g) if H_g is not None else None
+        H_v = self.bns[1](H_v) if H_v is not None else None
+        H_e = self.bns[2](H_e) if H_e is not None else None
+        if H_g is not None and X_d is not None:
+            H_g = torch.cat((H_g, self.X_d_transform(X_d)), dim=1)
+        if H_e is not None:
+            H_e = EdgePairOperand(H_e, bmg.rev_edge_index.to(torch.int32))
+        return H_g, H_v, H_e
+
+    def _predictions(self, fps, train: bool) -> list:
+        predss = []
+        for level, (fp, predictor) in enumerate(zip(fps, self.predictors)):
+            if predictor is None:
+                predss.append(None)
+                continue
+            preds = predictor.train_step(fp) if train else predictor(fp)
+            if level == 2:
+                preds = EdgePairMeanFunction.apply(preds, fp.rev)
+            predss.append(preds)
+        return predss
+
+    def _constrain(self, bmg, fps, predss, constraints) -> list:
+        out = list(predss)
+        for level, constrainer in ((1, self.atom_constrainer), (2, self.bond_constrainer)):
+            c = constraints[level - 1]
+            if constrainer is None or out[level] is None or c is None:
+                continue
+            batch = bmg.batch if level == 1 else bmg.batch[bmg.edge_index[0, ::2]]
+            preds = out[level]
+            if preds.dim() > 2:
+                preds = preds.clone()
+                preds[..., 0] = constrainer(fps[level], preds[..., 0], batch, c)
+            else:
+                preds = constrainer(fps[level], preds, batch, c)
+            out[level] = preds
+        return out
+
+    def forward(self, bmg, V_d: Tensor | None = None, E_d: Tensor | None = None, X_d: Tensor | None = None,
+                constraints=None) -> list:
+        fps = self.fingerprint(bmg, V_d, E_d, X_d)
+        predss = self._predictions(fps, train=False)
+        return predss if constraints is None else self._constrain(bmg, fps, predss, constraints)
+
+    def training_loss(self, bmg, targetss, weightss, V_d: Tensor | None = None, E_d: Tensor | None = None,
+                      X_d: Tensor | None = None, lt_masks=None, gt_masks=None, constraints=None) -> Tensor:
+        fps = self.fingerprint(bmg, V_d, E_d, X_d)
+        predss = self._predictions(fps, train=True)
+        if constraints is not None:
+            predss = self._constrain(bmg, fps, predss, constraints)
+        total = None
+        for level, (predictor, preds) in enumerate(zip(self.predictors, predss)):
+            if predictor is None:
+                continue
+            targets = targetss[level]
+            weights = None if weightss is None else weightss[level]
+            lt = None if lt_masks is None else lt_masks[level]
+            gt = None if gt_masks is None else gt_masks[level]
+            if level == 0:
+                crit = predictor.criterion
+                l = crit(preds, targets, None, weights) if lt is None and gt is None else crit(preds, targets, None, weights,
+                                                                                               lt, gt)
+            else:
+                l = row_criterion_loss(predictor.criterion, preds, targets, weights, lt, gt)
+            total = l if total is None else total + l
+        return total

@@ -591,6 +591,46 @@ int dmpnn_wasserstein_loss(const float* P, int64_t ldp, const float* Y, int64_t 
                            const float* task_weights, int64_t B, int64_t T, float threshold, float* loss, float* dP,
                            int64_t lddp, void* workspace, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Atom- and bond-level heads (csrc/row_head.cu; chemprop/models/mol_atom_bond.py:140-151, 237-339):
+ *   dmpnn_edge_pair_mean      the bond predictor's average over each reverse-edge pair: out[i, 0:C] = (P[2i] + P[2i+1]) / 2
+ *                             for i in [0, E/2), P an E x C f32 matrix (row stride ldp), out E/2 x C (row stride ldo).
+ *                             Chemprop's edge order is assumed, in which edge 2i+1 is the reverse of edge 2i; the kernel
+ *                             reads rev (int32, E) and writes NaN across every output row i with rev[2i] != 2i+1 instead
+ *                             of a silently wrong average (the reference's wrapper does not check; a kernel cannot raise
+ *                             without synchronising with the host).  E must be even (refused otherwise); E = 0 launches
+ *                             nothing.
+ *   dmpnn_edge_pair_mean_bwd  its mirror: dP[2i] = dP[2i+1] = G[i] / 2.
+ *   dmpnn_regression_loss_rows, dmpnn_bce_loss_rows, dmpnn_ce_loss_rows
+ *                             dmpnn_regression_loss, dmpnn_bce_loss and dmpnn_ce_loss with the same arguments, conventions
+ *                             and outputs (NaN targets masked, w and tw nullable, division by the mask count, loss 0 and
+ *                             dP 0 when every target is masked, NaN for a class label outside [0, C)), for B in the
+ *                             hundreds of thousands of atom or bond rows: the terms are spread over a grid of up to 1024
+ *                             CTAs (at least 2048 terms each), each CTA writing one partial sum to `workspace`, and a
+ *                             second launch sums the partials in a fixed order and writes loss[0] and dP.  The grid depends
+ *                             on B * T only: bitwise repeatable, no floating-point atomics, no host synchronisation, and
+ *                             graph-capturable.  The summation order differs from the single-block kernels', so the two
+ *                             agree to rounding, not bit for bit.  The mask count is an exact 64-bit integer.
+ *                             workspace: *_rows_workspace_bytes(B, T) bytes, any contents (every byte read is written
+ *                             first by the same call).
+ * ------------------------------------------------------------------------------------- */
+int dmpnn_edge_pair_mean(const float* P, int64_t ldp, const int32_t* rev, int64_t E, int64_t C, float* out, int64_t ldo,
+                         void* stream);
+int dmpnn_edge_pair_mean_bwd(const float* G, int64_t ldg, int64_t E, int64_t C, float* dP, int64_t lddp, void* stream);
+int dmpnn_regression_loss_rows_workspace_bytes(int64_t B, int64_t T, size_t* bytes);
+int dmpnn_regression_loss_rows(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                               const float* task_weights, const uint8_t* lt_mask, const uint8_t* gt_mask, int64_t ldm,
+                               int64_t B, int64_t T, int kind, float* loss, float* dP, int64_t lddp, void* workspace,
+                               void* stream);
+int dmpnn_bce_loss_rows_workspace_bytes(int64_t B, int64_t T, size_t* bytes);
+int dmpnn_bce_loss_rows(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                        const float* task_weights, int64_t B, int64_t T, float* loss, float* dP, int64_t lddp,
+                        void* workspace, void* stream);
+int dmpnn_ce_loss_rows_workspace_bytes(int64_t B, int64_t T, size_t* bytes);
+int dmpnn_ce_loss_rows(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                       const float* task_weights, int64_t B, int64_t T, int64_t C, float* loss, float* dP, int64_t lddp,
+                       void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
