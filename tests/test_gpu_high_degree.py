@@ -36,15 +36,17 @@ def _complete_graph(rng, k: int, d_v: int = 72, d_e: int = 14):
     return MolGraph(V=V, E=E[p], edge_index=ei[:, p], rev_edge_index=inv[rev[p]])
 
 
-def high_degree_molecules(n_mols: int, seed: int, kmax: int = 12, reps: int = 3, big: int = 0):
+def high_degree_molecules(n_mols: int, seed: int, kmax: int = 12, reps: int = 3, big: int = 0, d_v: int = 72, d_e: int = 14):
     """n_mols molecules of 6-30 atoms with atom degree up to 6, `reps` copies of each K_6 .. K_kmax, and `big` molecules of
     70-100 atoms with degree up to 6 (more than 128 directed edges); shuffled molecule order."""
     from chemprop_b200.data import make_molecule
 
     rng = np.random.default_rng(seed)
-    mgs = [make_molecule(rng, int(rng.integers(6, 31)), ring_frac=0.25, max_deg=6, shuffle_edges=True) for _ in range(n_mols)]
-    mgs += [_complete_graph(rng, k) for k in range(6, kmax + 1) for _ in range(reps)]
-    mgs += [make_molecule(rng, int(rng.integers(70, 101)), ring_frac=0.25, max_deg=6, shuffle_edges=True) for _ in range(big)]
+    mgs = [make_molecule(rng, int(rng.integers(6, 31)), d_v, d_e, ring_frac=0.25, max_deg=6, shuffle_edges=True)
+           for _ in range(n_mols)]
+    mgs += [_complete_graph(rng, k, d_v, d_e) for k in range(6, kmax + 1) for _ in range(reps)]
+    mgs += [make_molecule(rng, int(rng.integers(70, 101)), d_v, d_e, ring_frac=0.25, max_deg=6, shuffle_edges=True)
+            for _ in range(big)]
     return [mgs[i] for i in rng.permutation(len(mgs))]
 
 
