@@ -111,6 +111,9 @@ SIGNATURES = {
     "dmpnn_bce_loss_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i64, _vp, _vp]),
     "dmpnn_ce_loss_rows_workspace_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
     "dmpnn_ce_loss_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp]),
+    "dmpnn_constrain_fwd": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _vp]),
+    "dmpnn_constrain_bwd": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64,
+                                      _vp]),
 }
 
 # dmpnn_pred_transform kinds (include/dmpnn.h)

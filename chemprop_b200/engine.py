@@ -783,6 +783,32 @@ def ce_loss_rows(P: Tensor, Y: Tensor, w, tw, C_: int, loss: Tensor, dP: Tensor)
     _lib.check(rc, "dmpnn_ce_loss_rows")
 
 
+# ---- ConstrainerFFN (csrc/constrain.cu) --------------------------------------------------------------------------
+def constrain_fwd(Kl: Tensor, P: Tensor, ptr: Tensor, Cn: Tensor, out: Tensor, status: Tensor):
+    """out (R x t) = P adjusted so that each molecule's constrained columns sum to Cn's row (ffn.py:119-141); Kl: R x n_c
+    MLP output, ptr: int32 m + 1 molecule row offsets, Cn: m x t constraints (NaN in row 0 = unconstrained column).
+    status (int32, 1): 0, or the constrained column count when (n_c, that count) is a shape the reference rejects."""
+    lib = _lib.load()
+    R, n_c = Kl.shape
+    m, t = Cn.shape
+    rc = lib.dmpnn_constrain_fwd(Kl.data_ptr(), Kl.stride(0) if R else n_c, n_c, P.data_ptr(), P.stride(0) if R else t,
+                                 ptr.data_ptr(), m, Cn.data_ptr(), Cn.stride(0) if m else t, t, out.data_ptr(),
+                                 out.stride(0) if R else t, status.data_ptr(), _stream())
+    _lib.check(rc, "dmpnn_constrain_fwd")
+
+
+def constrain_bwd(G: Tensor, Kl: Tensor, P: Tensor, ptr: Tensor, Cn: Tensor, dP: Tensor, dKl: Tensor):
+    """dP (R x t) and dKl (R x n_c) of constrain_fwd given G = dL/dout; arguments as constrain_fwd."""
+    lib = _lib.load()
+    R, n_c = Kl.shape
+    m, t = Cn.shape
+    rc = lib.dmpnn_constrain_bwd(G.data_ptr(), G.stride(0) if R else t, Kl.data_ptr(), Kl.stride(0) if R else n_c, n_c,
+                                 P.data_ptr(), P.stride(0) if R else t, ptr.data_ptr(), m, Cn.data_ptr(),
+                                 Cn.stride(0) if m else t, t, dP.data_ptr(), dP.stride(0) if R else t, dKl.data_ptr(),
+                                 dKl.stride(0) if R else n_c, _stream())
+    _lib.check(rc, "dmpnn_constrain_bwd")
+
+
 def column_sum(Y: Tensor, R: int, N: int, out: Tensor, *, accumulate: bool = False):
     lib = _lib.load()
     n = C.c_size_t(0)

@@ -191,9 +191,37 @@ class EngineLinear(nn.Linear):
     EdgePairOperand input runs PairLinearFunction: the pair concatenation is gathered, never stored."""
 
     def forward(self, x: Tensor, act: int = _lib.ACT_NONE, act_param: float = 0.0) -> Tensor:
-        if isinstance(x, EdgePairOperand):
-            return PairLinearFunction.apply(x.H, x.rev, self.weight, self.bias, act, act_param)
-        return LinearActFunction.apply(x, self.weight, self.bias, act, act_param)
+        return linear_act(self, x, act, act_param)
+
+
+def linear_act(lin: nn.Linear, x, act: int = _lib.ACT_NONE, act_param: float = 0.0) -> Tensor:
+    """act(lin(x)) on the engine's GEMMs with the activation in the epilogue, for any nn.Linear; x may be an
+    EdgePairOperand (PairLinearFunction)."""
+    if isinstance(x, EdgePairOperand):
+        return PairLinearFunction.apply(x.H, x.rev, lin.weight, lin.bias, act, act_param)
+    return LinearActFunction.apply(x, lin.weight, lin.bias, act, act_param)
+
+
+def engine_mlp(ffn: nn.Sequential, Z) -> Tensor:
+    """`ffn(Z)` for an MLP of chemprop's module tree (nn/ffn.py:38-61: Linear, then [act, dropout, Linear] per further
+    layer) on the engine's GEMMs, with every activation the engine fuses folded into the epilogue of the GEMM before it.
+    The Linear layers may be plain nn.Linear (run through linear_act); EngineLinear layers are called as modules, so their
+    hooks run.  Z may be an EdgePairOperand."""
+    blocks = [list(b) for b in ffn if isinstance(b, nn.Sequential)]
+    X = Z
+    for k, block in enumerate(blocks):
+        lin = block[-1]
+        run = lin if isinstance(lin, EngineLinear) else (lambda x, *a, lin=lin: linear_act(lin, x, *a))
+        if k + 1 == len(blocks):
+            X = run(X)
+            break
+        tau, drop = blocks[k + 1][0], blocks[k + 1][1]
+        if is_fused_activation(tau):
+            X = run(X, *engine_activation(tau))              # act(W x + b) in the GEMM epilogue
+        else:
+            X = tau(run(X))
+        X = drop(X)                                          # identity when p = 0 or in eval mode
+    return X
 
 
 class BCELossFunction(torch.autograd.Function):
@@ -626,22 +654,7 @@ class _EngineFFNPredictor(nn.Module):
         return self.output_dim // self.n_targets
 
     def _mlp(self, Z: Tensor) -> Tensor:
-        """`self.ffn(Z)` (nn/ffn.py:38-61: Linear, then [act, dropout, Linear] per further layer) with every activation the
-        engine fuses folded into the epilogue of the GEMM before it."""
-        blocks = [list(b) for b in self.ffn if isinstance(b, nn.Sequential)]
-        X = Z
-        for k, block in enumerate(blocks):
-            lin = block[-1]
-            if k + 1 == len(blocks):
-                X = lin(X)
-                break
-            tau, drop = blocks[k + 1][0], blocks[k + 1][1]
-            if is_fused_activation(tau):
-                X = lin(X, *engine_activation(tau))          # act(W x + b) in the GEMM epilogue
-            else:
-                X = tau(lin(X))
-            X = drop(X)                                      # identity when p = 0 or in eval mode
-        return X
+        return engine_mlp(self.ffn, Z)
 
 
 class EngineRegressionFFN(_EngineFFNPredictor):

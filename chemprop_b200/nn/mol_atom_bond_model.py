@@ -11,9 +11,9 @@ reverse-edge pair, atom and bond constraints, and the sum of the per-level crite
 - Atom- and bond-level criteria: MSE, MAE, RMSE and their bounded variants, BCE and cross-entropy run on the row-parallel
   kernels (dmpnn_regression_loss_rows, dmpnn_bce_loss_rows, dmpnn_ce_loss_rows); any other engine criterion runs on its
   own kernel.  The molecule level calls its predictor's criterion, as EngineMPNN does.
-- No host synchronisation without constraints: a constraint-free training step captures into CudaGraphStep.
-  ConstrainerFFN reads which constraint columns are set on the host (`has.any()`), so steps with constraints are eager
-  only.
+- No host synchronisation: a training step, with or without atom and bond constraints, captures into CudaGraphStep.  The
+  constrainers get the molecules' atom and bond offsets from the layout and decide on the device which constraint columns
+  are set (ConstrainerFFN, dmpnn_constrain_fwd / _bwd); the constraints are inputs of the graph like the targets.
 
 Module tree and state-dict keys are the reference's (`bns.*`, `{mol,atom,bond}_predictor.*`, `{atom,bond}_constrainer.*`):
 a reference `MolAtomBondMPNN` state dict without its `metricss.*` entries loads with `strict=True`."""
@@ -24,8 +24,8 @@ from torch import Tensor, nn
 
 from .. import _lib
 from .. import engine as K
-from .head import (EdgePairOperand, PairLinearFunction, _BCECriterion, _Criterion, _CrossEntropyCriterion, _loss_weights,
-                   _RegressionCriterion, EngineBatchNorm1d)
+from .head import (EdgePairOperand, _BCECriterion, _Criterion, _CrossEntropyCriterion, _loss_weights,
+                   _RegressionCriterion, EngineBatchNorm1d, engine_mlp)
 
 _LEVELS = ("mol", "atom", "bond")
 
@@ -117,18 +117,13 @@ def row_criterion_loss(criterion: nn.Module, preds: Tensor, targets: Tensor, wei
 class _EdgePairMeanMLP(nn.Sequential):
     """The bond constrainer's MLP (`ConstrainerFFN.ffn`, same children and state-dict keys) followed by the reverse-edge
     pair mean, as the reference wraps `bond_constrainer.ffn.forward`.  It takes the model's EdgePairOperand: the first
-    Linear gathers H_e[rev] in its GEMM (PairLinearFunction), the remaining blocks run as ConstrainerFFN runs them."""
+    Linear gathers H_e[rev] in its GEMM (PairLinearFunction), and every layer runs on the engine as ConstrainerFFN runs it."""
 
     def forward(self, x):
         if not isinstance(x, EdgePairOperand):
             raise TypeError("the bond constrainer of EngineMolAtomBondMPNN takes the model's bond-level fingerprint "
                             "(an EdgePairOperand)")
-        first = self[0]
-        lin = first[-1]
-        X = PairLinearFunction.apply(x.H, x.rev, lin.weight, lin.bias, _lib.ACT_NONE, 0.0)
-        for block in list(self)[1:]:
-            X = block(X)
-        return EdgePairMeanFunction.apply(X, x.rev)
+        return EdgePairMeanFunction.apply(engine_mlp(self, x), x.rev)
 
 
 class EngineMolAtomBondMPNN(nn.Module):
@@ -141,9 +136,9 @@ class EngineMolAtomBondMPNN(nn.Module):
       bond level averaged over each reverse-edge pair, with the constrainers applied as the reference does (to
       `preds[..., 0]` for multi-target predictors).
     - `training_loss(bmg, targetss, weightss, V_d, E_d, X_d, lt_masks=None, gt_masks=None, constraints=None)`:
-      `MolAtomBondMPNN.training_step` without logging.  NaN targets are masked.  Without constraints the step never
-      synchronises with the host and captures into CudaGraphStep; with constraints it is eager only (ConstrainerFFN
-      reads the set constraint columns on the host).
+      `MolAtomBondMPNN.training_step` without logging.  NaN targets are masked.  The step, constraints included, never
+      synchronises with the host while a graph is being captured, and captures into CudaGraphStep.  Eagerly, a
+      constrainer with more than one MLP output reads one status word to raise on shapes the reference rejects.
 
     A bond constrainer gets its MLP wrapped in `_EdgePairMeanMLP` (same children, same state-dict keys), which averages the
     MLP output over each reverse-edge pair as the reference's wrapper does; that constrainer then takes this model's bond
@@ -210,17 +205,21 @@ class EngineMolAtomBondMPNN(nn.Module):
 
     def _constrain(self, bmg, fps, predss, constraints) -> list:
         out = list(predss)
+        lay = K.get_layout(bmg)
         for level, constrainer in ((1, self.atom_constrainer), (2, self.bond_constrainer)):
             c = constraints[level - 1]
             if constrainer is None or out[level] is None or c is None:
                 continue
             batch = bmg.batch if level == 1 else bmg.batch[bmg.edge_index[0, ::2]]
+            # the molecules' atom offsets, and their bond offsets: each molecule's directed edges are contiguous and
+            # paired (2i, 2i + 1), which the pair mean already requires, so its bonds are its edges halved
+            offsets = lay.mol_atom_ptr if level == 1 else lay.mol_row_ptr // 2
             preds = out[level]
             if preds.dim() > 2:
                 preds = preds.clone()
-                preds[..., 0] = constrainer(fps[level], preds[..., 0], batch, c)
+                preds[..., 0] = constrainer(fps[level], preds[..., 0], batch, c, offsets=offsets)
             else:
-                preds = constrainer(fps[level], preds, batch, c)
+                preds = constrainer(fps[level], preds, batch, c, offsets=offsets)
             out[level] = preds
         return out
 

@@ -631,6 +631,30 @@ int dmpnn_ce_loss_rows(const float* P, int64_t ldp, const float* Y, int64_t ldy,
                        const float* task_weights, int64_t B, int64_t T, int64_t C, float* loss, float* dP, int64_t lddp,
                        void* workspace, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * ConstrainerFFN's segmented part (csrc/constrain.cu; chemprop/nn/ffn.py:119-141).  Molecule s owns rows
+ * [ptr[s], ptr[s+1]) of R = ptr[m] rows (int32 ptr, m + 1 entries, ptr[0] = 0; empty molecules allowed anywhere).
+ * Kl is R x n_c f32 (the constrainer MLP's output), P R x t f32, C m x t f32 (the constraints), all with row strides.
+ *   dmpnn_constrain_fwd   out[r, j] = P[r, j] + w[r, i] * (C[s, j] - sum_{r' in s} P[r', j]) for every constrained
+ *                         column j, w[r, i] = exp(Kl[r, i]) / sum_{r' in s} exp(Kl[r', i]) (no max-subtraction, as the
+ *                         reference); every other column is copied bit for bit.  Column j is constrained iff C[0, j] is
+ *                         not NaN (row 0 only, as the reference), and i is its rank among the constrained columns when n_c
+ *                         equals their number nq, 0 when n_c == 1.  Any other (n_c, nq >= 1) is a shape the reference
+ *                         rejects: every constrained column of out is NaN.  *status (1 int32, device) is written by every
+ *                         call with m > 0: 0, or nq for a rejected shape.  No constrained column: out = P.
+ *   dmpnn_constrain_bwd   given G = dL/dout: dP[r, j] = G[r, j] - a_j and dKl[r, i] = sum over the constrained j paired
+ *                         with i of D_j * w[r, i] * (G[r, j] - a_j), with D_j = C[s, j] - sum_s P[., j] and
+ *                         a_j = sum_s G[., j] * w[., i]; unconstrained columns dP = G.  No constrained column: dKl = 0;
+ *                         a rejected shape: NaN in dKl and in the constrained columns of dP.  No gradient to C.
+ * One warp per molecule, sums in a fixed order: bitwise repeatable, no atomics, no workspace, no host synchronisation.
+ * ------------------------------------------------------------------------------------- */
+int dmpnn_constrain_fwd(const float* Kl, int64_t ldk, int64_t n_c, const float* P, int64_t ldp, const int32_t* ptr,
+                        int64_t m, const float* C, int64_t ldc, int64_t t, float* out, int64_t ldo, int32_t* status,
+                        void* stream);
+int dmpnn_constrain_bwd(const float* G, int64_t ldg, const float* Kl, int64_t ldk, int64_t n_c, const float* P, int64_t ldp,
+                        const int32_t* ptr, int64_t m, const float* C, int64_t ldc, int64_t t, float* dP, int64_t lddp,
+                        float* dKl, int64_t lddk, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
