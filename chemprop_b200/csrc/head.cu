@@ -25,6 +25,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "loss_terms.cuh"
 
 namespace dmpnn {
 namespace head {
@@ -128,13 +129,6 @@ k_bn_bwd(const float* __restrict__ dY, int64_t lddy, const float* __restrict__ X
 
 enum RegLossKind { kMseLoss = 0, kMaeLoss = 1, kRmseLoss = 2 };
 
-// p - y, or 0 where BoundedMixin (metrics.py:144-149) replaces the prediction by the target: p < y with lt_mask set, or
-// p > y with gt_mask set (a censored target the prediction already satisfies; torch.where passes no gradient there)
-__device__ __forceinline__ float reg_residual(float p, float y, const uint8_t* lt, const uint8_t* gt, int64_t i) {
-  if ((lt && lt[i] && p < y) || (gt && gt[i] && p > y)) return 0.f;
-  return p - y;
-}
-
 // one block: MSE  loss[0] = sum_{b,t} w_b tw_t m_bt e^2 / sum m,  dP = 2 w tw m e / sum m   (m = isfinite(y), e = p - y)
 //            MAE  |e| in place of e^2, dP = w tw m sign(e) / sum m (sign(0) = 0, as torch's abs)
 //            RMSE sqrt of the MSE value, dP = the MSE's dP / (2 loss) (0 where the loss is 0)
@@ -214,18 +208,6 @@ __device__ __forceinline__ float2 block_sum2(float l, float cnt) {
   return s_tot;
 }
 
-// binary_cross_entropy_with_logits as torch computes it: (1 - y) x + mx + log(e^{-mx} + e^{-x-mx}), mx = max(-x, 0)
-__device__ __forceinline__ float bce_with_logits(float x, float y) {
-  const float mx = fmaxf(-x, 0.f);
-  return (1.f - y) * x + mx + logf(expf(-mx) + expf(-x - mx));
-}
-
-__device__ __forceinline__ float sigmoid_stable(float x) {
-  if (x >= 0.f) return 1.f / (1.f + expf(-x));
-  const float e = expf(x);
-  return e / (1.f + e);
-}
-
 // one block: loss[0] = sum_{b,t} w_b tw_t m_bt bce(p, y) / sum m,  dP = (sigmoid(p) - y) w tw m / sum m   (m = isfinite(y))
 __global__ void __launch_bounds__(1024)
 k_bce_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y, int64_t ldy, const float* __restrict__ w,
@@ -252,12 +234,6 @@ k_bce_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y
       dP[b * lddp + t] = isfinite(y)
           ? (sigmoid_stable(P[b * ldp + t]) - y) * (w ? w[b] : 1.f) * (tw ? tw[t] : 1.f) * inv_n : 0.f;
     }
-}
-
-// class index of a finite label as torch's `.long()` truncates it; -1 when outside [0, C)
-__device__ __forceinline__ int class_of(float y, int C) {
-  const float k = truncf(y);
-  return (k >= 0.f && k < (float)C) ? (int)k : -1;
 }
 
 // one block; row (b, t) = logits P[b, t*C : (t+1)*C].  loss[0] = sum w_b tw_t m_bt (lse(row) - row[label]) / sum m,

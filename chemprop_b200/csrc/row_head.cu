@@ -17,6 +17,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "loss_terms.cuh"
 
 namespace dmpnn {
 namespace rowhead {
@@ -69,29 +70,7 @@ __device__ __forceinline__ void block_sum(float& l, long long& n) {
   n = t_n;
 }
 
-__device__ __forceinline__ float bce_with_logits(float x, float y) {
-  const float mx = fmaxf(-x, 0.f);
-  return (1.f - y) * x + mx + logf(expf(-mx) + expf(-x - mx));
-}
-
-__device__ __forceinline__ float sigmoid_stable(float x) {
-  if (x >= 0.f) return 1.f / (1.f + expf(-x));
-  const float e = expf(x);
-  return e / (1.f + e);
-}
-
-__device__ __forceinline__ float residual(const Args& a, float p, float y, int64_t b, int t) {
-  const int64_t i = b * a.ldm + t;
-  if ((a.lt && a.lt[i] && p < y) || (a.gt && a.gt[i] && p > y)) return 0.f;
-  return p - y;
-}
-
-__device__ __forceinline__ int class_of(float y, int C) {
-  const float k = truncf(y);
-  return (k >= 0.f && k < (float)C) ? (int)k : -1;
-}
-
-// the term of element (b, t), as the single-block kernels compute it (csrc/head.cu)
+// the term of element (b, t), from the per-element functions the single-block kernels use (loss_terms.cuh)
 template <int L>
 __device__ __forceinline__ float term(const Args& a, int64_t b, int t, float y) {
   const float ww = (a.w ? a.w[b] : 1.f) * (a.tw ? a.tw[t] : 1.f);
@@ -106,7 +85,7 @@ __device__ __forceinline__ float term(const Args& a, int64_t b, int t, float y) 
   }
   const float p = a.P[b * a.ldp + t];
   if (L == kBce) return ww * bce_with_logits(p, y);
-  const float e = residual(a, p, y, b, t);
+  const float e = reg_residual(p, y, a.lt, a.gt, b * a.ldm + t);
   if (L == kMae) return ww * fabsf(e);
   return ww * e * e;
 }
@@ -181,7 +160,7 @@ k_row_loss_finish(Args a, int64_t chunk, int G, const float* __restrict__ part_l
       if (L == kBce) {
         g = (sigmoid_stable(p) - y) * ww * inv_n;
       } else {
-        const float e = residual(a, p, y, b, t);
+        const float e = reg_residual(p, y, a.lt, a.gt, b * a.ldm + t);
         if (L == kMae) g = ww * (e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f)) * inv_n;
         else g = 2.f * ww * e * inv_n;
         if (L == kRmse) g *= rmse_scale;

@@ -60,29 +60,6 @@ class BatchNormTrainFunction(torch.autograd.Function):
         return dX, dg, db, None, None, None, None
 
 
-class MSELossFunction(torch.autograd.Function):
-    """chemprop's MSE criterion: sum(w_b * tw_t * mask * (p - y)^2) / sum(mask), mask = isfinite(targets); loss and
-    dLoss/dPreds in one launch (dmpnn_mse_loss)."""
-
-    @staticmethod
-    def forward(ctx, preds, targets, weights, task_weights):
-        K._require_cuda(preds, targets)
-        P, Y = preds.float().contiguous(), targets.float().contiguous()
-        w = None if weights is None else weights.float().reshape(-1).contiguous()
-        tw = None if task_weights is None else task_weights.float().reshape(-1).contiguous()
-        loss = torch.empty(1, device=P.device)
-        dP = torch.empty_like(P)
-        K.mse_loss(P, Y, w, tw, loss, dP)
-        ctx.save_for_backward(dP)
-        ctx.pdtype = preds.dtype
-        return loss.reshape(())
-
-    @staticmethod
-    def backward(ctx, g):
-        (dP,) = ctx.saved_tensors
-        return (dP * g).to(ctx.pdtype), None, None, None
-
-
 class LinearActFunction(torch.autograd.Function):
     """Y = act(X . W^T + b) with the activation in the GEMM epilogue (dmpnn_linear_fwd); mirror: dZ = dY * act'(Y)
     (dmpnn_act_bwd), dW / db (dmpnn_linear_wgrad), dX = dZ . W (dmpnn_linear_fwd)."""
@@ -224,47 +201,6 @@ def engine_mlp(ffn: nn.Sequential, Z) -> Tensor:
     return X
 
 
-class BCELossFunction(torch.autograd.Function):
-    """chemprop's BCE criterion: sum(w_b * tw_t * mask * bce_with_logits(p, y)) / sum(mask), mask = isfinite(targets), soft
-    labels allowed; loss and dLoss/dLogits in one launch (dmpnn_bce_loss)."""
-
-    @staticmethod
-    def forward(ctx, preds, targets, weights, task_weights):
-        K._require_cuda(preds, targets)
-        P, Y = preds.float().contiguous(), targets.float().contiguous()
-        w = None if weights is None else weights.float().reshape(-1).contiguous()
-        tw = None if task_weights is None else task_weights.float().reshape(-1).contiguous()
-        loss = torch.empty(1, device=P.device)
-        dP = torch.empty_like(P)
-        K.bce_loss(P, Y, w, tw, loss, dP)
-        ctx.save_for_backward(dP)
-        ctx.pdtype = preds.dtype
-        return loss.reshape(())
-
-    backward = staticmethod(MSELossFunction.backward)
-
-
-class CrossEntropyLossFunction(torch.autograd.Function):
-    """chemprop's cross-entropy criterion on b x T x C logits and b x T class labels (truncated like `targets.long()`):
-    sum(w_b * tw_t * mask * ce) / sum(mask); loss and dLoss/dLogits in one launch (dmpnn_ce_loss)."""
-
-    @staticmethod
-    def forward(ctx, preds, targets, weights, task_weights):
-        K._require_cuda(preds, targets)
-        b, T, C = preds.shape
-        P, Y = preds.float().reshape(b, T * C).contiguous(), targets.float().contiguous()
-        w = None if weights is None else weights.float().reshape(-1).contiguous()
-        tw = None if task_weights is None else task_weights.float().reshape(-1).contiguous()
-        loss = torch.empty(1, device=P.device)
-        dP = torch.empty_like(P)
-        K.ce_loss(P, Y, w, tw, C, loss, dP)
-        ctx.save_for_backward(dP.view(b, T, C))
-        ctx.pdtype = preds.dtype
-        return loss.reshape(())
-
-    backward = staticmethod(MSELossFunction.backward)
-
-
 class ClassProbsFunction(torch.autograd.Function):
     """Eval-mode outputs of the classification predictors (dmpnn_class_probs): sigmoid of every logit, or the softmax of every
     group of C columns.  The mirror (torch elementwise ops) is off the training path; it exists because chemprop's `forward`
@@ -328,130 +264,6 @@ class PredTransformFunction(torch.autograd.Function):
         return dX.to(dt), None, None, None, None
 
 
-class UncertaintyLossFunction(torch.autograd.Function):
-    """The uncertainty criteria on b x T x u predictions under the MSE criterion's reduction: loss and dLoss/dPreds in one
-    launch (engine.<name>: dmpnn_mve_loss / dmpnn_evidential_loss / dmpnn_quantile_loss / dmpnn_dirichlet_loss)."""
-
-    @staticmethod
-    def forward(ctx, preds, targets, weights, task_weights, name, args):
-        K._require_cuda(preds, targets)
-        b, T, u = preds.shape
-        if targets.shape != (b, T):
-            raise ValueError(f"targets must be {b} x {T}, got {tuple(targets.shape)}")
-        P, Y = preds.float().reshape(b, T * u).contiguous(), targets.float().contiguous()
-        w = None if weights is None else weights.float().reshape(-1).contiguous()
-        tw = None if task_weights is None else task_weights.float().reshape(-1)
-        if tw is not None and tw.numel() == 1:                 # a scalar task weight broadcasts, as in the reference
-            tw = tw.expand(T)
-        if (w is not None and w.numel() != b) or (tw is not None and tw.numel() != T):
-            raise ValueError(f"weights must have {b} entries and task_weights 1 or {T}")
-        tw = None if tw is None else tw.contiguous()
-        loss = torch.empty(1, device=P.device)
-        dP = torch.empty_like(P)
-        getattr(K, name)(P, Y, w, tw, *args, loss, dP)
-        ctx.save_for_backward(dP.view(b, T, u))
-        ctx.pdtype = preds.dtype
-        return loss.reshape(())
-
-    @staticmethod
-    def backward(ctx, g):
-        (dP,) = ctx.saved_tensors
-        return (dP * g).to(ctx.pdtype), None, None, None, None, None
-
-
-class _Criterion(nn.Module):
-    """chemprop's `ChempropMetric` interface (nn/metrics.py:59-123) around one loss kernel: `task_weights` buffer (1 x T),
-    NaN targets or `mask` select the terms, `weights` are per molecule."""
-    _loss_fn = MSELossFunction
-
-    def __init__(self, task_weights):
-        super().__init__()
-        self.register_buffer("task_weights", torch.as_tensor(task_weights, dtype=torch.float).view(1, -1))
-
-    def forward(self, preds, targets, mask=None, weights=None, lt_mask=None, gt_mask=None):
-        if lt_mask is not None or gt_mask is not None:
-            raise NotImplementedError(f"{type(self).__name__} takes no lt_mask / gt_mask; the bounded criteria "
-                                      "(EngineBoundedMSE, EngineBoundedMAE, EngineBoundedRMSE) do")
-        return self._loss(preds, self._masked(targets, mask), weights)
-
-    @staticmethod
-    def _masked(targets, mask):
-        return targets if mask is None else torch.where(mask, targets, torch.full_like(targets, float("nan")))
-
-    def _loss(self, preds, targets, weights):
-        return self._loss_fn.apply(preds, targets, weights, self.task_weights)
-
-
-class _BCECriterion(_Criterion):
-    """chemprop's BCELoss (nn/metrics.py:291-294)."""
-    _loss_fn = BCELossFunction
-
-
-class _CrossEntropyCriterion(_Criterion):
-    """chemprop's CrossEntropyLoss (nn/metrics.py:297-303)."""
-    _loss_fn = CrossEntropyLossFunction
-
-
-class EngineMVELoss(_Criterion):
-    """chemprop's MVELoss (nn/metrics.py:202-219) on b x T x 2 (mean, var) predictions (dmpnn_mve_loss)."""
-
-    def __init__(self, task_weights=1.0):
-        super().__init__(task_weights)
-
-    def _loss(self, preds, targets, weights):
-        return UncertaintyLossFunction.apply(preds, targets, weights, self.task_weights, "mve_loss", ())
-
-
-class EngineEvidentialLoss(_Criterion):
-    """chemprop's EvidentialLoss (nn/metrics.py:222-260) on b x T x 4 (mean, v, alpha, beta) predictions
-    (dmpnn_evidential_loss)."""
-
-    def __init__(self, task_weights=1.0, v_kl: float = 0.2, eps: float = 1e-8):
-        super().__init__(task_weights)
-        self.v_kl = v_kl
-        self.eps = eps
-
-    def _loss(self, preds, targets, weights):
-        return UncertaintyLossFunction.apply(preds, targets, weights, self.task_weights, "evidential_loss",
-                                             (self.v_kl, self.eps))
-
-    def extra_repr(self) -> str:
-        return f"v_kl={self.v_kl}, eps={self.eps}"
-
-
-class EngineQuantileLoss(_Criterion):
-    """chemprop's QuantileLoss (nn/metrics.py:588-613) on b x T x 2 (mean, interval) predictions (dmpnn_quantile_loss); the
-    `bounds` and `tau` buffers are the reference's, so that its state dicts load strictly."""
-
-    def __init__(self, task_weights=1.0, alpha: float = 0.1):
-        super().__init__(task_weights)
-        self.alpha = alpha
-        self.register_buffer("bounds", torch.tensor([-1 / 2, 1 / 2]).view(-1, 1, 1))
-        self.register_buffer("tau", torch.tensor([[alpha / 2, 1 - alpha / 2], [alpha / 2 - 1, -alpha / 2]]).view(2, 2, 1, 1))
-
-    def _loss(self, preds, targets, weights):
-        return UncertaintyLossFunction.apply(preds, targets, weights, self.task_weights, "quantile_loss", (self.alpha,))
-
-    def extra_repr(self) -> str:
-        return f"alpha={self.alpha}"
-
-
-class EngineDirichletLoss(_Criterion):
-    """chemprop's DirichletLoss (nn/metrics.py:502-544) on b x T x C concentrations alpha and b x T class labels
-    (dmpnn_dirichlet_loss)."""
-
-    def __init__(self, task_weights=1.0, v_kl: float = 0.2):
-        super().__init__(task_weights)
-        self.v_kl = v_kl
-
-    def _loss(self, preds, targets, weights):
-        return UncertaintyLossFunction.apply(preds, targets, weights, self.task_weights, "dirichlet_loss",
-                                             (preds.shape[2], self.v_kl))
-
-    def extra_repr(self) -> str:
-        return f"v_kl={self.v_kl}"
-
-
 def _loss_weights(weights, task_weights, b: int, T: int):
     """Per-molecule and per-task weights as contiguous f32 vectors of exactly b and T entries (or None), as the kernels read
     them.  A 1-entry task weight (the criteria's default `task_weights=1.0`) broadcasts, as in the reference; any other size
@@ -466,29 +278,169 @@ def _loss_weights(weights, task_weights, b: int, T: int):
     return (None if w is None else w.contiguous()), (None if tw is None else tw.contiguous())
 
 
-class RegressionLossFunction(torch.autograd.Function):
-    """MSE / MAE / RMSE (_lib.LOSS_*) under the MSE criterion's reduction, optionally bounded by b x T lt / gt masks: loss
-    and dLoss/dPreds in one launch (dmpnn_regression_loss)."""
+class CriterionLossFunction(torch.autograd.Function):
+    """A criterion's loss and dLoss/dPreds in one launch, at any level.  `preds` is b x T, or b x T x u when `grouped` (u
+    values per task: class logits, the uncertainty predictors' outputs), and `targets` b x T.  `launch(P, Y, w, tw, lt, gt,
+    loss, dP)` (_Criterion._loss) gets them as b x (T*u) and b x T f32, the weights as exactly b and T entries
+    (_loss_weights) and the bound masks as b x T uint8 (None where not given); it writes loss[0] and dP."""
 
     @staticmethod
-    def forward(ctx, preds, targets, weights, task_weights, lt_mask, gt_mask, kind):
+    def forward(ctx, preds, targets, weights, task_weights, lt_mask, gt_mask, launch, grouped):
         K._require_cuda(preds, targets, lt_mask, gt_mask)
-        P, Y = preds.float().contiguous(), targets.float().contiguous()
-        if P.dim() != 2 or Y.shape != P.shape:
-            raise ValueError(f"preds and targets must both be b x T, got {tuple(P.shape)} and {tuple(Y.shape)}")
-        w, tw = _loss_weights(weights, task_weights, *P.shape)
-        lt, gt = (None if m is None else m.to(torch.uint8).expand(P.shape).contiguous() for m in (lt_mask, gt_mask))
+        if preds.dim() != (3 if grouped else 2) or targets.shape != preds.shape[:2]:
+            raise ValueError(f"expected {'b x T x u' if grouped else 'b x T'} predictions and b x T targets, got "
+                             f"{tuple(preds.shape)} and {tuple(targets.shape)}")
+        b, T = targets.shape
+        P, Y = preds.float().flatten(1).contiguous(), targets.float().contiguous()
+        w, tw = _loss_weights(weights, task_weights, b, T)
+        lt, gt = (None if m is None else m.to(torch.uint8).expand(b, T).contiguous() for m in (lt_mask, gt_mask))
         loss = torch.empty(1, device=P.device)
         dP = torch.empty_like(P)
-        K.regression_loss(P, Y, w, tw, lt, gt, kind, loss, dP)
-        ctx.save_for_backward(dP)
+        launch(P, Y, w, tw, lt, gt, loss, dP)
+        ctx.save_for_backward(dP.view(preds.shape))
         ctx.pdtype = preds.dtype
         return loss.reshape(())
 
     @staticmethod
     def backward(ctx, g):
         (dP,) = ctx.saved_tensors
-        return (dP * g).to(ctx.pdtype), None, None, None, None, None, None
+        return (dP * g).to(ctx.pdtype), None, None, None, None, None, None, None
+
+
+# the engine wrappers that take the b x T bound masks and a _lib.LOSS_* kind after `tw`
+_REGRESSION_WRAPPERS = ("regression_loss", "regression_loss_rows")
+
+
+class _Criterion(nn.Module):
+    """chemprop's `ChempropMetric` interface (nn/metrics.py:59-123) around one loss kernel: `task_weights` buffer (1 x T),
+    NaN targets or `mask` select the terms, `weights` are per molecule.  This class is chemprop's MSE.
+
+    Each criterion names its engine wrappers: `_kernel` for molecules (a single-block kernel of csrc/head.cu) and
+    `_row_kernel` for atom or bond rows (a row-parallel one of csrc/row_head.cu), None where it has none and `row_loss`
+    runs `forward`.  `_args(preds)` are the wrapper's arguments between `tw` and `loss`; the regression wrappers take the
+    bound masks and `_kind` there instead."""
+    _kernel = "mse_loss"
+    _row_kernel = "regression_loss_rows"
+    _kind = _lib.LOSS_MSE
+    _bounded = False                      # takes lt_mask / gt_mask (BoundedMixin, nn/metrics.py:142-149)
+    _grouped = False                      # b x T x u predictions
+
+    def __init__(self, task_weights):
+        super().__init__()
+        self.register_buffer("task_weights", torch.as_tensor(task_weights, dtype=torch.float).view(1, -1))
+
+    def forward(self, preds, targets, mask=None, weights=None, lt_mask=None, gt_mask=None):
+        return self._loss(self._kernel, preds, self._masked(targets, mask), weights, lt_mask, gt_mask)
+
+    def row_loss(self, preds, targets, weights=None, lt_mask=None, gt_mask=None):
+        """The criterion over atom or bond rows (`weights` per row, NaN targets masked) on `_row_kernel`, or through
+        `forward` where there is none."""
+        if self._row_kernel is None:
+            return self(preds, targets, None, weights, lt_mask, gt_mask)
+        return self._loss(self._row_kernel, preds, targets, weights, lt_mask, gt_mask)
+
+    @staticmethod
+    def _masked(targets, mask):
+        return targets if mask is None else torch.where(mask, targets, torch.full_like(targets, float("nan")))
+
+    def _args(self, preds) -> tuple:
+        return ()
+
+    def _loss(self, kernel, preds, targets, weights, lt_mask, gt_mask):
+        if not self._bounded and (lt_mask is not None or gt_mask is not None):
+            raise NotImplementedError(f"{type(self).__name__} takes no lt_mask / gt_mask; the bounded criteria "
+                                      "(EngineBoundedMSE, EngineBoundedMAE, EngineBoundedRMSE) do")
+        fn, regression = getattr(K, kernel), kernel in _REGRESSION_WRAPPERS
+
+        def launch(P, Y, w, tw, lt, gt, loss, dP):
+            fn(P, Y, w, tw, *((lt, gt, self._kind) if regression else self._args(preds)), loss, dP)
+
+        return CriterionLossFunction.apply(preds, targets, weights, self.task_weights, lt_mask, gt_mask, launch,
+                                           self._grouped)
+
+
+class _BCECriterion(_Criterion):
+    """chemprop's BCELoss (nn/metrics.py:291-294): soft labels allowed."""
+    _kernel = "bce_loss"
+    _row_kernel = "bce_loss_rows"
+
+
+class _CrossEntropyCriterion(_Criterion):
+    """chemprop's CrossEntropyLoss (nn/metrics.py:297-303) on b x T x C logits and b x T class labels (truncated like
+    `targets.long()`)."""
+    _kernel = "ce_loss"
+    _row_kernel = "ce_loss_rows"
+    _grouped = True
+
+    def _args(self, preds) -> tuple:
+        return (preds.shape[2],)
+
+
+class EngineMVELoss(_Criterion):
+    """chemprop's MVELoss (nn/metrics.py:202-219) on b x T x 2 (mean, var) predictions (dmpnn_mve_loss)."""
+    _kernel = "mve_loss"
+    _row_kernel = None
+    _grouped = True
+
+    def __init__(self, task_weights=1.0):
+        super().__init__(task_weights)
+
+
+class EngineEvidentialLoss(_Criterion):
+    """chemprop's EvidentialLoss (nn/metrics.py:222-260) on b x T x 4 (mean, v, alpha, beta) predictions
+    (dmpnn_evidential_loss)."""
+    _kernel = "evidential_loss"
+    _row_kernel = None
+    _grouped = True
+
+    def __init__(self, task_weights=1.0, v_kl: float = 0.2, eps: float = 1e-8):
+        super().__init__(task_weights)
+        self.v_kl = v_kl
+        self.eps = eps
+
+    def _args(self, preds) -> tuple:
+        return self.v_kl, self.eps
+
+    def extra_repr(self) -> str:
+        return f"v_kl={self.v_kl}, eps={self.eps}"
+
+
+class EngineQuantileLoss(_Criterion):
+    """chemprop's QuantileLoss (nn/metrics.py:588-613) on b x T x 2 (mean, interval) predictions (dmpnn_quantile_loss); the
+    `bounds` and `tau` buffers are the reference's, so that its state dicts load strictly."""
+    _kernel = "quantile_loss"
+    _row_kernel = None
+    _grouped = True
+
+    def __init__(self, task_weights=1.0, alpha: float = 0.1):
+        super().__init__(task_weights)
+        self.alpha = alpha
+        self.register_buffer("bounds", torch.tensor([-1 / 2, 1 / 2]).view(-1, 1, 1))
+        self.register_buffer("tau", torch.tensor([[alpha / 2, 1 - alpha / 2], [alpha / 2 - 1, -alpha / 2]]).view(2, 2, 1, 1))
+
+    def _args(self, preds) -> tuple:
+        return (self.alpha,)
+
+    def extra_repr(self) -> str:
+        return f"alpha={self.alpha}"
+
+
+class EngineDirichletLoss(_Criterion):
+    """chemprop's DirichletLoss (nn/metrics.py:502-544) on b x T x C concentrations alpha and b x T class labels
+    (dmpnn_dirichlet_loss)."""
+    _kernel = "dirichlet_loss"
+    _row_kernel = None
+    _grouped = True
+
+    def __init__(self, task_weights=1.0, v_kl: float = 0.2):
+        super().__init__(task_weights)
+        self.v_kl = v_kl
+
+    def _args(self, preds) -> tuple:
+        return preds.shape[2], self.v_kl
+
+    def extra_repr(self) -> str:
+        return f"v_kl={self.v_kl}"
 
 
 class SpectralTransformFunction(torch.autograd.Function):
@@ -514,47 +466,13 @@ class SpectralTransformFunction(torch.autograd.Function):
         return dX.to(dt), None
 
 
-class SpectralLossFunction(torch.autograd.Function):
-    """SID or Wasserstein (engine.sid_loss / engine.wasserstein_loss) on b x T spectra under the MSE criterion's
-    reduction: loss and dLoss/dPreds from dmpnn_sid_loss / dmpnn_wasserstein_loss."""
-
-    @staticmethod
-    def forward(ctx, preds, targets, weights, task_weights, name, threshold):
-        K._require_cuda(preds, targets)
-        P, Y = preds.float().contiguous(), targets.float().contiguous()
-        if P.dim() != 2 or Y.shape != P.shape:
-            raise ValueError(f"preds and targets must both be b x T, got {tuple(P.shape)} and {tuple(Y.shape)}")
-        w, tw = _loss_weights(weights, task_weights, *P.shape)
-        loss = torch.empty(1, device=P.device)
-        dP = torch.empty_like(P)
-        getattr(K, name)(P, Y, w, tw, threshold, loss, dP)
-        ctx.save_for_backward(dP)
-        ctx.pdtype = preds.dtype
-        return loss.reshape(())
-
-    @staticmethod
-    def backward(ctx, g):
-        (dP,) = ctx.saved_tensors
-        return (dP * g).to(ctx.pdtype), None, None, None, None, None
-
-
 class _RegressionCriterion(_Criterion):
     """MSE / MAE / RMSE (`_kind`, _lib.LOSS_*) on b x T predictions, one launch of dmpnn_regression_loss; the `_bounded`
     ones take the batch's `lt_mask` / `gt_mask` (BoundedMixin, nn/metrics.py:142-149), the others refuse them."""
-    _kind = _lib.LOSS_MSE
-    _bounded = False
+    _kernel = "regression_loss"
 
     def __init__(self, task_weights=1.0):
         super().__init__(task_weights)
-
-    def forward(self, preds, targets, mask=None, weights=None, lt_mask=None, gt_mask=None):
-        if not self._bounded:
-            return super().forward(preds, targets, mask, weights, lt_mask, gt_mask)
-        return RegressionLossFunction.apply(preds, self._masked(targets, mask), weights, self.task_weights, lt_mask, gt_mask,
-                                            self._kind)
-
-    def _loss(self, preds, targets, weights):
-        return RegressionLossFunction.apply(preds, targets, weights, self.task_weights, None, None, self._kind)
 
 
 class EngineMAE(_RegressionCriterion):
@@ -589,14 +507,15 @@ class EngineBoundedRMSE(_RegressionCriterion):
 class EngineSID(_Criterion):
     """chemprop's SID (nn/metrics.py:547-566) on b x T spectra: predictions clamped at `threshold` (None: not clamped),
     normalised over the masked-in bins, symmetric KL against the targets (dmpnn_sid_loss)."""
-    _name = "sid_loss"
+    _kernel = "sid_loss"
+    _row_kernel = None
 
     def __init__(self, task_weights=1.0, threshold: float | None = None):
         super().__init__(task_weights)
         self.threshold = threshold
 
-    def _loss(self, preds, targets, weights):
-        return SpectralLossFunction.apply(preds, targets, weights, self.task_weights, self._name, self.threshold)
+    def _args(self, preds) -> tuple:
+        return (self.threshold,)
 
     def extra_repr(self) -> str:
         return f"threshold={self.threshold}"
@@ -608,7 +527,7 @@ class EngineWasserstein(EngineSID):
     the reference's `MPNN.training_step`, whose criterion sees `targets.nan_to_num(0)`.  Called directly with a `mask` and
     finite targets at the masked bins, the reference criterion would add those targets to its cumsum instead; the engine
     does not read them."""
-    _name = "wasserstein_loss"
+    _kernel = "wasserstein_loss"
 
 
 class _EngineFFNPredictor(nn.Module):

@@ -8,9 +8,10 @@ reverse-edge pair, atom and bond constraints, and the sum of the per-level crite
 - The pair mean `(P[2i] + P[2i+1]) / 2` is dmpnn_edge_pair_mean (NaN rows where edge 2i+1 is not the reverse of edge 2i),
   applied by the model to the bond predictor's output and, through `_EdgePairMeanMLP`, to the bond constrainer's MLP
   output, as the reference's wrappers do.
-- Atom- and bond-level criteria: MSE, MAE, RMSE and their bounded variants, BCE and cross-entropy run on the row-parallel
-  kernels (dmpnn_regression_loss_rows, dmpnn_bce_loss_rows, dmpnn_ce_loss_rows); any other engine criterion runs on its
-  own kernel.  The molecule level calls its predictor's criterion, as EngineMPNN does.
+- Atom- and bond-level criteria: each engine criterion's `row_loss`, which runs the row-parallel kernel the criterion
+  names (dmpnn_regression_loss_rows for MSE, MAE, RMSE and their bounded variants, dmpnn_bce_loss_rows,
+  dmpnn_ce_loss_rows), or its own kernel where it names none.  The molecule level, and any criterion that is not an engine
+  criterion, is called as a module, as EngineMPNN does.
 - No host synchronisation: a training step, with or without atom and bond constraints, captures into CudaGraphStep.  The
   constrainers get the molecules' atom and bond offsets from the layout and decide on the device which constraint columns
   are set (ConstrainerFFN, dmpnn_constrain_fwd / _bwd); the constraints are inputs of the graph like the targets.
@@ -22,10 +23,8 @@ from __future__ import annotations
 import torch
 from torch import Tensor, nn
 
-from .. import _lib
 from .. import engine as K
-from .head import (EdgePairOperand, _BCECriterion, _Criterion, _CrossEntropyCriterion, _loss_weights,
-                   _RegressionCriterion, EngineBatchNorm1d, engine_mlp)
+from .head import EdgePairOperand, _Criterion, EngineBatchNorm1d, engine_mlp
 
 _LEVELS = ("mol", "atom", "bond")
 
@@ -56,62 +55,6 @@ class EdgePairMeanFunction(torch.autograd.Function):
         if E > 0 and G.shape[1] > 0:
             K.edge_pair_mean_bwd(G, dP)
         return dP.view(shape).to(dt), None
-
-
-class RowLossFunction(torch.autograd.Function):
-    """The atom- and bond-level criteria on R x T predictions (R x T x C logits for cross-entropy): loss and dLoss/dPreds
-    from the row-parallel kernels -- `which` "regression" (kind _lib.LOSS_*, optional lt / gt masks), "bce" or "ce"."""
-
-    @staticmethod
-    def forward(ctx, preds, targets, weights, task_weights, lt_mask, gt_mask, kind, which):
-        K._require_cuda(preds, targets, lt_mask, gt_mask)
-        R = preds.shape[0]
-        P = preds.float().reshape(R, -1).contiguous()
-        Y = targets.float().reshape(R, -1).contiguous()
-        T = Y.shape[1]
-        if (which == "ce" and (preds.dim() != 3 or preds.shape[1] != T)) or (which != "ce" and P.shape != Y.shape):
-            raise ValueError(f"predictions {tuple(preds.shape)} do not match targets {tuple(targets.shape)}")
-        w, tw = _loss_weights(weights, task_weights, R, T)
-        loss = torch.empty(1, device=P.device)
-        dP = torch.empty_like(P)
-        if which == "regression":
-            lt, gt = (None if m is None else m.to(torch.uint8).reshape(R, -1).expand(R, T).contiguous()
-                      for m in (lt_mask, gt_mask))
-            K.regression_loss_rows(P, Y, w, tw, lt, gt, kind, loss, dP)
-        elif which == "bce":
-            K.bce_loss_rows(P, Y, w, tw, loss, dP)
-        else:
-            K.ce_loss_rows(P, Y, w, tw, preds.shape[2], loss, dP)
-        ctx.save_for_backward(dP.view(preds.shape))
-        ctx.pdtype = preds.dtype
-        return loss.reshape(())
-
-    @staticmethod
-    def backward(ctx, g):
-        (dP,) = ctx.saved_tensors
-        return (dP * g).to(ctx.pdtype), None, None, None, None, None, None, None
-
-
-def row_criterion_loss(criterion: nn.Module, preds: Tensor, targets: Tensor, weights: Tensor | None = None,
-                       lt_mask: Tensor | None = None, gt_mask: Tensor | None = None) -> Tensor:
-    """`criterion(preds, targets, isfinite(targets), weights, lt_mask, gt_mask)` over atom or bond rows: the MSE / MAE /
-    RMSE family (bounded or not), BCE and cross-entropy on the row-parallel kernels, any other criterion on its own."""
-    bounded = getattr(criterion, "_bounded", False)
-    masks = lt_mask is not None or gt_mask is not None
-    which = None
-    if type(criterion) is _Criterion or isinstance(criterion, _RegressionCriterion):
-        which = "regression"
-    elif type(criterion) is _BCECriterion:
-        which = "bce"
-    elif type(criterion) is _CrossEntropyCriterion:
-        which = "ce"
-    if which is None:
-        return criterion(preds, targets, None, weights, lt_mask, gt_mask) if masks else criterion(preds, targets, None, weights)
-    if masks and not bounded:
-        raise NotImplementedError(f"{type(criterion).__name__} takes no lt_mask / gt_mask; the bounded criteria "
-                                  "(EngineBoundedMSE, EngineBoundedMAE, EngineBoundedRMSE) do")
-    kind = getattr(criterion, "_kind", _lib.LOSS_MSE)
-    return RowLossFunction.apply(preds, targets, weights, criterion.task_weights, lt_mask, gt_mask, kind, which)
 
 
 class _EdgePairMeanMLP(nn.Sequential):
@@ -239,15 +182,14 @@ class EngineMolAtomBondMPNN(nn.Module):
         for level, (predictor, preds) in enumerate(zip(self.predictors, predss)):
             if predictor is None:
                 continue
-            targets = targetss[level]
+            crit = predictor.criterion
             weights = None if weightss is None else weightss[level]
             lt = None if lt_masks is None else lt_masks[level]
             gt = None if gt_masks is None else gt_masks[level]
-            if level == 0:
-                crit = predictor.criterion
-                l = crit(preds, targets, None, weights) if lt is None and gt is None else crit(preds, targets, None, weights,
-                                                                                               lt, gt)
+            masks = () if lt is None and gt is None else (lt, gt)
+            if level > 0 and isinstance(crit, _Criterion):
+                l = crit.row_loss(preds, targetss[level], weights, *masks)
             else:
-                l = row_criterion_loss(predictor.criterion, preds, targets, weights, lt, gt)
+                l = crit(preds, targetss[level], None, weights, *masks)
             total = l if total is None else total + l
         return total

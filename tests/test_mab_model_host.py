@@ -384,13 +384,14 @@ def test_pair_mean_refuses_odd_edge_counts_and_marks_unpaired_rows(monkeypatch):
     assert torch.isnan(out[:2]).all() and torch.isfinite(out[2]).all()
 
 
-def test_non_bounded_criteria_refuse_masks_at_row_level(monkeypatch):
+def test_row_loss_refuses_masks_for_non_bounded_criteria(monkeypatch):
+    """`_Criterion.row_loss`, which EngineMolAtomBondMPNN calls at atom and bond level, refuses lt_mask / gt_mask for a
+    criterion that is not bounded, and takes them for a bounded one."""
     import chemprop_b200.nn as N
-    from chemprop_b200.nn.mol_atom_bond_model import row_criterion_loss
 
     patch_mab_model(monkeypatch)
     P, Y = torch.randn(8, 2), torch.randn(8, 2)
     m = torch.zeros(8, 2, dtype=torch.bool)
     with pytest.raises(NotImplementedError):
-        row_criterion_loss(N.EngineMAE(torch.ones(2)), P, Y, None, m, m)
-    assert torch.isfinite(row_criterion_loss(N.EngineBoundedMAE(torch.ones(2)), P, Y, None, m, m))
+        N.EngineMAE(torch.ones(2)).row_loss(P, Y, None, m, m)
+    assert torch.isfinite(N.EngineBoundedMAE(torch.ones(2)).row_loss(P, Y, None, m, m))

@@ -57,7 +57,7 @@ def main():
     from chemprop_b200.data import BatchMolGraph, make_molecules
     from chemprop_b200.graph import CudaGraphStep
     from chemprop_b200.nn.head import EdgePairOperand, PairLinearFunction
-    from chemprop_b200.nn.mol_atom_bond_model import EdgePairMeanFunction, row_criterion_loss
+    from chemprop_b200.nn.mol_atom_bond_model import EdgePairMeanFunction
 
     dev = "cuda"
     torch.manual_seed(0)
@@ -80,11 +80,11 @@ def main():
         mol.criterion(mol.train_step(Hg), Yg).backward()
 
     def atom_head():
-        row_criterion_loss(atom.criterion, atom.train_step(Hv), Yv).backward()
+        atom.criterion.row_loss(atom.train_step(Hv), Yv).backward()
 
     def bond_head():
         P = EdgePairMeanFunction.apply(bond.train_step(EdgePairOperand(He, rev)), rev)
-        row_criterion_loss(bond.criterion, P, Ye).backward()
+        bond.criterion.row_loss(P, Ye).backward()
 
     res["head_fwd_bwd_ms"] = {"mol": t(mol_head), "atom": t(atom_head), "bond": t(bond_head)}
     W, b = bond.ffn[0][0].weight, bond.ffn[0][0].bias
