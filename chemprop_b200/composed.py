@@ -297,7 +297,10 @@ def edge_readout(mp, W_eo, E, H, lay) -> Tensor:
     """dropout(tau(W_eo([E || H]))) per directed edge, in the CALLER's edge order
     (chemprop/nn/message_passing/mol_atom_bond.py `edge_finalize`)."""
     Hc = PermuteRows.apply(H, lay.inv_perm, lay.perm)          # internal row of caller edge e is inv_perm[e]
-    Y = GatherLinear.apply(E, None, Hc, None, W_eo.weight, W_eo.bias, None, lay.E)
+    if E.shape[1] == 0:    # no bond features: [E || H] is H (the linear kernels take no zero-width first operand)
+        Y = GatherLinear.apply(Hc, None, None, None, W_eo.weight, W_eo.bias, None, lay.E)
+    else:
+        Y = GatherLinear.apply(E, None, Hc, None, W_eo.weight, W_eo.bias, None, lay.E)
     return mp.dropout(mp.tau(Y))
 
 

@@ -170,24 +170,36 @@ def message_passing_forward(kind, V, E, edge_index, rev_edge_index, W_i, b_i, W_
 
 def mab_forward(kind, V, E, edge_index, rev_edge_index, W_i, b_i, W_h, b_h, W_vo, b_vo, W_eo, b_eo, depth, act="relu",
                 undirected=False, V_d=None, W_vd=None, b_vd=None, E_d=None, W_ed=None, b_ed=None, prelu_weight=None,
-                return_vertex=True, return_edge=True):
+                return_vertex=True, return_edge=True, dropout_masks=None, act_param=None):
     """_MABMessagePassingBase.forward (chemprop/nn/message_passing/mol_atom_bond.py): the loop of base.py:196-206,
     then vertex_finalize (same as `finalize`) and edge_finalize: tau(W_eo([E || H])) [-> W_ed([. || E_d])] per directed
-    edge.  kind in {"bond", "atom"}.  Returns (H_v | None, H_e | None)."""
-    tau = activation(act, prelu_weight)
+    edge.  kind in {"bond", "atom"}.  Returns (H_v | None, H_e | None).
+    `dropout_masks`: training-mode dropout with the masks given explicitly, already scaled (0 or 1/(1-p)), in the order
+    the reference draws them: one E x h mask per depth step, then vertex_finalize's (after W_vo, after W_vd) when the vertex
+    read-out exists, then edge_finalize's (after W_eo, after W_ed) when the edge read-out does.
+    `act_param`: the LeakyReLU slope / ELU alpha when `act` is a name."""
+    tau = activation(act, prelu_weight, act_param)
+    masks = list(dropout_masks) if dropout_masks is not None else None
+    loop_masks = None
+    if masks is not None:
+        n = max(depth - 1, 0) + ((1 + (V_d is not None)) if W_vo is not None else 0)
+        # without a vertex read-out the dummy one below still consumes a mask: a scalar one
+        loop_masks, masks = masks[:n] + ([] if W_vo is not None else [torch.ones((), dtype=V.dtype, device=V.device)]), masks[n:]
     if W_vo is None:   # edge embeddings only: the vertex read-out does not exist; run the loop with a dummy W_o
-        W_vo_, b_vo_ = torch.zeros(1, V.shape[1] + W_h.shape[0], dtype=V.dtype), None
+        W_vo_, b_vo_ = torch.zeros(1, V.shape[1] + W_h.shape[0], dtype=V.dtype, device=V.device), None
     else:
         W_vo_, b_vo_ = W_vo, b_vo
     H_v, inter = message_passing_forward(kind, V, E, edge_index, rev_edge_index, W_i, b_i, W_h, b_h, W_vo_, b_vo_, depth,
                                          act, undirected, V_d if W_vo is not None else None, W_vd, b_vd,
-                                         return_intermediates=True, prelu_weight=prelu_weight)
+                                         return_intermediates=True, prelu_weight=prelu_weight, dropout_masks=loop_masks,
+                                         act_param=act_param)
     H = inter["H"][-1]
     H_e = None
     if return_edge:
-        H_e = tau(F.linear(torch.cat((E, H), dim=1), W_eo, b_eo))
+        dropout = _no_dropout if masks is None else (lambda X: X * masks.pop(0))
+        H_e = dropout(tau(F.linear(torch.cat((E, H), dim=1), W_eo, b_eo)))
         if E_d is not None:
-            H_e = F.linear(torch.cat((H_e, E_d), dim=1), W_ed, b_ed)
+            H_e = dropout(F.linear(torch.cat((H_e, E_d), dim=1), W_ed, b_ed))
     return (H_v if (return_vertex and W_vo is not None) else None), H_e
 
 

@@ -65,7 +65,7 @@ def _cat(X1, K1, idx1, X2, K2, idx2, R):
 def linear_fwd(X1, K1, W, out, N, *, idx1=None, X2=None, K2=0, idx2=None, bias=None, res=None, act=ACT_NONE,
                act_param=0.0, R=None, pad_to=None):
     R = out.shape[0] if R is None else R
-    assert W.shape == (N, K1 + K2) and (K2 == 0 or X2 is not None) and out.shape[1] >= N
+    assert K1 > 0 and W.shape == (N, K1 + K2) and (K2 == 0 or X2 is not None) and out.shape[1] >= N   # "bad sizes"
     Y = _cat(X1, K1, idx1, X2, K2, idx2, R) @ W.float().t()
     if bias is not None:
         Y = Y + bias.float()
@@ -79,6 +79,7 @@ def linear_fwd(X1, K1, W, out, N, *, idx1=None, X2=None, K2=0, idx2=None, bias=N
 
 def linear_wgrad(dY, X1, K1, dW, N, *, idx1=None, X2=None, K2=0, idx2=None, dbias=None, accumulate=False, R=None):
     R = dY.shape[0] if R is None else R
+    assert K1 > 0                                                    # "bad sizes"
     g = dY[:R, :N].float()
     upd = g.t() @ _cat(X1, K1, idx1, X2, K2, idx2, R)
     if accumulate:

@@ -141,11 +141,11 @@ def case_dims(c: dict) -> tuple:
     return c.get("dims", (72, 14))
 
 
-def molecules(c: dict, seed: int) -> list:
-    """The batch of case `c`, shuffled edge and molecule order.  "mixed": N_MOLS molecules of ~25 atoms, 20 of 66-200 atoms (more
+def molecules(c: dict, seed: int, n_mols: int = N_MOLS) -> list:
+    """The batch of case `c`, shuffled edge and molecule order.  "mixed": n_mols molecules of ~25 atoms, 20 of 66-200 atoms (more
     than 128 directed edges: the fused step's 128-row windows), and two copies of each K_6 .. K_12 (in-degree up to 11);
     "windows": the same without the K_k; "oversized": mixed plus one molecule of 130-140 atoms (more than an atom tile);
-    "edgeless": N_MOLS single atoms (its bf16 cases use tanh: with ReLU, a kink flip of one single-atom molecule
+    "edgeless": n_mols single atoms (its bf16 cases use tanh: with ReLU, a kink flip of one single-atom molecule
     moves the W_o gradient by 8 % of its scale).
 
     The K_k stay out of the tanh cases of the bf16 tier and of the deepest ones (depth 5 and 6): on a K_k every step multiplies a perturbation of H by
@@ -160,8 +160,8 @@ def molecules(c: dict, seed: int) -> list:
     rng = np.random.default_rng(seed)
     batch = c.get("batch", "mixed")
     if batch == "edgeless":
-        return [make_molecule(rng, 1, d_v, d_e) for _ in range(N_MOLS)]
-    mgs = make_molecules(N_MOLS, seed=seed, d_v=d_v, d_e=d_e, shuffle_edges=True)
+        return [make_molecule(rng, 1, d_v, d_e) for _ in range(n_mols)]
+    mgs = make_molecules(n_mols, seed=seed, d_v=d_v, d_e=d_e, shuffle_edges=True)
     big = 200 if c["kind"] == "bond" else 128        # an atom tile holds 128 atoms: larger is the "oversized" batch
     mgs += make_molecules(20, seed=seed + 1, mean_atoms=110.0, std_atoms=40.0, min_atoms=66, max_atoms=big, d_v=d_v, d_e=d_e,
                           shuffle_edges=True)
@@ -173,11 +173,11 @@ def molecules(c: dict, seed: int) -> list:
     return [mgs[i] for i in rng.permutation(len(mgs))]
 
 
-def _check_batch(c: dict, lay):
+def _check_batch(c: dict, lay, n_mols: int = N_MOLS):
     """The batch really has what the case is for, whatever the generators do."""
     batch = c.get("batch", "mixed")
     if batch == "edgeless":
-        assert lay.E == 0 and lay.V == N_MOLS
+        assert lay.E == 0 and lay.V == n_mols
         return
     assert (lay.max_indeg > 4) == (batch != "windows"), lay.max_indeg
     if c["kind"] == "bond":
