@@ -272,13 +272,50 @@ def collate_batch(batch: Iterable[Datum], pack_tiles: bool = False) -> TrainingB
     if pack_tiles and len(batch) > 1:
         order = tile_packing_order_of([d[0] for d in batch])
         batch = [batch[i] for i in order]
-    mgs, V_ds, x_ds, ys, weights, lt_masks, gt_masks = zip(*batch)
-    return TrainingBatch(
-        BatchMolGraph(mgs),
-        None if V_ds[0] is None else torch.from_numpy(np.concatenate(V_ds)).float(),
+    mgs, V_ds, *rest = zip(*batch)
+    return TrainingBatch(BatchMolGraph(mgs), _cat_V_d(V_ds), *_molecule_tensors(*rest))
+
+
+def _cat_V_d(V_ds) -> Tensor | None:
+    return None if V_ds[0] is None else torch.from_numpy(np.concatenate(V_ds)).float()
+
+
+def _molecule_tensors(x_ds, ys, weights, lt_masks, gt_masks) -> tuple:
+    """X_d, Y, w, lt_mask, gt_mask of a batch (chemprop/data/collate.py:90-96)."""
+    return (
         None if x_ds[0] is None else torch.from_numpy(np.array(x_ds)).float(),
         None if ys[0] is None else torch.from_numpy(np.array(ys)).float(),
         torch.tensor(weights, dtype=torch.float).unsqueeze(1),
         None if lt_masks[0] is None else torch.from_numpy(np.array(lt_masks)),
         None if gt_masks[0] is None else torch.from_numpy(np.array(gt_masks)),
     )
+
+
+class MulticomponentTrainingBatch(NamedTuple):
+    """chemprop/data/collate.py:186-193.  `bmgs`: one batch per component, or ONE union batch (see
+    `collate_multicomponent`); `V_ds` accordingly a list per component or one tensor in union atom order."""
+    bmgs: list[BatchMolGraph] | BatchMolGraph
+    V_ds: list[Tensor | None] | Tensor | None
+    X_d: Tensor | None
+    Y: Tensor | None
+    w: Tensor
+    lt_mask: Tensor | None
+    gt_mask: Tensor | None
+
+
+def collate_multicomponent(batches: Iterable[Sequence[Datum]], union: bool = False) -> MulticomponentTrainingBatch:
+    """chemprop/data/collate.py:196-208: `batches` holds one sequence of N Datums (one per component) per data point.
+    `union=False`: one BatchMolGraph per component, as the reference.  `union=True`: ONE BatchMolGraph of all N * b
+    molecules in datapoint-major interleaved order -- union molecule m * N + c is component c of data point m -- with its
+    host layout meta words (graph-capturable), for a shared encoder (EngineMulticomponentMPNN); its `V_ds` is one tensor
+    in union atom order (None when component 0 has none).  X_d, Y, weights and masks come from component 0, as in the
+    reference."""
+    batches = [list(dp) for dp in batches]
+    comps = list(zip(*batches))
+    head = _molecule_tensors(*list(zip(*comps[0]))[2:])
+    if not union:
+        tbs = [collate_batch(batch) for batch in comps]
+        return MulticomponentTrainingBatch([tb.bmg for tb in tbs], [tb.V_d for tb in tbs], *head)
+    union_data = [d for dp in batches for d in dp]
+    V_ds = None if comps[0][0].V_d is None else _cat_V_d([d.V_d for d in union_data])
+    return MulticomponentTrainingBatch(BatchMolGraph([d.mg for d in union_data]), V_ds, *head)

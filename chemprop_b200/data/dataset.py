@@ -142,6 +142,14 @@ class PackedMolGraphDataset:
         d = np.diff(self._atom_ptr_h)
         return d if ids is None else d[np.asarray(ids, dtype=np.int64)]
 
+    def n_edges(self, ids=None) -> np.ndarray:
+        d = np.diff(self._edge_ptr_h)
+        return d if ids is None else d[np.asarray(ids, dtype=np.int64)]
+
+    def host_buffer(self, pin_memory: bool = False, compact: bool = False) -> HostBatchBuffer:
+        """Staging memory for `batch(ids, buffer=...)` of this data set."""
+        return HostBatchBuffer(self.d_v, self.d_e, pin_memory=pin_memory, compact=compact)
+
     def to(self, device, non_blocking: bool = False) -> "PackedMolGraphDataset":
         """A copy of the data set on `device` (the six arrays; a few GB per million molecules)."""
         dev = torch.device(device)
@@ -157,13 +165,29 @@ class PackedMolGraphDataset:
             raise ValueError("k >= 1")
         if k == 1:
             return self
-        ap, ep = torch.from_numpy(self._atom_ptr_h), torch.from_numpy(self._edge_ptr_h)
-        Vt, Et = int(ap[-1]), int(ep[-1])
-        dev = self.device
-        rep_ptr = lambda p, tot: torch.cat([p[:-1] + j * tot for j in range(k)] + [torch.tensor([k * tot], dtype=torch.int64)])  # noqa: E731
-        return PackedMolGraphDataset(self.V_all.repeat(k, 1), self.E_all.repeat(k, 1), self.ei_local.repeat(1, k),
-                                     self.rev_local.repeat(k), rep_ptr(ap, Vt).to(dev), rep_ptr(ep, Et).to(dev),
-                                     np.tile(self._max_indeg_h, k))
+        return PackedMolGraphDataset.concatenate([self] * k)
+
+    @classmethod
+    def concatenate(cls, datasets: Sequence["PackedMolGraphDataset"]) -> "PackedMolGraphDataset":
+        """One data set holding the molecules of `datasets` one after the other (molecule i of datasets[j] is molecule
+        i + sum_{j' < j} len(datasets[j'])); the feature widths and the device must agree."""
+        if not datasets:
+            raise ValueError("nothing to concatenate")
+        d0 = datasets[0]
+        if any((d.d_v, d.d_e, d.device) != (d0.d_v, d0.d_e, d0.device) for d in datasets):
+            raise ValueError("data sets of different feature widths or devices cannot be concatenated")
+
+        def cat_ptr(ptrs):
+            out, base = [], 0
+            for p in ptrs:
+                out.append(torch.from_numpy(p[:-1] + base))
+                base += int(p[-1])
+            return torch.cat(out + [torch.tensor([base], dtype=torch.int64)]).to(d0.device)
+
+        return cls(torch.cat([d.V_all for d in datasets]), torch.cat([d.E_all for d in datasets]),
+                   torch.cat([d.ei_local for d in datasets], 1), torch.cat([d.rev_local for d in datasets]),
+                   cat_ptr([d._atom_ptr_h for d in datasets]), cat_ptr([d._edge_ptr_h for d in datasets]),
+                   np.concatenate([d._max_indeg_h for d in datasets]))
 
     def molgraph(self, i: int) -> MolGraph:
         """Molecule `i` as a MolGraph (host data sets; for inspection and tests)."""
@@ -253,3 +277,84 @@ class PackedMolGraphDataset:
         bmg._xfer = xf
         bmg._meta_host = meta
         return bmg
+
+
+class MulticomponentPackedDataset:
+    """N aligned `PackedMolGraphDataset`s (component c of data point m is molecule m of `datasets[c]`) behind the interface
+    `PackedBatchLoader` draws from, so that the loader's samplers, sharding, `drop_last` rule, `arrays` / `extras`,
+    prefetching and host / HBM-resident modes apply unchanged; ids are DATA POINT ids.
+
+      * `union=True` (shared encoder; the components must agree in d_v / d_e): the components are stacked once, component c
+        of data point m being packed molecule c * n + m, and `batch(ids)` is ONE union BatchMolGraph in datapoint-major
+        interleaved order (union molecule k * N + c is component c of ids[k]) -- one `dmpnn_dataset_gather` (or its host
+        twin) over the expanded ids [m_0, n + m_0, ..., m_1, n + m_1, ...], its layout meta words planned on the host.  Only
+        the stacked copy is kept (the given data sets are not referenced), so the features are held once.
+      * `union=False`: `batch(ids)` is the list of the N components' batches of the same ids.
+
+    `packed_order(ids)` orders data points by their summed sizes (`tile_packing_order`); each data point's molecules then
+    stay together, in component order."""
+
+    def __init__(self, datasets: Sequence[PackedMolGraphDataset], union: bool = False):
+        datasets = list(datasets)
+        if not datasets:
+            raise ValueError("no components")
+        n = len(datasets[0])
+        if any(len(d) != n for d in datasets):
+            raise ValueError("the components' data sets must have one molecule per data point each (equal lengths)")
+        if len({d.device for d in datasets}) != 1:
+            raise ValueError("the components' data sets must live on one device")
+        self.union, self._n, self._N = bool(union), n, len(datasets)
+        # per data point, the atoms and edges of all its components (host arrays: the tile-packing order)
+        self._atoms = sum(d.n_atoms() for d in datasets)
+        self._edges = sum(d.n_edges() for d in datasets)
+        self.components = None if self.union else datasets
+        self.stacked = PackedMolGraphDataset.concatenate(datasets) if self.union else None
+
+    def __len__(self) -> int:
+        return self._n
+
+    @property
+    def n_components(self) -> int:
+        return self._N
+
+    @property
+    def device(self) -> torch.device:
+        return self.stacked.device if self.union else self.components[0].device
+
+    def to(self, device, non_blocking: bool = False) -> "MulticomponentPackedDataset":
+        out = object.__new__(MulticomponentPackedDataset)
+        out.__dict__.update(self.__dict__)
+        if self.union:
+            out.stacked = self.stacked.to(device, non_blocking)
+        else:
+            out.components = [d.to(device, non_blocking) for d in self.components]
+        return out
+
+    def union_ids(self, ids) -> np.ndarray:
+        """The packed molecule ids of the union batch of data points `ids`: [m_0, n + m_0, ..., m_1, n + m_1, ...]."""
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        return (ids[:, None] + self._n * np.arange(self._N, dtype=np.int64)[None, :]).reshape(-1)
+
+    def packed_order(self, ids) -> np.ndarray:
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        return ids[tile_packing_order(self._atoms[ids], self._edges[ids])]
+
+    def plan(self, ids):
+        if self.union:
+            return self.stacked.plan(self.union_ids(ids))
+        return [d.plan(ids) for d in self.components]
+
+    def host_buffer(self, pin_memory: bool = False, compact: bool = False):
+        if self.union:
+            return self.stacked.host_buffer(pin_memory, compact)
+        return [d.host_buffer(pin_memory, compact) for d in self.components]
+
+    def batch(self, ids, pin_memory: bool = False, transfer_dtype: torch.dtype | None = None, buffer=None,
+              n_threads: int = 0, plan=None):
+        """The union BatchMolGraph of data points `ids` (union=True), or the list of the components' BatchMolGraphs."""
+        kw = dict(pin_memory=pin_memory, transfer_dtype=transfer_dtype, n_threads=n_threads)
+        if self.union:
+            return self.stacked.batch(self.union_ids(ids), buffer=buffer, plan=plan, **kw)
+        buffers = [None] * self._N if buffer is None else buffer
+        plans = [None] * self._N if plan is None else plan
+        return [d.batch(ids, buffer=b, plan=p, **kw) for d, b, p in zip(self.components, buffers, plans)]

@@ -17,6 +17,9 @@ on top of a `PackedMolGraphDataset`:
     engine's 128-row tiles come out ~0.94 full instead of ~0.81 (the fused depth step costs the same per tile whatever its
     fill); batch membership is the sampler's, `LoadedBatch.ids` / `extras` follow the order used.
 
+A `MulticomponentPackedDataset` is drawn from the same way, by data point: each batch is one union BatchMolGraph of its
+data points' components in interleaved order (`union=True`) or the list of the components' batches of the same ids.
+
 Per-molecule side arrays (`Y`, `weights`, `X_d`, ... -- anything indexed by molecule) given as `arrays={name: ndarray}`
 come back gathered for the batch in `batch.extras[name]`.
 """
@@ -30,12 +33,12 @@ import numpy as np
 import torch
 
 from .collate import BatchMolGraph
-from .dataset import HostBatchBuffer, PackedMolGraphDataset
+from .dataset import MulticomponentPackedDataset, PackedMolGraphDataset
 
 
 class LoadedBatch(NamedTuple):
-    bmg: BatchMolGraph
-    ids: np.ndarray          # molecule ids of the batch, in batch order
+    bmg: BatchMolGraph       # a list of one batch per component for MulticomponentPackedDataset(union=False)
+    ids: np.ndarray          # molecule (data point) ids of the batch, in batch order
     extras: dict             # name -> tensor gathered from `arrays`
 
 
@@ -51,8 +54,15 @@ def epoch_shard(order: np.ndarray, rank: int, world: int) -> np.ndarray:
     return order[rank:total:world]
 
 
+def _cuda_copy(host, device):
+    """A host batch -- or a list of them (MulticomponentPackedDataset(union=False)) -- copied to `device` asynchronously."""
+    if isinstance(host, list):
+        return [h.cuda_copy(device, non_blocking=True) for h in host]
+    return host.cuda_copy(device, non_blocking=True)
+
+
 class PackedBatchLoader:
-    def __init__(self, dataset: PackedMolGraphDataset, batch_size: int = 64, shuffle: bool = True,
+    def __init__(self, dataset: PackedMolGraphDataset | MulticomponentPackedDataset, batch_size: int = 64, shuffle: bool = True,
                  seed: int | None = None, drop_last: bool | None = None, rank: int = 0, world: int = 1,
                  device: str | torch.device | None = None, prefetch: int = 3, transfer_dtype: torch.dtype | None = None,
                  arrays: dict | None = None, n_threads: int = 0, pack_tiles: bool = True):
@@ -173,7 +183,7 @@ class PackedBatchLoader:
         chunks = self.batches_of(self.epoch_order())
         to_cuda = self.device is not None and self.device.type == "cuda"
         compact = self.transfer_dtype is not None
-        ring = [HostBatchBuffer(ds.d_v, ds.d_e, pin_memory=to_cuda, compact=compact) for _ in range(self.prefetch)]
+        ring = [ds.host_buffer(pin_memory=to_cuda, compact=compact) for _ in range(self.prefetch)]
         free_evt = [None] * self.prefetch                           # H2D-complete event of the last use of each buffer
         free: queue.Queue = queue.Queue()                           # staging buffers the producer may write
         for k in range(self.prefetch):
@@ -207,15 +217,16 @@ class PackedBatchLoader:
                 k, ids, host = item
                 if to_cuda:
                     with torch.cuda.stream(copy_stream):
-                        bmg = host.cuda_copy(self.device, non_blocking=True)
+                        bmg = _cuda_copy(host, self.device)
                         ev = torch.cuda.Event()
                         ev.record(copy_stream)
                     free_evt[k] = ev
                     free.put(k)                                     # reusable once `ev` has completed (the producer waits)
                     cur = torch.cuda.current_stream(self.device)
                     cur.wait_event(ev)
-                    for t in (bmg.V, bmg.E, bmg.edge_index, bmg.rev_edge_index, bmg.batch):
-                        t.record_stream(cur)
+                    for b in (bmg if isinstance(bmg, list) else [bmg]):
+                        for t in (b.V, b.E, b.edge_index, b.rev_edge_index, b.batch):
+                            t.record_stream(cur)
                     yield LoadedBatch(bmg, ids, self._extras(ids))
                 else:
                     yield LoadedBatch(host, ids, self._extras(ids))  # views of ring[k]: valid until the next batch is drawn

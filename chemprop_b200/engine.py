@@ -2042,6 +2042,41 @@ class SegmentAggFunction(torch.autograd.Function):
         return dH, None, None, None, None, None
 
 
+class SegmentAggColumnsFunction(torch.autograd.Function):
+    """Mean / Sum / Norm aggregation of several batches of the same molecule count into the column blocks of ONE b x sum(d_c)
+    f32 buffer: `torch.cat([agg(H_0, batch_0), agg(H_1, batch_1), ...], 1)` of models/multi.py:51-52 without the cat.  One
+    dmpnn_segment_sum per batch writes its block through the row stride `ldy`; the backward is one dmpnn_segment_bcast per
+    batch reading its block through `ldg`.  `segs`: the (ptr, seg_of_row, b) of each batch (`segments_of`)."""
+
+    @staticmethod
+    def forward(ctx, segs, scale_mode, scale, *Hs):
+        _require_cuda(*Hs)
+        b = segs[0][2]
+        widths = [int(H.shape[1]) for H in Hs]
+        out = torch.empty((b, sum(widths)), dtype=torch.float32, device=Hs[0].device)
+        c0 = 0
+        for H, (ptr, _, _), d in zip(Hs, segs, widths):
+            segment_sum(H if H.stride(1) == 1 else H.contiguous(), ptr, b, d, out[:, c0:c0 + d], scale_mode=scale_mode,
+                        scale=scale, pad_to=d)
+            c0 += d
+        ctx.segs, ctx.mode, ctx.scale, ctx.widths = segs, scale_mode, scale, widths
+        ctx.rows = [(int(H.shape[0]), H.dtype) for H in Hs]
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        g = g.contiguous()
+        if g.dtype not in (torch.float32, torch.bfloat16):
+            g = g.float()
+        dHs, c0 = [], 0
+        for (ptr, seg_of_row, b), d, (nV, dt) in zip(ctx.segs, ctx.widths, ctx.rows):
+            dH = torch.empty((nV, d), dtype=dt, device=g.device)
+            segment_bcast(g[:, c0:c0 + d], seg_of_row, ptr, nV, d, dH, scale_mode=ctx.mode, scale=ctx.scale, n_seg=b)
+            dHs.append(dH)
+            c0 += d
+        return (None, None, None, *dHs)
+
+
 class SegmentBcastFunction(torch.autograd.Function):
     """rows <- their segment's row (`Z[batch]` of chemprop/nn/agg.py:127, nn/ffn.py:127): dmpnn_segment_bcast; the mirror
     is the segment sum."""

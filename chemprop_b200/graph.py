@@ -36,6 +36,13 @@ class _Captured:
     __slots__ = ("graph", "bmg", "out", "last", "last_ref", "launches")
 
 
+def _static_copy(bmg: BatchMolGraph) -> BatchMolGraph:
+    static = BatchMolGraph.from_tensors(bmg.V.clone(), bmg.E.clone(), bmg.edge_index.clone(), bmg.rev_edge_index.clone(),
+                                        bmg.batch.clone(), len(bmg))
+    static._meta_host = list(bmg._meta_host)
+    return static
+
+
 class CudaGraphStep:
     """`step = CudaGraphStep(fn)`; `loss = step(bmg)`.
 
@@ -50,7 +57,11 @@ class CudaGraphStep:
 
     The returned tensors are static outputs of the graph: valid until the next call with the same signature.  Parameters'
     `.grad` tensors must exist before the first call (run one eager step, or `p.grad = torch.zeros_like(p)`), so that the
-    captured backward accumulates into fixed buffers."""
+    captured backward accumulates into fixed buffers.
+
+    `step(bmgs)` also takes a list or tuple of batches (one per component of a multicomponent model with unshared
+    encoders): `fn` then receives a list of static batches, one per given batch, and the graph's signature is the tuple of
+    the batches' signatures."""
 
     def __init__(self, fn: Callable, max_graphs: int = 8, warmup: int = 2, pool=None):
         self.fn, self.max_graphs, self.warmup = fn, int(max_graphs), int(warmup)
@@ -60,68 +71,80 @@ class CudaGraphStep:
         self.replays = 0
         self.last_launches = 0
 
-    def _capture(self, bmg: BatchMolGraph) -> _Captured:
-        dev = bmg.V.device
-        static = BatchMolGraph.from_tensors(bmg.V.clone(), bmg.E.clone(), bmg.edge_index.clone(), bmg.rev_edge_index.clone(),
-                                            bmg.batch.clone(), len(bmg))
-        static._meta_host = list(bmg._meta_host)
+    def _capture(self, bmg) -> _Captured:
+        many = isinstance(bmg, (list, tuple))
+        dev = (bmg[0] if many else bmg).V.device
+        static = [_static_copy(b) for b in bmg] if many else _static_copy(bmg)
+        statics = static if many else [static]
+
+        def run():
+            for s in statics:
+                s._layout = None
+            return self.fn(static)
+
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):                 # warm-up on a side stream, as torch's capture protocol asks
             for _ in range(self.warmup):
-                static._layout = None
-                self.fn(static)
+                run()
         torch.cuda.current_stream(dev).wait_stream(side)
         cap = _Captured()
         cap.graph = torch.cuda.CUDAGraph()
         cap.bmg = static
         cap.last = cap.last_ref = None
-        static._layout = None
         kw = {} if self._pool is None else {"pool": self._pool}
         from . import _lib
 
         l0 = _lib.load().dmpnn_launch_count()
         with torch.cuda.graph(cap.graph, **kw):
-            cap.out = self.fn(static)
+            cap.out = run()
         cap.launches = int(_lib.load().dmpnn_launch_count() - l0)      # libdmpnn kernels one replay launches
         if self._pool is None:
             self._pool = cap.graph.pool()             # later graphs share this one's memory pool
         self.captures += 1
         return cap
 
-    def load(self, cap: _Captured, bmg: BatchMolGraph):
+    def load(self, cap: _Captured, bmg):
         # The very same (unmodified) batch object as last time -- a resident batch replayed step after step: nothing to copy.
         # "Same" = the object itself (held through a weak reference: an `id()` is reused as soon as a batch is freed, and a
         # fresh batch's tensors are all at version 0), the same storage and no in-place change torch knows of.  Tensors that
         # are rewritten through raw pointers behind torch's back are not seen: pass such a batch as a new object.
-        ts = (bmg.V, bmg.E, bmg.edge_index, bmg.rev_edge_index, bmg.batch)
-        stamp = tuple((t.data_ptr(), t._version, tuple(t.shape)) for t in ts)
-        if cap.last_ref is not None and cap.last_ref() is bmg and cap.last == stamp:
+        # A list of batches is compared batch by batch.
+        many = isinstance(cap.bmg, list)
+        bmgs, statics = (list(bmg), cap.bmg) if many else ([bmg], [cap.bmg])
+        stamp = tuple(tuple((t.data_ptr(), t._version, tuple(t.shape)) for t in (b.V, b.E, b.edge_index, b.rev_edge_index,
+                                                                                   b.batch)) for b in bmgs)
+        if (cap.last_ref is not None and len(cap.last_ref) == len(bmgs)
+                and all(r() is b for r, b in zip(cap.last_ref, bmgs)) and cap.last == stamp):
             return
         try:
-            cap.last_ref, cap.last = weakref.ref(bmg), stamp
+            cap.last_ref, cap.last = [weakref.ref(b) for b in bmgs], stamp
         except TypeError:                                  # a batch type without weak references: copied every time
             cap.last_ref = cap.last = None
-        s = cap.bmg
-        s.V.copy_(bmg.V, non_blocking=True)
-        s.E.copy_(bmg.E, non_blocking=True)
-        s._edge_index.copy_(bmg.edge_index, non_blocking=True)
-        s._rev_edge_index.copy_(bmg.rev_edge_index, non_blocking=True)
-        s._batch.copy_(bmg.batch, non_blocking=True)
+        for s, b in zip(statics, bmgs):
+            s.V.copy_(b.V, non_blocking=True)
+            s.E.copy_(b.E, non_blocking=True)
+            s._edge_index.copy_(b.edge_index, non_blocking=True)
+            s._rev_edge_index.copy_(b.rev_edge_index, non_blocking=True)
+            s._batch.copy_(b.batch, non_blocking=True)
 
-    def __call__(self, bmg: BatchMolGraph):
-        if not bmg.V.is_cuda:
+    def __call__(self, bmg):
+        many = isinstance(bmg, (list, tuple))
+        bmgs = list(bmg) if many else [bmg]
+        if not bmgs:
+            raise ValueError("CudaGraphStep needs at least one batch")
+        if not all(b.V.is_cuda for b in bmgs):
             raise ValueError("CudaGraphStep takes a device batch (BatchMolGraph.cuda_copy / a resident data set)")
-        sig = batch_signature(bmg)
+        sig = tuple(batch_signature(b) for b in bmgs) if many else batch_signature(bmg)
         cap = self._graphs.get(sig)
         if cap is None:
-            cap = self._capture(bmg)
+            cap = self._capture(bmgs if many else bmg)
             self._graphs[sig] = cap
             while len(self._graphs) > self.max_graphs:
                 self._graphs.popitem(last=False)
         else:
             self._graphs.move_to_end(sig)
-        self.load(cap, bmg)
+        self.load(cap, bmgs if many else bmg)
         cap.graph.replay()
         self.replays += 1
         self.last_launches = cap.launches

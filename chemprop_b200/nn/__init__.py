@@ -9,6 +9,7 @@ from .head import (EngineBatchNorm1d, EngineBinaryClassificationFFN, EngineBinar
 from .message_passing import AtomMessagePassing, BondMessagePassing
 from .mol_atom_bond import MABAtomMessagePassing, MABBondMessagePassing
 from .mol_atom_bond_model import EngineMolAtomBondMPNN
+from .multi import EngineMulticomponentMessagePassing, EngineMulticomponentMPNN
 from .transforms import GraphTransform, ScaleTransform, UnscaleTransform
 
 __all__ = ["Aggregation", "AggregationRegistry", "AttentiveAggregation", "MeanAggregation", "NormAggregation", "SumAggregation",
@@ -18,4 +19,5 @@ __all__ = ["Aggregation", "AggregationRegistry", "AttentiveAggregation", "MeanAg
            "EngineQuantileFFN", "EngineBinaryDirichletFFN", "EngineMulticlassDirichletFFN", "EngineMVELoss",
            "EngineEvidentialLoss", "EngineQuantileLoss", "EngineDirichletLoss", "EngineSpectralFFN", "EngineSID",
            "EngineWasserstein", "EngineMAE", "EngineRMSE", "EngineBoundedMSE", "EngineBoundedMAE", "EngineBoundedRMSE",
-           "EngineBatchNorm1d", "EngineLinear", "EngineMolAtomBondMPNN"]
+           "EngineBatchNorm1d", "EngineLinear", "EngineMolAtomBondMPNN",
+           "EngineMulticomponentMessagePassing", "EngineMulticomponentMPNN"]
