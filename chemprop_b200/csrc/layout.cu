@@ -415,10 +415,12 @@ extern "C" int dmpnn_layout_build(const int64_t* edge_index, const int64_t* rev_
   return 0;
 }
 
-// Work table of the fused depth step for batches holding molecules of more than 128 directed edges: every tile of the
-// layout with <= 128 rows becomes one work item (flag 0), every larger tile -- one oversized molecule -- is cut into
-// ceil(rows / 128) windows of <= 128 consecutive rows (flag 1: siblings / reverse edges may lie in another window, the
-// kernel gathers them from global memory).  One block; tiles are scanned in chunks of 1024 (fixed order).
+// Work table of the fused depth step for batches holding molecules of more than 128 directed edges or more than 128 atoms:
+// every tile of the layout with <= 128 rows and <= 128 atoms becomes one work item (flag 0), every larger tile -- one
+// oversized molecule -- is cut into ceil(rows / 128) windows of <= 128 consecutive rows (flag 1: siblings / reverse edges
+// may lie in another window, the kernel gathers them from global memory).  A tile of <= 128 rows but more than 128 atoms
+// (many fragments, e.g. a short chain and isolated atoms) is one window with flag 1: the kernel's staged row-pointer slice
+// holds the row pointers of at most 128 atoms, the global gathers need none.  One block; tiles are scanned in chunks of 1024 (fixed order).
 __global__ void __launch_bounds__(1024)
 k_work_table(const int32_t* __restrict__ tile_row_ptr, const int32_t* __restrict__ tile_atom_ptr, int n_tiles,
              int32_t* __restrict__ work_row_ptr, int32_t* __restrict__ work_atom_ptr, int8_t* __restrict__ work_flag,
@@ -431,10 +433,12 @@ k_work_table(const int32_t* __restrict__ tile_row_ptr, const int32_t* __restrict
   for (int t0 = 0; t0 < n_tiles; t0 += 1024) {
     const int t = t0 + tid;
     int r0 = 0, nr = 0, cnt = 0;
+    bool far = false;
     if (t < n_tiles) {
       r0 = tile_row_ptr[t];
       nr = tile_row_ptr[t + 1] - r0;
       cnt = nr > 128 ? (nr + 127) >> 7 : 1;
+      far = cnt > 1 || tile_atom_ptr[t + 1] - tile_atom_ptr[t] > 128;
     }
     int incl = cnt;                                   // inclusive scan inside the warp
     for (int o = 1; o < 32; o <<= 1) {
@@ -458,7 +462,7 @@ k_work_table(const int32_t* __restrict__ tile_row_ptr, const int32_t* __restrict
       for (int k = 0; k < cnt; ++k) {
         work_row_ptr[base + k] = r0 + 128 * k;
         work_atom_ptr[base + k] = a0;
-        work_flag[base + k] = cnt > 1 ? 1 : 0;
+        work_flag[base + k] = far ? 1 : 0;
       }
     }
     __syncthreads();

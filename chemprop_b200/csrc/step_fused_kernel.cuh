@@ -52,7 +52,8 @@ struct Params {
   const int32_t* rev_row;
   const int32_t* tile_row_ptr;   // work items: the layout's tiles, or (work_flag != nullptr) the work table in which
   const int32_t* tile_atom_ptr;  // every tile of more than 128 rows is cut into 128-row windows
-  const int8_t* work_flag;       // nullable; 1 = window of a multi-window molecule: siblings / rev() partners may lie outside
+  const int8_t* work_flag;       // nullable; 1 = window of a molecule of more than 128 rows or atoms: siblings / rev() partners
+                                 // may lie outside, and its row-pointer slice would not fit s_rowptr's 132 words
   const int32_t* n_work_dev;     // nullable; number of work items when the work table is in use (device scalar)
   const int32_t* dst_row;        // destination atom of every row (needed by the non-local windows only)
   const __nv_bfloat16* Hprev;    // the H tile's matrix again, for the non-local windows' global gathers
@@ -428,7 +429,7 @@ k_bond_step_fused(const __grid_constant__ CUtensorMap tmapH, Params p) {
     int t = blockIdx.x;
     // ATOM kernels: `atom0` / `natoms` are the first EDGE row and the edge count of the atom tile (its CSR slice), rows are atoms
     int row0 = 0, atom0 = 0, natoms = 0, nr = 0;
-    bool far = false;                        // this work item is a window of a multi-window molecule
+    bool far = false;                        // this work item is a window of an oversized molecule (work_flag)
     if (t < n_items) {
       row0 = __ldg(p.tile_row_ptr + t);
       nr = __ldg(p.tile_row_ptr + t + 1) - row0;

@@ -148,10 +148,11 @@ class Layout:
 
     def step_tables(self):
         """(tile_row_ptr, tile_atom_ptr, n_tiles, work_flag, n_work_dev, dst_row) for the fused depth step.  Batches whose
-        molecules all fit a 128-row tile pass the layout's tile tables as they are; a batch with larger molecules (condensed
-        reaction graphs) gets the work table of dmpnn_work_table_build: oversized tiles cut into 128-row windows, built once
-        per batch on the device (no host read-back: the kernel reads the window count from device memory)."""
-        if self.max_tile_rows <= 128:
+        molecules all fit a tile of 128 rows and 128 atoms pass the layout's tile tables as they are; a batch with larger
+        molecules (condensed reaction graphs; a molecule of many fragments) gets the work table of dmpnn_work_table_build:
+        oversized tiles cut into 128-row windows that gather from global memory, built once per batch on the device (no host
+        read-back: the kernel reads the window count from device memory)."""
+        if self.max_tile_rows <= 128 and self.max_tile_atoms <= 128:
             return self.tile_row_ptr, self.tile_atom_ptr, self.n_tiles, None, None, None
         if self._work is None:
             lib = _lib.load()

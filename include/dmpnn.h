@@ -283,8 +283,11 @@ int dmpnn_act_bwd(const void* G, int g_dtype, int64_t ldg, const int32_t* gidx,
  * i.e. message (mixins.py:11-18) + update (base.py:135-141) in ONE launch, one CTA per SM,
  * molecule-aligned 128-row tiles from dmpnn_layout_build.  g = tau when first_step!=0
  * (H_prev = H_0 and H^0 = tau(H_0) is recomputed on load), identity otherwise.
- * Wpk is W_h packed by dmpnn_pack_weight_bf16.  Requires ld % 16 == 0, a 32-byte aligned H_next, h <= 304, all tiles
- * <= 128 rows, DMPNN_FLAG_REV_INVOLUTION.  Returns <0 (and does nothing) otherwise.
+ * Wpk is W_h packed by dmpnn_pack_weight_bf16.  Requires ld % 16 == 0, a 32-byte aligned H_next, h <= 304,
+ * DMPNN_FLAG_REV_INVOLUTION; returns <0 (and does nothing) otherwise.  Without a work table (work_flag, n_work_dev and dst_row
+ * NULL) every tile must hold <= 128 rows and <= 128 atoms (DMPNN_META_MAX_TILE_ROWS / _ATOMS): the kernel stages a tile's
+ * row-pointer slice of natoms + 1 entries in 132 words.  A layout with a larger tile must pass dmpnn_work_table_build's
+ * tables, which flag every such tile.
  * M_out (nullable; first_step only; bf16, same ld, 32-byte aligned, ld % 16 == 0): also stores the message
  * M^1[e] (mixins.py:11-18) that the step consumed, saved for the W_h gradient instead of being recomputed.
  * Precondition: columns [h, pad16(h)) of every hidden input (H_prev, H_0) are zero (finite).  The kernel reads them (its TMA
@@ -344,7 +347,8 @@ int dmpnn_linear_tc_rows_bf16(const void* A, int64_t lda, int64_t R, int64_t K, 
  * before the single rounding, so that step writes dH_0 = dZ^{T-1} + .. + dZ^1 + dH^0 * tau'(H_0) directly.
  * G_out (nullable, bf16, same ld, 32-byte aligned, ld % 16 == 0): also writes the gathered operand G = (S.P) dZ, so
  * that the W_h gradient of this step is the plain GEMM dW_h += G^T . H^{t-1} (dZ^T . M^t == ((S.P) dZ)^T . H^{t-1}).
- * Same size / layout requirements as dmpnn_bond_step_fused_bf16, and the same precondition: columns [h, pad16(h)) of every
+ * Same size / layout / tile requirements as dmpnn_bond_step_fused_bf16 (tiles of more than 128 rows or atoms only through
+ * the work table), and the same precondition: columns [h, pad16(h)) of every
  * hidden input (dZ, Yact, add0, add1) are zero (finite).  Columns [h, pad16(h)) of dOut are written as zeros. */
 int dmpnn_bond_step_bwd_fused_bf16(const void* dZ, const void* Yact, void* dOut, int64_t ld, int64_t n_rows_alloc,
                                    int64_t h, const void* WpkT, const int32_t* rowptr, const int32_t* rev_row,
@@ -426,11 +430,13 @@ int dmpnn_bond_step_fused_bf16(const void* H_prev, const void* H_0, void* H_next
 int dmpnn_dropout_bits(void* bits, int64_t n_rows, int64_t words_per_row, float p, uint64_t seed, uint64_t offset, void* stream);
 
 /* Work table for batches with molecules of MORE than 128 directed edges (condensed reaction graphs, BASELINE config 4 with
- * BondMessagePassing): the layout's tiles, with every tile of > 128 rows (one oversized molecule) cut into windows of <= 128
- * consecutive rows.  Outputs: work_row_ptr / work_atom_ptr (n_work + 1 entries; capacity n_tiles + E / 128 + 2), work_flag
- * (1 = window of a cut molecule) and the device scalar n_work.  Pass work_row_ptr / work_atom_ptr as the tile tables of the
- * fused step together with work_flag, n_work and the layout's dst_row (all three NULL for batches without such molecules):
- * a flagged window gathers its sibling / reverse-edge rows from global memory instead of its shared-memory tile. */
+ * BondMessagePassing) or MORE than 128 atoms: the layout's tiles, with every tile of > 128 rows (one oversized molecule) cut
+ * into windows of <= 128 consecutive rows, and every tile of <= 128 rows but > 128 atoms (one molecule of many fragments)
+ * kept as one window.  Outputs: work_row_ptr / work_atom_ptr (n_work + 1 entries; capacity n_tiles + E / 128 + 2), work_flag
+ * (1 = window of an oversized molecule, 0 = a tile within both limits) and the device scalar n_work.  Pass work_row_ptr /
+ * work_atom_ptr as the tile tables of the fused step together with work_flag, n_work and the layout's dst_row (all three
+ * NULL for batches whose tiles all hold <= 128 rows and <= 128 atoms): a flagged window gathers its sibling / reverse-edge
+ * rows from global memory instead of its shared-memory tile.  n_tiles == 0 gives n_work = 0 and zero sentinels. */
 int dmpnn_work_table_build(const int32_t* tile_row_ptr, const int32_t* tile_atom_ptr, int64_t n_tiles,
                            int32_t* work_row_ptr, int32_t* work_atom_ptr, int8_t* work_flag, int32_t* n_work, void* stream);
 
