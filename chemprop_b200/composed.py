@@ -64,9 +64,9 @@ def _x3_first_use_check(out_x3: Tensor, X1c: Tensor, K1: int, Wc: Tensor, N: int
 
 
 class GatherLinear(torch.autograd.Function):
-    """Y[r] = [X1[i1(r)] || X2[i2(r)]] . W^T + b + res[r]   (r < R)  -- dmpnn_linear_fwd.
+    """Y[r] = [X1[i1(r)] || X2[i2(r)]] . W^T + b + res[r]   (r < R)  -- on the 3xTF32 or the SIMT GEMM family (engine.GEMMS).
     Covers W_i (mixins.py:8-9, :22-23), W_h with the H_0 residual (base.py:136-138) and W_o (base.py:180).
-    Gradients: W, b (dmpnn_linear_wgrad), res (identity), and X1 / X2 when they are not gathered."""
+    Gradients: W, b, res (identity), and X1 / X2 when they are not gathered."""
 
     @staticmethod
     def forward(ctx, X1, idx1, X2, idx2, W, b, res, R):
@@ -81,53 +81,49 @@ class GatherLinear(torch.autograd.Function):
         x3 = (idx1 is None and X2c is None and R > 0 and K1 % 4 == 0 and N % 4 == 0 and 0 < K1 <= K.MAX_X3_DIM
               and 0 < N <= K.MAX_X3_DIM and X1c.data_ptr() % 16 == 0 and (resc is None or resc.data_ptr() % 16 == 0)
               and K.X3_ENABLED and K._fused_available() and _X3_STATE["ok"] is not False)
-        if x3 and _X3_STATE["ok"] is None and X1c.is_cuda and torch.cuda.is_current_stream_capturing():
-            x3 = False                                  # the first-use check synchronises: not inside a graph capture
-        if x3:
-            K.linear_x3(X1c, K1, K.pack_weight_x3(Wc), N, out, bias=bc, res=resc, R=R, pad_to=N)
-            if _X3_STATE["ok"] is None:
+        first_use = x3 and _X3_STATE["ok"] is None
+        if first_use and X1c.is_cuda and torch.cuda.is_current_stream_capturing():
+            x3 = first_use = False                      # the first-use check synchronises: not inside a graph capture
+        X = X1c if idx1 is None and X2c is None else K.Rows(X1c, idx1, X2c, idx2)
+        if R > 0:
+            gemm = K.GEMMS[K.X3 if x3 else K.SIMT]
+            gemm.product(X, K1 + K2, gemm.pack(Wc), N, out, R=R, bias=bc, res=resc, pad_to=N)
+            if first_use:
                 out = _x3_first_use_check(out, X1c, K1, Wc, N, bc, resc, R)
                 x3 = bool(_X3_STATE["ok"])
-        elif R > 0:
-            K.linear_fwd(X1c, K1, Wc, out, N, idx1=idx1, X2=X2c, K2=K2, idx2=idx2, bias=bc, res=resc, R=R, pad_to=N)
         ctx.x3 = x3
-        ctx.args = (X1c, idx1, X2c, idx2, Wc, K1, K2, N, R)
+        ctx.args = (X, idx1, idx2, Wc, K1, K2, N, R)
         ctx.wdtype = W.dtype
         ctx.bdtype = None if b is None else b.dtype
         return out
 
     @staticmethod
     def backward(ctx, dY):
-        X1c, idx1, X2c, idx2, Wc, K1, K2, N, R = ctx.args
+        X, idx1, idx2, Wc, K1, K2, N, R = ctx.args
         need_x1, _, need_x2, _, need_w, need_b, need_res, _ = ctx.needs_input_grad
         dY = _c(dY)
         x3 = ctx.x3 and dY.data_ptr() % 16 == 0 and _X3_STATE["ok"] is True
+        gemm = K.GEMMS[K.X3 if x3 else K.SIMT]
         dX1 = dX2 = dW = db = None
         if need_w or need_b:
             dW = torch.zeros_like(Wc)
             db = torch.zeros(N, dtype=torch.float32, device=Wc.device) if need_b else None
-            if x3:
-                K.wgrad_x3(dY, X1c, R, N, K1, dW)
-                if db is not None:
-                    K.column_sum(dY, R, N, db)
-            elif R > 0:
-                K.linear_wgrad(dY, X1c, K1, dW, N, idx1=idx1, X2=X2c, K2=K2, idx2=idx2, dbias=db, R=R)
+            if R > 0:
+                gemm.wgrad(dY, X, R, N, K1 + K2, dW, db)
             dW = dW.to(ctx.wdtype)
             db = None if db is None else db.to(ctx.bdtype)
         if need_x1:
             if idx1 is not None:
                 raise K.DmpnnError("GatherLinear: no gradient through a gathered operand")
             dX1 = _buf(R, K1, Wc)
-            if x3:
-                K.linear_x3(dY, N, K.pack_weight_x3(Wc, transpose=True), K1, dX1, R=R, pad_to=K1)
-            elif R > 0:
-                K.linear_fwd(dY, N, Wc[:, :K1].t().contiguous(), dX1, K1, R=R, pad_to=K1)
+            if R > 0:
+                gemm.product(dY, N, gemm.pack(Wc[:, :K1], transpose=True), K1, dX1, R=R, pad_to=K1)
         if need_x2:
             if idx2 is not None:
                 raise K.DmpnnError("GatherLinear: no gradient through a gathered operand")
             dX2 = _buf(R, K2, Wc)
             if R > 0:
-                K.linear_fwd(dY, N, Wc[:, K1:].t().contiguous(), dX2, K2, R=R, pad_to=K2)
+                gemm.product(dY, N, gemm.pack(Wc[:, K1:], transpose=True), K2, dX2, R=R, pad_to=K2)
         return dX1, None, dX2, None, dW, db, (dY if need_res else None), None
 
 

@@ -34,18 +34,18 @@ STEP_EVENTS: list | None = None
 
 
 class _StepTimer:
-    def __init__(self, tag: str):
+    def __init__(self, tag: str | None):      # None: nothing is timed
         self.tag = tag
 
     def __enter__(self):
-        if STEP_EVENTS is not None:
+        if STEP_EVENTS is not None and self.tag is not None:
             self.e0 = torch.cuda.Event(enable_timing=True)
             self.e1 = torch.cuda.Event(enable_timing=True)
             self.e0.record(torch.cuda.current_stream())
         return self
 
     def __exit__(self, *exc):
-        if STEP_EVENTS is not None:
+        if STEP_EVENTS is not None and self.tag is not None:
             self.e1.record(torch.cuda.current_stream())
             STEP_EVENTS.append((self.tag, self.e0, self.e1))
         return False
@@ -1067,6 +1067,143 @@ class Plan:
     reason: str | None = None  # mol-atom-bond kinds: why the bf16 path does not apply (None: it does)
 
 
+@dataclass(frozen=True)
+class Rows:
+    """The operand [X1[idx1] || X2[idx2]] of a SIMT GEMM, read in place by dmpnn_linear_fwd / _wgrad: X1 gives its first
+    X1.shape[1] columns, X2 the rest of the GEMM's K (an index None: rows in order)."""
+    X1: Tensor
+    idx1: Tensor | None = None
+    X2: Tensor | None = None
+    idx2: Tensor | None = None
+
+
+def _sources(A, K: int) -> tuple:
+    """(X1, K1, the two-source keywords) of a SIMT operand: a Rows, or a tensor whose first K columns are the operand."""
+    if isinstance(A, Rows):
+        K1 = A.X1.shape[1]
+        return A.X1, K1, dict(idx1=A.idx1, X2=A.X2, K2=K - K1, idx2=A.idx2)
+    return A, K, {}
+
+
+class _Gemm:
+    """The GEMM family of Plan.gemm == SIMT (f32 FMA pipes), and the interface of all three: what the generic bond path
+    (bond_forward / bond_backward) and composed.GatherLinear need to state each GEMM once.  A family owns its kernels'
+    argument order and padding rules, its weight image, its operand formats, its output buffers and where its bias gradient
+    comes from.  Methods call the op wrappers through the module globals at call time (the tests substitute them)."""
+    timer = None      # _StepTimer tag of the unfused depth step's W_h GEMM
+
+    def pack(self, W: Tensor, transpose: bool = False):
+        """The weight image of W (N x K), or with `transpose` of a K x N matrix used as B[n][k] = W[k][n]."""
+        return W.t().contiguous() if transpose else W
+
+    def product(self, A, K: int, Wp, N: int, out: Tensor, *, pad_to: int | None = None, **epilogue):
+        """out[:R, :N] = act(A[:, :K] . W^T + bias + res), columns [N, pad_to) zeroed; `epilogue`: R, bias, res, act and
+        act_param of the op wrappers."""
+        X1, K1, src = _sources(A, K)
+        linear_fwd(X1, K1, Wp, out, N, **src, pad_to=pad_to, **epilogue)
+
+    def wgrad(self, dY: Tensor, X, R: int, N: int, K: int, dW: Tensor, db: Tensor | None = None, accumulate: bool = False):
+        """dW (+)= dY[:R, :N]^T . X[:R, :K] and, with `db`, db (+)= the column sums of dY."""
+        X1, K1, src = _sources(X, K)
+        linear_wgrad(dY, X1, K1, dW, N, **src, dbias=db, accumulate=accumulate, R=R)
+
+    def hidden(self, rows: int, hp: int, dtype, dev) -> Tensor:
+        """A hidden-width (hp columns) GEMM output."""
+        return _hidden(rows, hp, dtype, dev)
+
+    def output(self, rows: int, N: int, dtype, dev) -> tuple:
+        """(the read-out GEMM's output buffer, H_v: its rows [0, rows) and first N columns)."""
+        out = torch.empty((rows, N), dtype=dtype, device=dev)
+        return out, out
+
+    def wi_operand(self, V: Tensor, E: Tensor, lay: Layout):
+        """W_i's operand [V[src] || E] over the dst-sorted edge rows (mixins.py:8-9)."""
+        return Rows(V, lay.src_row, E, lay.perm)
+
+    def wo_operand(self, lay: Layout, V: Tensor, Hprev: Tensor, first: bool, h: int, cfg: MPConfig, ones: bool) -> tuple:
+        """(W_o's operand [V || M_v], M_v = sum_{dst(e)=v} H[e] of Hprev, tau applied on load when `first` (base.py:180,
+        208-211); the operand's ones column or None).  `ones` asks for a ones column when the family takes one."""
+        Mv = _hidden(lay.V, pad_hidden(h), cfg.hidden_dtype, V.device)
+        segment_sum(Hprev, lay.rowptr, lay.V, h, Mv, act=(cfg.act if first else ACT_NONE), act_param=cfg.act_param,
+                    pad_to=Mv.shape[1])
+        return Rows(V, X2=Mv), None
+
+
+class _X3Gemm(_Gemm):
+    """Plan.gemm == X3: 3xTF32 on the tensor cores (f32-accurate); every dimension a multiple of 4 (16-byte rows), the
+    operands materialised in f32."""
+    timer = "x3_gemm"
+
+    def pack(self, W: Tensor, transpose: bool = False):
+        return pack_weight_x3(W, transpose=transpose)
+
+    def product(self, A, K: int, Wp, N: int, out: Tensor, *, pad_to: int | None = None, **epilogue):
+        # A carries zero columns up to the next multiple of 4 (wi_operand)
+        linear_x3(A, (K + 3) // 4 * 4, Wp, N, out, pad_to=pad_to, **epilogue)
+
+    def wgrad(self, dY: Tensor, X, R: int, N: int, K: int, dW: Tensor, db: Tensor | None = None, accumulate: bool = False):
+        K4 = (K + 3) // 4 * 4       # W_i's operand: dW computed over its zero padding columns, then copied out
+        dW4 = dW if K4 == K else torch.empty((N, K4), dtype=torch.float32, device=dW.device)
+        wgrad_x3(dY, X, R, N, K4, dW4, accumulate=accumulate)
+        if dW4 is not dW:
+            dW.copy_(dW4[:, :K])
+        if db is not None:
+            column_sum(dY, R, N, db, accumulate=accumulate)
+
+    def wi_operand(self, V: Tensor, E: Tensor, lay: Layout):
+        d_v, d_e = V.shape[1], E.shape[1]
+        X0 = torch.empty((lay.E, (d_v + d_e + 3) // 4 * 4), dtype=torch.float32, device=V.device)
+        concat_f32(V, d_v, X0, lay.E, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm)
+        return X0
+
+    def wo_operand(self, lay: Layout, V: Tensor, Hprev: Tensor, first: bool, h: int, cfg: MPConfig, ones: bool) -> tuple:
+        # the torch.cat of base.py:180 assembled once: V copied in, M_v written in place by the segment sum
+        d_v = V.shape[1]
+        XO = torch.empty((lay.V, d_v + h), dtype=cfg.hidden_dtype, device=V.device)
+        XO[:, :d_v].copy_(V)
+        segment_sum(Hprev, lay.rowptr, lay.V, h, XO[:, d_v:], act=(cfg.act if first else ACT_NONE), act_param=cfg.act_param,
+                    pad_to=h)
+        return XO, None
+
+
+class _TcGemm(_Gemm):
+    """Plan.gemm == TC: bf16 operands on the tensor cores, f32 accumulate; its epilogues store pad16(N) columns."""
+
+    def pack(self, W: Tensor, transpose: bool = False):
+        return pack_weight_tc(W, transpose=transpose)
+
+    def product(self, A, K: int, Wp, N: int, out: Tensor, *, pad_to: int | None = None, **epilogue):
+        linear_tc(A, K, Wp, N, out, **epilogue)
+
+    def wgrad(self, dY: Tensor, X, R: int, N: int, K: int, dW: Tensor, db: Tensor | None = None, accumulate: bool = False):
+        dYb = dY
+        if dY.dtype == torch.float32:      # an f32 accumulator (dH_0): the GEMM takes its bf16 image, the bias its f32 sums
+            dYb = torch.empty((R, dY.shape[1]), dtype=torch.bfloat16, device=dY.device)
+            concat_bf16(dY, N, dYb, R)
+        wgrad_tc(dYb, X, R, N, K, dW, accumulate=accumulate)
+        if db is not None:
+            column_sum(dY, R, N, db, accumulate=accumulate)
+
+    def hidden(self, rows: int, hp: int, dtype, dev) -> Tensor:
+        return _empty_hidden(rows, hp, dtype, dev)
+
+    def output(self, rows: int, N: int, dtype, dev) -> tuple:
+        out = _empty_hidden(rows, pad_hidden(N), dtype, dev)
+        return out, out[:rows, :N]
+
+    def wi_operand(self, V: Tensor, E: Tensor, lay: Layout):
+        d_v, d_e = V.shape[1], E.shape[1]
+        X0 = torch.empty((lay.E, (d_v + d_e + 15) // 16 * 16), dtype=torch.bfloat16, device=V.device)
+        concat_bf16(V, d_v, X0, lay.E, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm)
+        return X0
+
+    def wo_operand(self, lay: Layout, V: Tensor, Hprev: Tensor, first: bool, h: int, cfg: MPConfig, ones: bool) -> tuple:
+        return _readout_operand(lay, V, Hprev, first, h, cfg, None, V.shape[1], ones)
+
+
+GEMMS = {TC: _TcGemm(), X3: _X3Gemm(), SIMT: _Gemm()}     # the family of each Plan.gemm value
+
+
 def plan(kind: str, cfg: MPConfig, lay: Layout | None, h: int, d_v: int, d_e: int) -> Plan:
     """The execution path of one message-passing call.  `kind`: "bond" / "atom" (Bond / AtomMPFunction and the export op's
     bonds), "mab_bond" / "mab_atom" (MABMPFunction), "export_atom" (the export op's atoms: never on the fused atom step).
@@ -1147,35 +1284,18 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
     T = cfg.hidden_dtype
     nE, nV = lay.E, lay.V
     a, ap = cfg.act, cfg.act_param
-    tc, x3 = path.gemm == TC, path.gemm == X3
-    X0 = X0f = None
-    # H_0 = W_i([V[src] || E])   (mixins.py:8-9); rows in dst-sorted order
-    if tc and nE > 0:
-        kx = (d_v + d_e + 15) // 16 * 16
-        X0 = torch.empty((nE, kx), dtype=T, device=dev)
-        concat_bf16(V, d_v, X0, nE, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm)
-        H0 = _empty_hidden(nE, hp, T, dev)
-        linear_tc(X0, d_v + d_e, pack_weight_tc(Wi), h, H0, bias=bi, R=nE)
-    elif x3 and nE > 0:
-        # fp32 tier on the tensor cores: [V[src] || E] materialised once in f32 (zero-padded to a multiple of 4 columns),
-        # W_i as a 3xTF32 GEMM; the same operand serves the W_i gradient
-        kx4 = (d_v + d_e + 3) // 4 * 4
-        X0f = torch.empty((nE, kx4), dtype=torch.float32, device=dev)
-        concat_f32(V, d_v, X0f, nE, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm)
-        H0 = _hidden(nE, hp, T, dev)
-        linear_x3(X0f, kx4, pack_weight_x3(Wi), h, H0, bias=bi, R=nE, pad_to=hp)
-    else:
-        H0 = _hidden(nE, hp, T, dev)
-        linear_fwd(V, d_v, Wi, H0, h, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm, bias=bi, R=nE, pad_to=hp)
+    gemm = GEMMS[path.gemm]
+    egemm = gemm if nE > 0 else GEMMS[SIMT]    # the edge GEMMs of a batch without edges: empty launches of the SIMT kernel
+    # H_0 = W_i([V[src] || E])   (mixins.py:8-9); rows in dst-sorted order.  The operand serves the W_i gradient too
+    X0 = egemm.wi_operand(V, E, lay)
+    H0 = egemm.hidden(nE, hp, T, dev)
+    egemm.product(X0, d_v + d_e, egemm.pack(Wi), h, H0, R=nE, bias=bi, pad_to=hp)
     Hs, Ms, Hbars = [], [], []
     Hprev, first = H0, True  # H^0 = tau(H_0) is applied on load (base.py:200)
     use_fused = path.fused
     Wpk = pack_weight_bf16(Wh) if use_fused else None
-    # fp32 tier with x3: W_h / W_o GEMMs as 3xTF32 on the tensor cores (f32-accurate)
-    Wh_x3 = pack_weight_x3(Wh) if (x3 and cfg.depth > 1 and nE > 0) else None
-    # bf16 tier off the fused kernel (undirected=True): the W_h GEMM still runs on the tensor cores (k_linear_tc, H_0 residual,
-    # bias and tau in its epilogue -- the form AtomMessagePassing's unfused step uses), not on the f32 FMA pipes
-    Wh_tc = pack_weight_tc(Wh) if (tc and not use_fused and cfg.depth > 1 and nE > 0) else None
+    # off the fused kernel the W_h GEMM takes the H_0 residual, bias and tau in its epilogue
+    Whp = egemm.pack(Wh) if (not use_fused and cfg.depth > 1) else None
     for _ in range(1, cfg.depth):
         if use_fused:
             Hn = _empty_hidden(nE, hp, T, dev)
@@ -1211,48 +1331,26 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             Hn = _hidden(nE, hp, T, dev)
             with _StepTimer("unfused_first" if first else "unfused"):
                 bond_message(src_in, lay, h, M, act=fa, act_param=ap)           # mixins.py:11-18
-                if Wh_x3 is not None:
-                    with _StepTimer("x3_gemm"):
-                        linear_x3(M, h, Wh_x3, h, Hn, bias=bh, res=H0, act=a, act_param=ap, R=nE, pad_to=hp)
-                elif Wh_tc is not None:
-                    linear_tc(M, h, Wh_tc, h, Hn, bias=bh, res=H0, act=a, act_param=ap, R=nE)
-                else:
-                    linear_fwd(M, h, Wh, Hn, h, bias=bh, res=H0, act=a, act_param=ap, R=nE, pad_to=hp)  # base.py:135-141
+                with _StepTimer(egemm.timer):
+                    egemm.product(M, h, Whp, h, Hn, R=nE, bias=bh, res=H0, act=a, act_param=ap, pad_to=hp)  # base.py:135-141
             Ms.append(M)
         Hs.append(Hn)
         Hprev, first = Hn, False
-    XO = Mv = Hv = ones_col = None
-    if Wo is not None and tc:
-        XO, ones_col = _readout_operand(lay, V, Hprev, first, h, cfg, None, d_v, for_backward and bo is not None)
-        Mv = XO[:, d_v:d_v + h]
+    XO = Hv = ones_col = None
+    if Wo is not None:
+        if cfg.dropout_p > 0 and path.gemm != TC:
+            raise DmpnnError("dropout on the monolithic tier needs the tensor-core path (see Plan.dropout_ok)")
+        # H_v = tau(W_o([V || M_v]))   (base.py:180-182)
+        XO, ones_col = gemm.wo_operand(lay, V, Hprev, first, h, cfg, for_backward and bo is not None)
         if readout_f32:
             Hv = torch.empty((max(nV, 1), h), dtype=torch.float32, device=dev)[:nV]
             linear_tc_rows(XO, d_v + h, pack_weight_tc(Wo), h, Hv, R=nV, bias=bo, act=a, act_param=ap)
         else:
-            Hvp = torch.empty((max(nV, 1), pad_hidden(h)), dtype=T, device=dev)
-            linear_tc(XO, d_v + h, pack_weight_tc(Wo), h, Hvp, bias=bo, act=a, act_param=ap, R=nV)
+            Hvp, Hv = gemm.output(nV, h, T, dev)
+            gemm.product(XO, d_v + h, gemm.pack(Wo), h, Hvp, R=nV, bias=bo, act=a, act_param=ap, pad_to=h)
             if cfg.dropout_p > 0:
                 _dropout_(Hvp, cfg)                                                    # base.py:182
-            Hv = Hvp[:nV, :h]
-    elif Wo is not None:
-        if cfg.dropout_p > 0:
-            raise DmpnnError("dropout on the monolithic tier needs the tensor-core path (see Plan.dropout_ok)")
-        if x3:
-            # [V || M_v] assembled once in f32 (torch.cat of base.py:180): V copied in, M_v written in place by the segment sum
-            XO = torch.empty((nV, d_v + h), dtype=T, device=dev)
-            XO[:, :d_v].copy_(V)
-            Mv = XO[:, d_v:]
-            segment_sum(Hprev, lay.rowptr, nV, h, Mv, act=(a if first else ACT_NONE), act_param=ap, pad_to=h)
-            Hv = torch.empty((nV, h), dtype=T, device=dev)
-            linear_x3(XO, d_v + h, pack_weight_x3(Wo), h, Hv, bias=bo, act=a, act_param=ap, R=nV, pad_to=h)
-        else:
-            # M_v = sum_{dst(e)=v} H[e]   (base.py:208-211)
-            Mv = _hidden(nV, hp, T, dev)
-            segment_sum(Hprev, lay.rowptr, nV, h, Mv, act=(a if first else ACT_NONE), act_param=ap, pad_to=hp)
-            # H_v = tau(W_o([V || M_v]))   (base.py:180-182)
-            Hv = torch.empty((nV, h), dtype=T, device=dev)
-            linear_fwd(V, d_v, Wo, Hv, h, X2=Mv, K2=h, bias=bo, act=a, act_param=ap, R=nV, pad_to=h)
-    saved = dict(H0=H0, Hs=Hs, Ms=Ms, Hbars=Hbars, Mv=Mv, Hv=Hv, X0=X0, XO=XO, X0f=X0f, dvp=d_v, ones_col=ones_col)
+    saved = dict(H0=H0, Hs=Hs, Ms=Ms, Hbars=Hbars, Hv=Hv, X0=X0, XO=XO, dvp=d_v, ones_col=ones_col)
     return Hv, saved
 
 
@@ -1267,7 +1365,7 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
     T = cfg.hidden_dtype
     nE, nV = lay.E, lay.V
     a, ap = cfg.act, cfg.act_param
-    H0, Hs, Ms, Hbars, Mv, Hv = saved["H0"], saved["Hs"], saved["Ms"], saved["Hbars"], saved["Mv"], saved["Hv"]
+    H0, Hs, Ms, Hbars, Hv = saved["H0"], saved["Hs"], saved["Ms"], saved["Hbars"], saved["Hv"]
     f32 = dict(dtype=torch.float32, device=dev)
     dWi = torch.zeros_like(Wi, dtype=torch.float32)
     dWh = torch.zeros_like(Wh, dtype=torch.float32)
@@ -1275,45 +1373,26 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
     dbi = torch.zeros(h, **f32) if need_bias[0] else None
     dbh = torch.zeros(h, **f32) if need_bias[1] else None
     dbo = torch.zeros(h, **f32) if need_bias[2] else None
-    tc, x3 = path.gemm == TC, path.gemm == X3
+    gemm = GEMMS[path.gemm]
     if gHv.stride(1) != 1:
         gHv = gHv.contiguous()
     # readout: dY = g * tau'(Y); dW_o = dY^T [V || M_v]; dM_v = dY . W_o[:, d_v:]
     dY = _hidden(nV, hp, T, dev)
     act_bwd(gHv, Hv, nV, h, act=a, act_param=ap, dZ=dY)
-    if tc:
-        wgrad_tc(dY, saved["XO"], nV, h, d_v + h, dWo)
-        if dbo is not None:
-            column_sum(dY, nV, h, dbo)
-    elif x3:
-        wgrad_x3(dY, saved["XO"], nV, h, d_v + h, dWo)
-        if dbo is not None:
-            column_sum(dY, nV, h, dbo)
-    else:
-        linear_wgrad(dY, V, d_v, dWo, h, X2=Mv, K2=h, dbias=dbo, R=nV)
-    if tc:
-        dMv = _empty_hidden(nV, hp, T, dev)
-        linear_tc(dY, h, pack_weight_tc(Wo[:, d_v:], transpose=True), h, dMv, R=nV)
-    elif x3:
-        dMv = _hidden(nV, hp, T, dev)
-        linear_x3(dY, h, pack_weight_x3(Wo[:, d_v:], transpose=True), h, dMv, R=nV, pad_to=hp)
-    else:
-        WoT = Wo[:, d_v:].t().contiguous()
-        dMv = _hidden(nV, hp, T, dev)
-        linear_fwd(dY, h, WoT, dMv, h, R=nV, pad_to=hp)
+    gemm.wgrad(dY, saved["XO"], nV, h, d_v + h, dWo, dbo)
+    dMv = gemm.hidden(nV, hp, T, dev)
+    gemm.product(dY, h, gemm.pack(Wo[:, d_v:], transpose=True), h, dMv, R=nV, pad_to=hp)
     dH0 = torch.zeros((max(nE, 1), hp), **f32)  # f32 accumulator of dH_0 over all depth steps
     if nE > 0:
         if cfg.depth == 1:
             # dH^0[e] = dM_v[dst(e)];  dH_0 = dH^0 * tau'(H_0)
             act_bwd(dMv, H0, nE, h, act=a, act_param=ap, gidx=lay.dst_row, from_preact=True, acc=dH0)
         else:
-            WhT = None if (tc or x3) else Wh.t().contiguous()
-            WhT_pk = pack_weight_tc(Wh, transpose=True) if tc else None
-            WhT_x3 = pack_weight_x3(Wh, transpose=True) if x3 else None
+            WhT = gemm.pack(Wh, transpose=True)
             dZ = _hidden(nE, hp, T, dev)
             act_bwd(dMv, Hs[-1], nE, h, act=a, act_param=ap, gidx=lay.dst_row, dZ=dZ, acc=dH0)
             # undirected steps that ran on the fused kernel (they saved no M^t): their mirror on the fused kernel too
-            fused_undirected = cfg.undirected and tc and path.fused
+            fused_undirected = cfg.undirected and path.fused and path.gemm == TC
             WhT_f = pack_weight_bf16(Wh.t().contiguous()) if fused_undirected else None
             for t in range(cfg.depth - 1, 0, -1):
                 # inputs of step t: Hin = H^{t-1} (or tau(H_0) when t == 1)
@@ -1338,25 +1417,9 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
                             bond_message(Hbars[t - 1], lay, h, M)
                         else:
                             bond_message(Hin, lay, h, M, act=(a if first else ACT_NONE), act_param=ap)
-                    if tc:
-                        wgrad_tc(dZ, M, nE, h, h, dWh, accumulate=True)
-                        if dbh is not None:
-                            column_sum(dZ, nE, h, dbh, accumulate=True)
-                    elif x3:
-                        wgrad_x3(dZ, M, nE, h, h, dWh, accumulate=True)
-                        if dbh is not None:
-                            column_sum(dZ, nE, h, dbh, accumulate=True)
-                    else:
-                        linear_wgrad(dZ, M, h, dWh, h, dbias=dbh, accumulate=True, R=nE)
-                    if tc:
-                        dM = _empty_hidden(nE, hp, T, dev)
-                        linear_tc(dZ, h, WhT_pk, h, dM, R=nE)
-                    elif x3:
-                        dM = _hidden(nE, hp, T, dev)
-                        linear_x3(dZ, h, WhT_x3, h, dM, R=nE, pad_to=hp)
-                    else:
-                        dM = _hidden(nE, hp, T, dev)
-                        linear_fwd(dZ, h, WhT, dM, h, R=nE, pad_to=hp)
+                    gemm.wgrad(dZ, M, nE, h, h, dWh, dbh, accumulate=True)
+                    dM = gemm.hidden(nE, hp, T, dev)
+                    gemm.product(dZ, h, WhT, h, dM, R=nE, pad_to=hp)
                     dHin = _hidden(nE, hp, T, dev)
                     bond_message(dM, lay, h, dHin, permute_on_read=True)
                     if cfg.undirected:
@@ -1368,21 +1431,7 @@ def bond_backward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, Wh: Tensor, Wo:
                 else:
                     dZ = _hidden(nE, hp, T, dev)
                     act_bwd(dHin, Hin, nE, h, act=a, act_param=ap, dZ=dZ, acc=dH0)
-        if tc:
-            dH0b = torch.empty((nE, hp), dtype=T, device=dev)
-            concat_bf16(dH0, h, dH0b, nE)                      # f32 accumulator -> bf16 operand
-            wgrad_tc(dH0b, saved["X0"], nE, h, d_v + d_e, dWi)
-            if dbi is not None:
-                column_sum(dH0, nE, h, dbi)
-        elif x3:
-            X0f = saved["X0f"]
-            dWi4 = torch.empty((h, X0f.shape[1]), dtype=torch.float32, device=dev)
-            wgrad_x3(dH0, X0f, nE, h, X0f.shape[1], dWi4)
-            dWi.copy_(dWi4[:, : d_v + d_e])
-            if dbi is not None:
-                column_sum(dH0, nE, h, dbi)
-        else:
-            linear_wgrad(dH0, V, d_v, dWi, h, idx1=lay.src_row, X2=E, K2=d_e, idx2=lay.perm, dbias=dbi, R=nE)
+        gemm.wgrad(dH0, saved["X0"], nE, h, d_v + d_e, dWi, dbi)
     return dWi, dbi, dWh, dbh, dWo, dbo
 
 
