@@ -12,6 +12,12 @@ in-degree, ...): everything that a launch parameter was derived from at capture 
 signature (LRU) and copies each new batch's five tensors into the static input buffers of the matching graph; a batch with a new
 signature is captured on first sight (two eager warm-up steps + the capture, ~10 ms).  Fixed-shape loaders (bucketed or padded
 batches, or a resident batch as in bench.py) therefore replay one graph for the whole run.
+
+That holds because every host-side argument of every launch is derived from the signature, and everything that depends on
+the batch's contents (layout, window table, atom tiles, segment pointers, mol-atom-bond index maps) is rebuilt inside the
+graph from the static inputs.  tests/test_graph_signature_host.py checks the first on the CPU for every capturable path
+and head, on batches of one signature and different topology (tests/graph_twins.py); tests/test_gpu_graph_replay.py
+replays such batches with the optimizer in the graph against the eager steps, bit for bit, and against float64.
 """
 from __future__ import annotations
 
