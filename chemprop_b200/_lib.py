@@ -114,6 +114,13 @@ SIGNATURES = {
     "dmpnn_constrain_fwd": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _vp]),
     "dmpnn_constrain_bwd": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _i64,
                                       _vp]),
+    "dmpnn_metric_workspace_bytes": (C.c_int, [_i64, _i64, _i64, C.POINTER(_sz)]),
+    "dmpnn_metric_accumulate": (C.c_int, [_i32, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp,
+                                          _vp, _vp, _vp]),
+    "dmpnn_metric_multiclass_mcc": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "dmpnn_metric_rank_format": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dmpnn_rank_curve_workspace_bytes": (C.c_int, [_i64, C.POINTER(_sz)]),
+    "dmpnn_rank_curve": (C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _sz, _vp]),
 }
 
 # dmpnn_pred_transform kinds (include/dmpnn.h)
@@ -121,6 +128,8 @@ PRED_REGRESSION, PRED_MVE, PRED_EVIDENTIAL, PRED_QUANTILE, PRED_DIRICHLET, PRED_
 # dmpnn_regression_loss kinds and dmpnn_spectral_transform activations (include/dmpnn.h)
 LOSS_MSE, LOSS_MAE, LOSS_RMSE = range(3)
 SPEC_SOFTPLUS, SPEC_EXP = range(2)
+# dmpnn_metric_accumulate kinds (include/dmpnn.h)
+METRIC_SQERR, METRIC_ABSERR, METRIC_R2, METRIC_CONFUSION, METRIC_SOFT_MCC = range(5)
 
 
 class DmpnnError(RuntimeError):

@@ -10,7 +10,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "lib" / "libdmpnn_sm90.so"
-SOURCES = ["api_misc.cu", "dataset.cu", "layout.cu", "linear.cu", "segment.cu", "step_fused.cu", "step_fused_fwd.cu", "step_fused_bwd.cu", "step_fused_far_fwd.cu", "step_fused_far_bwd.cu", "step_fused_atom_fwd.cu", "step_fused_atom_bwd.cu", "linear_tc.cu", "wgrad_tc.cu", "gemm_x3.cu", "head.cu", "row_head.cu", "constrain.cu"]
+SOURCES = ["api_misc.cu", "dataset.cu", "layout.cu", "linear.cu", "segment.cu", "step_fused.cu", "step_fused_fwd.cu", "step_fused_bwd.cu", "step_fused_far_fwd.cu", "step_fused_far_bwd.cu", "step_fused_atom_fwd.cu", "step_fused_atom_bwd.cu", "linear_tc.cu", "wgrad_tc.cu", "gemm_x3.cu", "head.cu", "row_head.cu", "constrain.cu", "metrics.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xptxas=-v", "-Xcompiler", "-fPIC",

@@ -810,6 +810,68 @@ def constrain_bwd(G: Tensor, Kl: Tensor, P: Tensor, ptr: Tensor, Cn: Tensor, dP:
     _lib.check(rc, "dmpnn_constrain_bwd")
 
 
+# ---- validation / test metrics (csrc/metrics.cu) ------------------------------------------------------------------
+def _metric_workspace(B: int, T: int, C_: int, dev) -> Tensor:
+    lib = _lib.load()
+    n = C.c_size_t(0)
+    _lib.check(lib.dmpnn_metric_workspace_bytes(B, T, C_, C.byref(n)), "dmpnn_metric_workspace_bytes")
+    return torch.empty(max(n.value, 1), dtype=torch.uint8, device=dev)
+
+
+def _masks_ok(B: int, T: int, *ms):
+    for m in ms:
+        if m is not None:
+            assert m.dtype == torch.uint8 and m.shape == (B, T) and m.is_contiguous(), "masks: contiguous B x T uint8"
+
+
+def metric_accumulate(kind: int, P: Tensor, Y: Tensor, mask, w, tw, lt_mask, gt_mask, fstate, istate, status):
+    """Adds one batch to a metric's state (_lib.METRIC_*): P, Y B x T f32; mask / lt_mask / gt_mask B x T uint8 or None
+    (mask None: the finite targets); w (B) / tw (T) f32 or None; fstate f64, istate int64, status int32 (device)."""
+    lib = _lib.load()
+    B, T = Y.shape
+    _masks_ok(B, T, mask, lt_mask, gt_mask)
+    ws = _metric_workspace(B, T, 1, P.device)
+    rc = lib.dmpnn_metric_accumulate(kind, P.data_ptr(), P.stride(0) if B else T, Y.data_ptr(), Y.stride(0) if B else T,
+                                     _ptr(mask), _ptr(w), _ptr(tw), _ptr(lt_mask), _ptr(gt_mask), T, B, T, _ptr(fstate),
+                                     _ptr(istate), _ptr(status), ws.data_ptr(), _stream())
+    _lib.check(rc, "dmpnn_metric_accumulate")
+
+
+def metric_multiclass_mcc(P: Tensor, Y: Tensor, mask, w, C_: int, fstate: Tensor, status: Tensor):
+    """Adds one batch to the multiclass MCC's T x (2C + 2) f64 state; P: B x (T*C) f32 class scores, Y: B x T labels."""
+    lib = _lib.load()
+    B, T = Y.shape
+    _masks_ok(B, T, mask)
+    ws = _metric_workspace(B, T, C_, P.device)
+    rc = lib.dmpnn_metric_multiclass_mcc(P.data_ptr(), P.stride(0) if B else T * C_, Y.data_ptr(), Y.stride(0) if B else T,
+                                         _ptr(mask), T, _ptr(w), B, T, C_, fstate.data_ptr(), status.data_ptr(),
+                                         ws.data_ptr(), _stream())
+    _lib.check(rc, "dmpnn_metric_multiclass_mcc")
+
+
+def metric_rank_format(P: Tensor, Y: Tensor, mask, score: Tensor, label: Tensor, keep: Tensor, status: Tensor):
+    """One update of AUROC / AUPRC: writes score (f32), label and keep (uint8), B * T entries each."""
+    lib = _lib.load()
+    B, T = Y.shape
+    _masks_ok(B, T, mask)
+    ws = _metric_workspace(B, T, 1, P.device)
+    rc = lib.dmpnn_metric_rank_format(P.data_ptr(), P.stride(0) if B else T, Y.data_ptr(), Y.stride(0) if B else T,
+                                      _ptr(mask), T, B, T, score.data_ptr(), label.data_ptr(), keep.data_ptr(),
+                                      status.data_ptr(), ws.data_ptr(), _stream())
+    _lib.check(rc, "dmpnn_metric_rank_format")
+
+
+def rank_curve(score: Tensor, label: Tensor, keep: Tensor, out: Tensor):
+    """out (f64, 2) = AUROC, AUPRC of the kept entries of the formatted updates (dmpnn_rank_curve)."""
+    lib = _lib.load()
+    n = score.numel()
+    nb = C.c_size_t(0)
+    _lib.check(lib.dmpnn_rank_curve_workspace_bytes(n, C.byref(nb)), "dmpnn_rank_curve_workspace_bytes")
+    ws = torch.empty(max(nb.value, 1), dtype=torch.uint8, device=out.device)
+    rc = lib.dmpnn_rank_curve(_ptr(score), _ptr(label), _ptr(keep), n, out.data_ptr(), ws.data_ptr(), nb.value, _stream())
+    _lib.check(rc, "dmpnn_rank_curve")
+
+
 def column_sum(Y: Tensor, R: int, N: int, out: Tensor, *, accumulate: bool = False):
     lib = _lib.load()
     n = C.c_size_t(0)

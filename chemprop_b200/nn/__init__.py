@@ -7,6 +7,7 @@ from .head import (EngineBatchNorm1d, EngineBinaryClassificationFFN, EngineBinar
                    EngineMveFFN, EngineMVELoss, EngineQuantileFFN, EngineQuantileLoss, EngineRegressionFFN, EngineRMSE,
                    EngineSID, EngineSpectralFFN, EngineWasserstein)
 from .message_passing import AtomMessagePassing, BondMessagePassing
+from .metrics import EngineCriterionMetric, EngineMetric, EngineMetricRegistry
 from .mol_atom_bond import MABAtomMessagePassing, MABBondMessagePassing
 from .mol_atom_bond_model import EngineMolAtomBondMPNN
 from .multi import EngineMulticomponentMessagePassing, EngineMulticomponentMPNN
@@ -20,4 +21,5 @@ __all__ = ["Aggregation", "AggregationRegistry", "AttentiveAggregation", "MeanAg
            "EngineEvidentialLoss", "EngineQuantileLoss", "EngineDirichletLoss", "EngineSpectralFFN", "EngineSID",
            "EngineWasserstein", "EngineMAE", "EngineRMSE", "EngineBoundedMSE", "EngineBoundedMAE", "EngineBoundedRMSE",
            "EngineBatchNorm1d", "EngineLinear", "EngineMolAtomBondMPNN",
-           "EngineMulticomponentMessagePassing", "EngineMulticomponentMPNN"]
+           "EngineMulticomponentMessagePassing", "EngineMulticomponentMPNN", "EngineMetric", "EngineMetricRegistry",
+           "EngineCriterionMetric"]

@@ -779,3 +779,65 @@ class EngineMPNN(nn.Module):
         if lt_mask is None and gt_mask is None:
             return self.predictor.criterion(preds, targets, None, weights)  # NaN targets are the mask (model.py:140-141)
         return self.predictor.criterion(preds, targets, None, weights, lt_mask, gt_mask)
+
+    def _eval_modules(self) -> list[nn.Module]:
+        """The modules `on_validation_model_eval` (models/model.py:162-167, models/multi.py) keeps in training mode: every
+        encoder block's V_d and graph transforms, the X_d transform and the predictor's output transform."""
+        blocks = [getattr(b, n) for b in self.message_passing.modules() for n in ("V_d_transform", "graph_transform")
+                  if isinstance(getattr(b, n, None), nn.Module)]
+        return blocks + [self.X_d_transform, self.predictor.output_transform]
+
+    def evaluate(self, batches, metrics=None, *, stage: str = "val") -> dict[str, float]:
+        """chemprop's `validation_step` / `test_step` over `batches` (TrainingBatch, or MulticomponentTrainingBatch for
+        EngineMulticomponentMPNN), then each metric's epoch value (models/model.py:162-202).
+
+        stage="val": eval mode except the input and output transforms (V_d / graph / X_d transforms and the predictor's
+        output transform stay in training mode, so predictions are compared to the scaled targets), `val_loss` from
+        `predictor.train_step` and the criterion with the batch's weights, and every metric on `forward`'s output with
+        weights of one.  stage="test": eval mode, metrics only.  Both take `preds[..., 0]` when the predictor has several
+        targets per task, and mask non-finite targets.  `metrics` (EngineMetric objects, reset here) default to the
+        predictor's default metric (nn.metrics.default_metric).  Runs under no_grad, restores every module's training flag,
+        and synchronises with the host once, at the end.  Returns {"val_loss": .., "val/<alias>": ..} or
+        {"test/<alias>": ..}; raises ValueError where an update met a target its metric cannot take."""
+        from .metrics import EngineCriterionMetric, default_metric
+
+        if stage not in ("val", "test"):
+            raise ValueError(f"stage must be 'val' or 'test', got {stage!r}")
+        metrics = [default_metric(self.predictor)] if metrics is None else list(metrics)
+        loss = EngineCriterionMetric(self.predictor.criterion) if stage == "val" else None
+        for m in metrics:
+            m.reset()
+        flags = [(m, m.training) for m in self.modules()]
+        try:
+            self.eval()
+            if stage == "val":
+                for m in self._eval_modules():
+                    m.train()
+            with torch.no_grad():
+                for bmg, V_d, X_d, targets, weights, lt_mask, gt_mask in batches:
+                    mask = targets.isfinite()
+                    targets = targets.nan_to_num(nan=0.0)
+                    Z = self.fingerprint(bmg, V_d, X_d)
+                    preds = self.predictor(Z)
+                    if self.predictor.n_targets > 1:
+                        preds = preds[..., 0]
+                    ones = torch.ones_like(weights)
+                    for m in metrics:
+                        m.update(preds, targets, mask, ones, lt_mask, gt_mask)
+                    if loss is not None:     # validation_step: the same fingerprint through train_step
+                        loss.update(self.predictor.train_step(Z), targets, mask, weights, lt_mask, gt_mask)
+                values = [m.compute() for m in metrics] + ([] if loss is None else [loss.compute()])
+                checked = [m for m in metrics if m._status is not None]
+                host = torch.stack([v.double().reshape(()) for v in values]
+                                   + [m._status.double().reshape(()) for m in checked]).tolist()
+        finally:
+            for m, f in flags:
+                m.training = f
+        bad = [m.alias for m, s in zip(checked, host[len(values):]) if s]
+        if bad:
+            raise ValueError(f"metric(s) {bad}: a target is not a valid label (binary targets must be 0 or 1, class "
+                             "targets in [-C, C))")
+        out = {f"{stage}/{m.alias}": v for m, v in zip(metrics, host)}
+        if loss is not None:
+            out = {"val_loss": host[len(metrics)], **out}
+        return out

@@ -661,6 +661,55 @@ int dmpnn_constrain_bwd(const float* G, int64_t ldg, const float* Kl, int64_t ld
                         const int32_t* ptr, int64_t m, const float* C, int64_t ldc, int64_t t, float* dP, int64_t lddp,
                         float* dKl, int64_t lddk, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Validation and test metrics (csrc/metrics.cu; chemprop/nn/metrics.py:59-499 and the torchmetrics classes it wraps).
+ * P, Y are B x T f32 (row strides ldp, ldy); `mask`, lt_mask, gt_mask are nullable B x T uint8 with row stride ldm, and a
+ * null mask means m = isfinite(Y).  Each call ADDS into caller-owned state: f64 sums (fstate) and int64 counts (istate),
+ * zeroed by the caller to start.  `status` (1 int32, device) is set to 1 by a call that meets a masked-in target its
+ * metric cannot take (a binary label outside {0, 1} after truncation, a class outside [-C, C)) and is otherwise left
+ * alone.  Classification inputs follow torchmetrics' per-update formatting: where any considered prediction of the call
+ * lies outside [0, 1] (or is NaN) the call reads sigmoid(P) (softmax over the classes for the multiclass MCC); the
+ * considered predictions are the masked-in ones for accuracy / F1 / AUROC / AUPRC (chemprop passes preds[mask]) and all of
+ * them for the MCCs (the reference tests preds.min() / preds.max()).
+ *   dmpnn_metric_accumulate   kind 0 squared error, 1 absolute error (MSE / MAE / RMSE; lt_mask / gt_mask give the bounded
+ *                             variants as in dmpnn_regression_loss): fstate[0] += sum w tw m L, istate[0] += sum m;
+ *                             kind 2 (R2, pooled over tasks): fstate[0..2] += sum y, sum y^2, sum (y - p)^2, istate[0] +=
+ *                             sum m; kind 3 (accuracy / F1, pooled, threshold p > 0.5): istate[0..3] += TP, FP, TN, FN;
+ *                             kind 4 (binary MCC, per task, soft): fstate[j * T + t] += the TP, FP, TN, FN (j = 0..3) of
+ *                             task t weighted by w m.  weights (B) / task_weights (T) nullable; kinds 2 and 3 ignore them.
+ *   dmpnn_metric_multiclass_mcc  P is B x T x C (row stride ldp >= T C, C >= 2); per task t, fstate[t (2C + 2) + j] += p_j
+ *                             (j < C), t_j (C + j), c (2C), s (2C + 1) of MulticlassMCCLoss._calc_unreduced_loss, weighted
+ *                             by w m; argmax takes the first maximum.
+ *   dmpnn_metric_rank_format  one update of AUROC / AUPRC: for element e = b T + t, score[e] = the formatted prediction,
+ *                             label[e] = its 0 / 1 target, keep[e] = m (masked-out elements: 0, 0, 0).
+ *   Workspace of the three: dmpnn_metric_workspace_bytes(B, T, C) bytes (C = 1 except for the multiclass MCC), any
+ *   contents.  Two-phase fixed-order reductions over a grid that depends on the shape only: bitwise repeatable, no
+ *   floating-point atomics, no host synchronisation.
+ *   dmpnn_rank_curve          AUROC and AUPRC of the n formatted elements kept: out[0] = AUROC (torchmetrics' binary_auroc:
+ *                             trapezoids over (fpr, tpr) from the origin, summed exactly in int64 and divided once by
+ *                             2 P N; 0 when either class is absent), out[1] = AUPRC (auc(recall, precision) of
+ *                             binary_precision_recall_curve with the point (0, 1) appended, trapezoids summed in f64 in a
+ *                             fixed order; NaN without positives).  Masked elements sort below every score instead of
+ *                             being compacted, so the sort needs no device count on the host: one key pass, one
+ *                             cub::DeviceRadixSort (descending, stable), one scan of (positives, run start), a fixed-order
+ *                             reduction.  n <= 2^31 - 1; workspace: dmpnn_rank_curve_workspace_bytes(n) bytes, any
+ *                             contents, `workspace_bytes` its size.  n = 0 writes (0, NaN).
+ * ------------------------------------------------------------------------------------- */
+int dmpnn_metric_workspace_bytes(int64_t B, int64_t T, int64_t C, size_t* bytes);
+int dmpnn_metric_accumulate(int kind, const float* P, int64_t ldp, const float* Y, int64_t ldy, const uint8_t* mask,
+                            const float* weights, const float* task_weights, const uint8_t* lt_mask,
+                            const uint8_t* gt_mask, int64_t ldm, int64_t B, int64_t T, double* fstate, int64_t* istate,
+                            int32_t* status, void* workspace, void* stream);
+int dmpnn_metric_multiclass_mcc(const float* P, int64_t ldp, const float* Y, int64_t ldy, const uint8_t* mask, int64_t ldm,
+                                const float* weights, int64_t B, int64_t T, int64_t C, double* fstate, int32_t* status,
+                                void* workspace, void* stream);
+int dmpnn_metric_rank_format(const float* P, int64_t ldp, const float* Y, int64_t ldy, const uint8_t* mask, int64_t ldm,
+                             int64_t B, int64_t T, float* score, uint8_t* label, uint8_t* keep, int32_t* status,
+                             void* workspace, void* stream);
+int dmpnn_rank_curve_workspace_bytes(int64_t n, size_t* bytes);
+int dmpnn_rank_curve(const float* score, const uint8_t* label, const uint8_t* keep, int64_t n, double* out,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
