@@ -127,6 +127,9 @@ static int launch_step(const char* what, const void* H_prev, const void* H_0, vo
   DMPNN_CHECK_ARG(atom || ((work_flag == nullptr) == (n_work_dev == nullptr) && (work_flag == nullptr || dst_row != nullptr)),
                   "%s: work_flag, n_work_dev and dst_row come together (dmpnn_work_table_build)", what);
   DMPNN_CHECK_ARG(!atom || (work_flag == nullptr && drop_bits == nullptr), "%s: no windows / keep bits in the atom step", what);
+  DMPNN_CHECK_ARG(drop_bits == nullptr || (drop_scale > 0.f && isfinite(drop_scale) &&
+                                           (reinterpret_cast<uintptr_t>(drop_bits) & 1) == 0),
+                  "%s: keep bits need a finite drop_scale > 0 and a 2-byte aligned array", what);
   DMPNN_CHECK_ARG((add0 == nullptr && add1 == nullptr) || (mode == MODE_BWD_LAST && add0 != nullptr),
                   "%s: addends need y_is_preact (and add0 before add1)", what);
   DMPNN_CHECK_ARG(((reinterpret_cast<uintptr_t>(add0) | reinterpret_cast<uintptr_t>(add1)) & 15) == 0,
@@ -209,7 +212,6 @@ static int launch_step(const char* what, const void* H_prev, const void* H_0, vo
             : dispatch_fwd<false>(act, first_step != 0, bias != nullptr, drop_bits != nullptr, grid, st, mH, p);
   else
     e = far ? dispatch_bwd<true>(mode, act, grid, st, mH, p) : dispatch_bwd<false>(mode, act, grid, st, mH, p);
-  DMPNN_CHECK_ARG(!(drop_bits != nullptr && act != DMPNN_ACT_RELU), "%s: dropout in the epilogue is built for ReLU only", what);
   DMPNN_CHECK_ARG(e == cudaSuccess, "%s: cannot configure %d B dynamic smem: %s", what, kSmemAlloc, cudaGetErrorString(e));
   DMPNN_CHECK_LAUNCH(what, 1);
   return 0;

@@ -1,4 +1,4 @@
-// The fused depth-step kernel of csrc/step_fused.cu (see there for the description), as a template: its ~70 instantiations
+// The fused depth-step kernel of csrc/step_fused.cu (see there for the description), as a template: its ~100 instantiations
 // (activation x first step x bias x autograd-mirror mode x {windows of oversized molecules} x {dropout in the epilogue}) are
 // compiled in six translation units in parallel (step_fused_{fwd,bwd,far_fwd,far_bwd,atom_fwd,atom_bwd}.cu).
 #pragma once
@@ -705,7 +705,10 @@ static cudaError_t launch_variant(int grid, cudaStream_t st, const CUtensorMap& 
   return cudaSuccess;
 }
 
-// forward step: every fused activation x first x bias; dropout (keep bits) is a ReLU-only feature (engine.dropout_fused_ok)
+// forward step: every fused activation x first x bias x {keep bits in the epilogue}.  Training steps take the keep bits
+// with ReLU only (engine.plan's dropout_ok: the mirror reads the mask out of tau' of the stored state); a forward-only call
+// (Monte Carlo dropout) takes them with every activation.  Bond steps only: the reference drops every directed edge's copy of
+// an atom state independently, which an atom-row mask cannot express.
 template <bool FAR, bool ATOM = false>
 cudaError_t dispatch_fwd(int act, bool first, bool bias, bool drop, int grid, cudaStream_t st, const CUtensorMap& mH, const Params& p) {
 #define DMPNN_FB(A, D)                                                                                              \
@@ -713,17 +716,21 @@ cudaError_t dispatch_fwd(int act, bool first, bool bias, bool drop, int grid, cu
                  : launch_variant<A, true, false, MODE_FWD, FAR, D, ATOM>(grid, st, mH, p))                            \
          : (bias ? launch_variant<A, false, true, MODE_FWD, FAR, D, ATOM>(grid, st, mH, p)                            \
                  : launch_variant<A, false, false, MODE_FWD, FAR, D, ATOM>(grid, st, mH, p)))
+#define DMPNN_FA(D)                                                  \
+  switch (act) {                                                     \
+    case DMPNN_ACT_NONE: return DMPNN_FB(DMPNN_ACT_NONE, D);           \
+    case DMPNN_ACT_RELU: return DMPNN_FB(DMPNN_ACT_RELU, D);           \
+    case DMPNN_ACT_LEAKYRELU: return DMPNN_FB(DMPNN_ACT_LEAKYRELU, D); \
+    case DMPNN_ACT_TANH: return DMPNN_FB(DMPNN_ACT_TANH, D);           \
+    case DMPNN_ACT_ELU: return DMPNN_FB(DMPNN_ACT_ELU, D);             \
+  }
   if (drop) {
-    if constexpr (ATOM) return cudaErrorInvalidValue;
-    else return act == DMPNN_ACT_RELU ? DMPNN_FB(DMPNN_ACT_RELU, true) : cudaErrorInvalidValue;
+    if constexpr (ATOM) return cudaErrorInvalidValue;   // atom rows stand for every out-edge of the atom: no per-edge masks
+    else { DMPNN_FA(true) }
+  } else {
+    DMPNN_FA(false)
   }
-  switch (act) {
-    case DMPNN_ACT_NONE: return DMPNN_FB(DMPNN_ACT_NONE, false);
-    case DMPNN_ACT_RELU: return DMPNN_FB(DMPNN_ACT_RELU, false);
-    case DMPNN_ACT_LEAKYRELU: return DMPNN_FB(DMPNN_ACT_LEAKYRELU, false);
-    case DMPNN_ACT_TANH: return DMPNN_FB(DMPNN_ACT_TANH, false);
-    case DMPNN_ACT_ELU: return DMPNN_FB(DMPNN_ACT_ELU, false);
-  }
+#undef DMPNN_FA
 #undef DMPNN_FB
   return cudaErrorInvalidValue;
 }

@@ -390,8 +390,9 @@ class MPConfig:
     undirected: bool
     hidden_dtype: torch.dtype  # torch.float32 (<=1e-5 tier) or torch.bfloat16 (<=1e-2 tier)
     fused: bool = True         # use the fused wgmma depth-step kernel when applicable
-    dropout_p: float = 0.0     # > 0: training-mode dropout on the fused bf16 / ReLU path (Plan.dropout_ok)
+    dropout_p: float = 0.0     # > 0: active nn.Dropout -- on the fused bf16 / ReLU path (Plan.dropout_ok), or forward-only
     mask_fn: object = None     # keep-mask source `f(like) -> {0,1} tensor like `like``; None = torch's bernoulli_
+    forward_only: bool = False  # no backward follows (Monte Carlo dropout): dropout runs on every bond path, any activation
 
 
 def _hidden(rows: int, hp: int, dtype, dev) -> Tensor:
@@ -1288,8 +1289,11 @@ def plan(kind: str, cfg: MPConfig, lay: Layout | None, h: int, d_v: int, d_e: in
     # state is the keep mask times tau' of the pre-dropout one, so no mask is stored and 1 / (1 - p) folds into the mirror's
     # packed weights -- with every GEMM on the tensor cores and every depth step fused.  Of a bond call with dropout only the
     # GEMM limits are warned about, and only when they alone keep it off that path (it then runs on the composed tier).
+    # A forward-only call (cfg.forward_only: Monte Carlo dropout) stores no mask for a mirror, so its dropout runs wherever the
+    # call would run without it: keep bits in every fused bond step, dmpnn_scale_mask everywhere else (bond_forward).
+    train_drop = cfg.dropout_p > 0 and not cfg.forward_only
     drop_shape = cfg.act == ACT_RELU and not cfg.undirected and lay.E > 0 and h % 4 == 0
-    if not tc and bf16 and not (bond and cfg.dropout_p > 0 and not drop_shape) and _fused_available():
+    if not tc and bf16 and not (bond and train_drop and not drop_shape) and _fused_available():
         _warn_once("tc_limits", f"chemprop_b200: precision='bf16' with d_h = {h}, GEMM inner dimensions {Ks}: outside the "
                    f"tensor-core kernels' limits (d_h <= {MAX_TC_HIDDEN}, d_v + d_e and d_v + d_h <= {MAX_TC_K}); the linear "
                    "layers run on the f32 FMA pipes with bf16 storage (the fp32 tier's 3xTF32 tensor-core GEMMs take d_h up "
@@ -1302,7 +1306,7 @@ def plan(kind: str, cfg: MPConfig, lay: Layout | None, h: int, d_v: int, d_e: in
         # Layout.step_tables); undirected bonds too, the reverse-edge average being a prologue pass (bond_forward)
         step = (bf16 and h <= MAX_TC_HIDDEN and lay.E > 0 and (not cfg.undirected or (UNDIRECTED_FUSED and h % 4 == 0))
                 and _fused_available())
-        if cfg.depth > 1 and not step and bf16 and lay.E > 0 and cfg.dropout_p == 0:
+        if cfg.depth > 1 and not step and bf16 and lay.E > 0 and not train_drop:
             why = (f"d_h = {h} > {MAX_TC_HIDDEN}" if h > MAX_TC_HIDDEN else
                    "undirected=True with d_h % 4 != 0" if cfg.undirected else "kernel unavailable")
             _warn_once("unfused", f"chemprop_b200: this batch leaves the fused depth-step kernel ({why}): the depth loop runs "
@@ -1374,15 +1378,15 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
             # training: the first step also stores M^1 (it is tau(H_0)-gathered, which no later kernel can rebuild
             # from a stored activation); the later steps' W_h gradients use (S.P) dZ from the backward kernel instead
             M1 = _empty_hidden(nE, hp, T, dev) if (first_in and for_backward) else None
-            # base.py:139 (training-mode dropout): keep bits from Philox, applied in the step's epilogue -- no pass over E x h
+            # base.py:139 (active dropout): keep bits from Philox, applied in the step's epilogue -- no pass over E x h
             bits = dropout_keep_bits(nE, h, cfg, Hn) if cfg.dropout_p > 0 else None
             with _StepTimer("fused_first" if first else "fused"):
                 bond_step_fused(src_in, H0, Hn, h, Wpk, bh, lay, a, ap, first_in, M_out=M1, drop_bits=bits,
                                 drop_scale=1.0 / (1.0 - cfg.dropout_p) if bits is not None else 1.0)
             Ms.append(M1)
         else:
-            if cfg.dropout_p > 0:
-                raise DmpnnError("dropout on the monolithic tier needs the fused depth step (see Plan.dropout_ok)")
+            if cfg.dropout_p > 0 and not cfg.forward_only:
+                raise DmpnnError("training-mode dropout on the monolithic tier needs the fused depth step (see Plan.dropout_ok)")
             src_in, fa = Hprev, (a if first else ACT_NONE)
             if cfg.undirected:  # H = (H + H[rev]) / 2   (base.py:202-203)
                 Hbar = _hidden(nE, hp, T, dev)
@@ -1395,18 +1399,22 @@ def bond_forward(lay: Layout, V: Tensor, E: Tensor, Wi: Tensor, bi, Wh: Tensor, 
                 bond_message(src_in, lay, h, M, act=fa, act_param=ap)           # mixins.py:11-18
                 with _StepTimer(egemm.timer):
                     egemm.product(M, h, Whp, h, Hn, R=nE, bias=bh, res=H0, act=a, act_param=ap, pad_to=hp)  # base.py:135-141
+                if cfg.dropout_p > 0:
+                    _dropout_(Hn, cfg)                                                 # base.py:139
             Ms.append(M)
         Hs.append(Hn)
         Hprev, first = Hn, False
     XO = Hv = ones_col = None
     if Wo is not None:
-        if cfg.dropout_p > 0 and path.gemm != TC:
-            raise DmpnnError("dropout on the monolithic tier needs the tensor-core path (see Plan.dropout_ok)")
+        if cfg.dropout_p > 0 and path.gemm != TC and not cfg.forward_only:
+            raise DmpnnError("training-mode dropout on the monolithic tier needs the tensor-core path (see Plan.dropout_ok)")
         # H_v = tau(W_o([V || M_v]))   (base.py:180-182)
         XO, ones_col = gemm.wo_operand(lay, V, Hprev, first, h, cfg, for_backward and bo is not None)
         if readout_f32:
             Hv = torch.empty((max(nV, 1), h), dtype=torch.float32, device=dev)[:nV]
             linear_tc_rows(XO, d_v + h, pack_weight_tc(Wo), h, Hv, R=nV, bias=bo, act=a, act_param=ap)
+            if cfg.dropout_p > 0 and nV > 0:
+                _dropout_(Hv, cfg)                                                     # mol_atom_bond.py vertex_finalize
         else:
             Hvp, Hv = gemm.output(nV, h, T, dev)
             gemm.product(XO, d_v + h, gemm.pack(Wo), h, Hvp, R=nV, bias=bo, act=a, act_param=ap, pad_to=h)
@@ -2062,6 +2070,8 @@ class MABMPFunction(torch.autograd.Function):
                 Xe = torch.empty((nE, (d_e + h + 15) // 16 * 16), dtype=T, device=dev)
                 concat_bf16(E, d_e, Xe, nE, X2=Hfin, K2=h, idx2=src_idx)
                 linear_tc_rows(Xe, d_e + h, pack_weight_tc(Weo_), h, He, R=nE, bias=beo_, act=a, act_param=ap)
+                if cfg.dropout_p > 0:
+                    _dropout_(He, cfg)                                                 # mol_atom_bond.py edge_finalize
         _mp_save(ctx, lay, cfg, p, V, E, (Wi_, Wh_, Wvo_, Weo_), saved, Hv)
         ctx.kind = kind
         ctx.edge = (Xe, None if He is None else He.detach())

@@ -747,6 +747,26 @@ class EngineBatchNorm1d(nn.BatchNorm1d):
                                             self.momentum)
 
 
+def _predict(model: nn.Module, batches, step, active_dropout: bool, gather):
+    """The predict loop of EngineMPNN / EngineMolAtomBondMPNN: `step(batch)` per batch in eval mode (nn.Dropout modules
+    trained when `active_dropout`) under torch.inference_mode(), `gather(outputs)`; training flags restored even on error."""
+    flags = [(m, m.training) for m in model.modules()]
+    try:
+        model.eval()
+        if active_dropout:
+            for m in model.modules():
+                if isinstance(m, nn.Dropout):
+                    m.train()
+        with torch.inference_mode():
+            outs = [step(b) for b in batches]
+            if not outs:
+                raise ValueError("predict: no batches")
+            return gather(outs)
+    finally:
+        for m, f in flags:
+            m.training = f
+
+
 class EngineMPNN(nn.Module):
     """`chemprop.models.MPNN` reduced to the path (models/model.py:66-161): message passing -> aggregation -> batch norm ->
     predictor -> criterion, all on the engine.  The predictor is EngineRegressionFFN (the default),
@@ -779,6 +799,15 @@ class EngineMPNN(nn.Module):
         if lt_mask is None and gt_mask is None:
             return self.predictor.criterion(preds, targets, None, weights)  # NaN targets are the mask (model.py:140-141)
         return self.predictor.criterion(preds, targets, None, weights, lt_mask, gt_mask)
+
+    def predict(self, batches, *, active_dropout: bool = False) -> Tensor:
+        """chemprop's `predict_step` over `batches` (TrainingBatch, or MulticomponentTrainingBatch for
+        EngineMulticomponentMPNN), concatenated along molecules: `trainer.predict` followed by `torch.concat(preds, 0)`
+        (models/model.py:203-206).  Eval mode under torch.inference_mode(); `active_dropout` then trains every nn.Dropout
+        module, as chemprop's DropoutEstimator does for each pass.  Every module's training flag is restored, even on error.
+        No host synchronisation: the result is a device tensor, ready when the stream is."""
+        return _predict(self, batches, lambda b: self(b[0], b[1], b[2]), active_dropout,
+                        lambda outs: torch.cat(outs, 0))
 
     def _eval_modules(self) -> list[nn.Module]:
         """The modules `on_validation_model_eval` (models/model.py:162-167, models/multi.py) keeps in training mode: every

@@ -7,10 +7,19 @@ Differences a user can see: the module must live on a CUDA device (there is no C
 within 1e-5) or "bf16" (bf16 hidden states + tensor-core depth step; within 1e-2).
 
 Two execution tiers sit behind `forward`: the monolithic autograd functions of engine.py (tau fused into the
-kernels: ReLU / LeakyReLU / Tanh / ELU, dropout inactive) and the composed tier of composed.py (the reference's op
-sequence, one libdmpnn kernel per op, `self.tau` / `self.dropout` applied by torch in between) for everything else:
-PReLU, SELU or user activation modules, LeakyReLU / ELU with a negative parameter, dropout > 0 in training,
-AtomMessagePassing(undirected=True).
+kernels: ReLU / LeakyReLU / Tanh / ELU) and the composed tier of composed.py (the reference's op sequence, one libdmpnn
+kernel per op, `self.tau` / `self.dropout` applied by torch in between) for everything else: PReLU, SELU or user
+activation modules, LeakyReLU / ELU with a negative parameter, AtomMessagePassing(undirected=True), and active dropout
+that the monolithic tier cannot take.
+
+Dropout is active when `self.dropout` is in training mode with p > 0 -- the flag of the nn.Dropout module, as in the
+reference (base.py:139, :182), so that chemprop's DropoutEstimator, which trains only the nn.Dropout modules of an eval-mode
+model, samples the encoder too.  `p` is read at call time.  Active dropout runs on the monolithic tier
+  * on a forward-only call (`torch.is_grad_enabled()` false, or no parameter requiring grad) of BondMessagePassing: keep
+    bits in the fused bf16 depth step for every fused activation, dmpnn_scale_mask on every other bond path;
+  * in a training step of BondMessagePassing on the fused bf16 / ReLU path (engine.Plan.dropout_ok).
+AtomMessagePassing's monolithic tiers restate the reference on atoms, which needs every out-edge of an atom to carry the
+same state; the reference drops each edge's copy independently, so active dropout runs it on the composed tier.
 """
 from __future__ import annotations
 
@@ -135,12 +144,27 @@ class _MessagePassingBase(nn.Module):
         """Training-mode dropout that can stay on the fused bf16 path for this batch (BondMessagePassing only)."""
         return False
 
+    def dropout_active(self) -> bool:
+        """nn.Dropout's own test (base.py:139): its training flag and p > 0, read now (DropoutEstimator rewrites p)."""
+        return bool(self.dropout.training and self.dropout.p > 0)
+
+    def forward_only(self) -> bool:
+        """No backward can follow this call: autograd is off, or no parameter asks for a gradient."""
+        return not torch.is_grad_enabled() or not any(p.requires_grad for p in self.parameters())
+
+    def _forward_only_dropout(self) -> bool:
+        """Active dropout that runs on the monolithic tier because no mirror needs its masks (BondMessagePassing only)."""
+        return False
+
     def uses_composed_tier(self, lay=None) -> bool:
-        """True when this call cannot run on the monolithic functions (see the module docstring).  Training-mode
-        dropout stays monolithic only on the fused bf16 / ReLU path, which depends on the batch's layout `lay`."""
+        """True when this call cannot run on the monolithic functions (see the module docstring).  Active dropout stays
+        monolithic on a forward-only bond call, and in training on the fused bf16 / ReLU path, which depends on the batch's
+        layout `lay`."""
         if not is_fused_activation(self.tau):
             return True
-        if self.training and self.dropout.p > 0:
+        if self.dropout_active():
+            if self._forward_only_dropout():
+                return False
             return not (lay is not None and self._dropout_on_fused_path(lay))
         return False
 
@@ -169,6 +193,7 @@ class _MessagePassingBase(nn.Module):
                 # of the bf16 rate), W_i / W_o on the f32 FMA pipes, and every reference op is a launch of its own
                 why = (f"activation {activation_name(self.tau)}" if not is_fused_activation(self.tau) else
                        "undirected AtomMessagePassing" if (self.undirected and type(self)._kind == 1) else
+                       "dropout in AtomMessagePassing" if type(self)._kind == 1 else
                        "training-mode dropout outside the fused ReLU path")
                 _warn_once("composed_bf16", f"chemprop_b200: precision='bf16' requested, but this configuration ({why}) runs on "
                            "the composed tier: f32 hidden states, one kernel per reference op, no fused depth step "
@@ -176,8 +201,9 @@ class _MessagePassingBase(nn.Module):
             H = type(self)._composed_forward(self, bmg, lay)          # computed in f32 on this tier
         else:
             cfg = self._config()
-            if self.training and self.dropout.p > 0:
+            if self.dropout_active():
                 cfg.dropout_p = float(self.dropout.p)
+                cfg.forward_only = self._forward_only_dropout()
                 cfg.mask_fn = getattr(self, "_mask_fn", None)      # test hook: where the keep masks come from
             H = type(self)._function.apply(
                 bmg.V, bmg.E, self.W_i.weight, self.W_i.bias, self.W_h.weight, self.W_h.bias,
@@ -204,6 +230,9 @@ class BondMessagePassing(_MessagePassingBase):
     """Directed-bond message passing (chemprop/nn/message_passing/base.py:215-251)."""
     _function = BondMPFunction
     _composed_forward = staticmethod(composed.bond_forward)
+
+    def _forward_only_dropout(self) -> bool:
+        return 0.0 < self.dropout.p < 1.0 and self.forward_only()
 
     def _dropout_on_fused_path(self, lay) -> bool:
         if not (self.precision == "bf16" and 0.0 < self.dropout.p < 1.0 and is_fused_activation(self.tau)):

@@ -9,7 +9,8 @@ Per-edge outputs are handed back in the caller's edge order.  CUDA only, like th
     `dropout` applied by torch in between, f32 hidden states; matches the reference within 1e-5.
   * "bf16": engine.MABMPFunction -- bf16 hidden states, the fused depth step of the bf16 tier, the W_vo read-out and the
     per-edge W_eo head as tensor-core GEMMs with bias, tau and an f32 store in their epilogues; within 1e-2.  It applies
-    when the activation is fused (ReLU, LeakyReLU, Tanh, ELU), `undirected=False`, no training-mode dropout, and the GEMM
+    when the activation is fused (ReLU, LeakyReLU, Tanh, ELU), `undirected=False`, no active dropout (except on a
+    forward-only call of MABBondMessagePassing: keep bits in the fused depth step, dmpnn_scale_mask after W_vo / W_eo), and the GEMM
     sizes fit the tensor-core kernels (d_h <= engine.MAX_TC_HIDDEN and a multiple of 4, every inner dimension -- d_e + d_h
     for W_eo included -- <= engine.MAX_TC_K).  Anything else runs on the composed tier, with a one-time RuntimeWarning
     naming the reason.
@@ -80,10 +81,23 @@ class _MABMessagePassingBase(nn.Module):
             return f"activation {activation_name(self.tau)}"
         if self.undirected:
             return "undirected=True"
-        if self.training and self.dropout.p > 0:
-            return "training-mode dropout"
+        if self.dropout_active() and not self._forward_only_dropout():
+            return "training-mode dropout" if self._kind == "bond" or not self.forward_only() else "dropout on atom states"
         return plan("mab_" + self._kind, self._config(), None, self.W_h.out_features, self.hparams["d_v"],
                     self.hparams["d_e"]).reason
+
+    def dropout_active(self) -> bool:
+        """nn.Dropout's own test (mol_atom_bond.py `update` / `*_finalize`): its training flag and p > 0, read now."""
+        return bool(self.dropout.training and self.dropout.p > 0)
+
+    def forward_only(self) -> bool:
+        """No backward can follow this call: autograd is off, or no parameter asks for a gradient."""
+        return not torch.is_grad_enabled() or not any(p.requires_grad for p in self.parameters())
+
+    def _forward_only_dropout(self) -> bool:
+        """Active dropout on the bf16 tier: forward-only bond calls (the atom kind's restatement on atoms needs every
+        out-edge of an atom to carry the same state, which per-edge masks break)."""
+        return self._kind == "bond" and 0.0 < self.dropout.p < 1.0 and self.forward_only()
 
     def uses_composed_tier(self) -> bool:
         return self.precision != "bf16" or self.composed_reason() is not None
@@ -109,10 +123,14 @@ class _MABMessagePassingBase(nn.Module):
         why = self.composed_reason() if self.precision == "bf16" else None
         if self.precision == "bf16" and why is None:
             W_vo, W_eo = self.W_vo, self.W_eo
+            cfg = self._config()
+            if self.dropout_active():
+                cfg.dropout_p, cfg.forward_only = float(self.dropout.p), True
+                cfg.mask_fn = getattr(self, "_mask_fn", None)      # test hook: where the keep masks come from
             H_v, H_e = MABMPFunction.apply(
                 bmg.V, bmg.E, self.W_i.weight, self.W_i.bias, self.W_h.weight, self.W_h.bias,
                 None if W_vo is None else W_vo.weight, None if W_vo is None else W_vo.bias,
-                None if W_eo is None else W_eo.weight, None if W_eo is None else W_eo.bias, lay, self._config(), self._kind)
+                None if W_eo is None else W_eo.weight, None if W_eo is None else W_eo.bias, lay, cfg, self._kind)
             H_v = H_v if W_vo is not None else None
             H_e = H_e if W_eo is not None else None
         else:

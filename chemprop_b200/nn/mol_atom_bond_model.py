@@ -24,7 +24,7 @@ import torch
 from torch import Tensor, nn
 
 from .. import engine as K
-from .head import EdgePairOperand, _Criterion, EngineBatchNorm1d, engine_mlp
+from .head import EdgePairOperand, _Criterion, _predict, EngineBatchNorm1d, engine_mlp
 
 _LEVELS = ("mol", "atom", "bond")
 
@@ -171,6 +171,15 @@ class EngineMolAtomBondMPNN(nn.Module):
         fps = self.fingerprint(bmg, V_d, E_d, X_d)
         predss = self._predictions(fps, train=False)
         return predss if constraints is None else self._constrain(bmg, fps, predss, constraints)
+
+    def predict(self, batches, *, active_dropout: bool = False) -> list:
+        """chemprop's `predict_step` over `batches` (tuples `(bmg, V_d, E_d, X_d, ..., constraints)`, as the reference's
+        MolAtomBondTrainingBatch), each level concatenated along its rows (models/mol_atom_bond.py:435-440 followed by
+        the estimators' `torch.concat(preds, 0)`): `[mol, atom, bond]`, None for an absent level.  Eval mode under
+        torch.inference_mode(); `active_dropout` trains every nn.Dropout module (DropoutEstimator).  Every module's
+        training flag is restored, even on error; no host synchronisation."""
+        return _predict(self, batches, lambda b: self(b[0], b[1], b[2], b[3], b[-1]), active_dropout,
+                        lambda outs: [None if level[0] is None else torch.cat(level, 0) for level in zip(*outs)])
 
     def training_loss(self, bmg, targetss, weightss, V_d: Tensor | None = None, E_d: Tensor | None = None,
                       X_d: Tensor | None = None, lt_masks=None, gt_masks=None, constraints=None) -> Tensor:

@@ -423,8 +423,11 @@ int dmpnn_bond_step_fused_bf16(const void* H_prev, const void* H_0, void* H_next
                                const void* drop_bits, float drop_scale, void* stream);
 
 /* Training-mode dropout of base.py:139 INSIDE the fused step: `drop_bits` (nullable) holds 16 keep bits per (row, 16-column
- * block) -- uint16 [n_rows][pad16(h) / 16], bit q of word j = column 16 j + q -- and the epilogue writes
- * keep ? tau(z) * drop_scale : 0 with one rounding (drop_scale = 1 / (1 - p)); no mask pass over the E x h matrix.
+ * block) -- uint16 [n_rows][pad16(h) / 16], bit q of word j = column 16 j + q, 2-byte aligned -- and the epilogue writes
+ * keep ? tau(z) * drop_scale : 0 with one rounding (drop_scale = 1 / (1 - p), finite and > 0); no mask pass over the E x h
+ * matrix.  Every fused activation takes keep bits, on every work item (the windows of oversized molecules too).  The
+ * autograd mirror reads the mask back out of tau' of the stored state, which holds for ReLU only: a training step uses
+ * keep bits with ReLU, a forward-only call (Monte Carlo dropout) with any activation.
  * dmpnn_dropout_bits fills such an array from Philox4x32-10 (key = seed, counter = (word index, offset)): bit = [u16 >= round(p *
  * 65536)], i.e. P(drop) = p to 2^-16; the same (seed, offset) always gives the same bits. */
 int dmpnn_dropout_bits(void* bits, int64_t n_rows, int64_t words_per_row, float p, uint64_t seed, uint64_t offset, void* stream);
