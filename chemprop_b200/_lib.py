@@ -96,6 +96,7 @@ SIGNATURES = {
     "dmpnn_evidential_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _f32, _vp, _vp, _i64, _vp]),
     "dmpnn_quantile_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _i64, _vp]),
     "dmpnn_dirichlet_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _f32, _vp, _vp, _i64, _vp]),
+    "dmpnn_enrichment_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _f32, _i32, _f32, _f32, _vp, _vp, _i64, _vp]),
     "dmpnn_regression_loss": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp, _i64, _vp]),
     "dmpnn_spectral_transform": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _vp, _i64, _vp]),
     "dmpnn_spectral_transform_bwd": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _i64, _i32, _vp, _i64, _vp]),
@@ -109,6 +110,8 @@ SIGNATURES = {
                                              _vp, _vp]),
     "dmpnn_bce_loss_rows_workspace_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
     "dmpnn_bce_loss_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i64, _vp, _vp]),
+    "dmpnn_pinball_loss_rows_workspace_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
+    "dmpnn_pinball_loss_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _i64, _vp, _vp]),
     "dmpnn_ce_loss_rows_workspace_bytes": (C.c_int, [_i64, _i64, C.POINTER(_sz)]),
     "dmpnn_ce_loss_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp]),
     "dmpnn_constrain_fwd": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _vp, _i64, _vp, _vp]),
@@ -125,6 +128,9 @@ SIGNATURES = {
 
 # dmpnn_pred_transform kinds (include/dmpnn.h)
 PRED_REGRESSION, PRED_MVE, PRED_EVIDENTIAL, PRED_QUANTILE, PRED_DIRICHLET, PRED_DIRICHLET_PROBS, PRED_DIRICHLET_BINARY = range(7)
+PRED_SOFTPLUS = 7
+# dmpnn_enrichment_loss methods (include/dmpnn.h), by NLogProbEnrichment's names
+ENRICH_METHODS = {"sqrt": 0, "score": 1, "wald": 2}
 # dmpnn_regression_loss kinds and dmpnn_spectral_transform activations (include/dmpnn.h)
 LOSS_MSE, LOSS_MAE, LOSS_RMSE = range(3)
 SPEC_SOFTPLUS, SPEC_EXP = range(2)

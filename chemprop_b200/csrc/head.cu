@@ -16,9 +16,11 @@
 //   dmpnn_mve_loss, dmpnn_evidential_loss, dmpnn_quantile_loss, dmpnn_dirichlet_loss
 //                        the uncertainty criteria (metrics.py:202-257, 502-544, 588-613) under the same reduction, one launch
 //   dmpnn_regression_loss  MSE / MAE / RMSE and their bounded variants (metrics.py:128-169); dmpnn_mse_loss is its MSE case
+//   dmpnn_enrichment_loss  NLogProbEnrichment (metrics.py:616-692) on b x 1 predictions and b x 2 counts, one launch
 //   dmpnn_spectral_transform(_bwd), dmpnn_sid_loss, dmpnn_wasserstein_loss
 //                        SpectralFFN's output and the SID / Wasserstein criteria (predictors.py:342-376, metrics.py:547-585),
 //                        one CTA per spectrum row
+#include <float.h>
 #include <math_constants.h>
 
 #include <algorithm>
@@ -311,7 +313,7 @@ k_class_probs(const float* __restrict__ P, int64_t ldp, int64_t B, int T, int C,
 // ---- uncertainty predictors (chemprop/nn/predictors.py:172-228, 250-270, 319-336; nn/metrics.py:202-257, 502-544,
 // 588-613) ------------------------------------------------------------------------------------------------------------
 enum PredKind { kRegression = 0, kMve = 1, kEvidential = 2, kQuantile = 3, kDirichlet = 4, kDirichletProbs = 5,
-                kDirichletBinary = 6 };
+                kDirichletBinary = 6, kSoftplus = 7 };
 
 // F.softplus(x) (beta 1, threshold 20) and its derivative as torch's softplus_backward computes it
 __device__ __forceinline__ float softplus20(float x) { return x > 20.f ? x : log1pf(expf(x)); }
@@ -355,6 +357,7 @@ k_pred_transform(const float* __restrict__ X, int64_t ldx, int64_t B, int T, int
     auto unscale_var = [&](float v) { return scale ? __fmul_rn(v, s2) : v; };
     switch (kind) {
       case kRegression: o[0] = unscale(x[t]); break;
+      case kSoftplus: o[0] = softplus20(x[t]); break;
       case kMve:
         o[0] = unscale(x[t]);
         o[1] = unscale_var(softplus20(x[T + t]));
@@ -390,7 +393,7 @@ k_pred_transform(const float* __restrict__ X, int64_t ldx, int64_t B, int T, int
   }
 }
 
-// mirror of k_pred_transform for kinds kRegression .. kDirichlet: dOut (B x T x u) -> dX (B x (T*u))
+// mirror of k_pred_transform for kinds kRegression .. kDirichlet and kSoftplus: dOut (B x T x u) -> dX (B x (T*u))
 __global__ void __launch_bounds__(256)
 k_pred_transform_bwd(const float* __restrict__ X, int64_t ldx, const float* __restrict__ dO, int64_t lddo, int64_t B, int T,
                      int kind, int u, const float* __restrict__ scale, float* __restrict__ dX, int64_t lddx) {
@@ -404,6 +407,7 @@ k_pred_transform_bwd(const float* __restrict__ X, int64_t ldx, const float* __re
     const float s = scale ? scale[t] : 1.f, s2 = s * s;
     switch (kind) {
       case kRegression: d[t] = g[0] * s; break;
+      case kSoftplus: d[t] = g[0] * softplus20_grad(x[t]); break;
       case kMve:
         d[t] = g[0] * s;
         d[T + t] = g[1] * s2 * softplus20_grad(x[T + t]);
@@ -563,6 +567,78 @@ k_uq_loss(const float* __restrict__ P, int64_t ldp, const float* __restrict__ Y,
       term(P + b * ldp + (int64_t)t * u, y, d);
       const float sc = loss_weight(w, tw, b, t) * inv_n;
       for (int c = 0; c < u; ++c) d[c] *= sc;
+    }
+}
+
+// ---- NLogProbEnrichment (chemprop/nn/metrics.py:616-692) ----------------------------------------------------------------
+enum EnrichMethod { kEnrichSqrt = 0, kEnrichScore = 1, kEnrichWald = 2 };
+
+// training_step's nan_to_num(nan=0.0): NaN -> 0, +-inf -> +-FLT_MAX
+__device__ __forceinline__ float nan_to_num0(float y) {
+  return isnan(y) ? 0.f : fminf(fmaxf(y, -FLT_MAX), FLT_MAX);
+}
+
+// the loss term of one molecule and dL/dR (*g): z = get_zstats(R, k1, k2) with Rd = R / d, c = clamp(z / zscale, +-zi),
+// L = -log(1 - erf(|c| / sqrt 2)).  1 - erf(x) is erfc(x) = erfcx(x) e^{-x^2}, so L = x^2 - log(erfcx(x)): a sum of two
+// non-negative terms, exact to f32 rounding at any |c| (the reference's f32 1 - erf cancels near its default zi = 5), and
+// dL/d|c| = sqrt(2 / pi) / erfcx(x).  The gradient follows torch's autograd: the clamp passes it at its bounds (inclusive)
+// and not outside, d|c|/dc = 0 at c = 0.  A NaN z stays NaN through the clamp, so L and *g are NaN.
+__device__ __forceinline__ float enrichment_term(float R, float k1, float k2, float d, int method, float zscale, float zi,
+                                                 float* g) {
+  const float Rd = R / d;
+  float z, dz;                                                 // z and dz / dRd
+  if (method == kEnrichScore) {
+    const float D = sqrtf((k1 + k2) * Rd);
+    z = (k1 - k2 * Rd) / D;
+    dz = -k2 / D - z / (2.f * Rd);
+  } else if (method == kEnrichWald) {
+    const float D = sqrtf(k1 + k2 * (Rd * Rd));
+    z = (k1 - k2 * Rd) / D;
+    dz = -k2 / D - z * k2 * Rd / (D * D);
+  } else {
+    const float A = sqrtf(k1 + 0.375f), Bq = sqrtf((k2 + 0.375f) * Rd), S = sqrtf(1.f + Rd);
+    z = 2.f * (A - Bq) / S;
+    dz = -(k2 + 0.375f) / (Bq * S) - z / (2.f * (1.f + Rd));
+  }
+  const float c = z / zscale;
+  const float cl = c < -zi ? -zi : (c > zi ? zi : c);          // NaN compares false both ways and stays NaN
+  const float x = fabsf(cl) * 0.70710678118654752f;
+  const float ex = erfcxf(x);
+  const float dLdc = (cl > 0.f ? 1.f : (cl < 0.f ? -1.f : 0.f)) * 0.79788456080286536f / ex;
+  const float pass = (c >= -zi && c <= zi) ? 1.f / zscale : 0.f;
+  *g = dLdc * pass * dz / d;
+  return x * x - logf(ex);
+}
+
+// one block: loss[0] = sum_b L_b w_b (tw_0 m_b0 + tw_1 m_b1) / sum m (m = isfinite(Y), the reference's b x 1 loss broadcast
+// against its b x 2 mask), dR = dloss/dR.  Every molecule's term enters the sum, masked ones with weight 0, so a NaN z
+// anywhere (the reference raises) makes loss[0] NaN.
+__global__ void __launch_bounds__(1024)
+k_enrichment_loss(const float* __restrict__ R, int64_t ldr, const float* __restrict__ Y, int64_t ldy,
+                  const float* __restrict__ w, const float* __restrict__ tw, int64_t B, float d, int method, float zscale,
+                  float zi, float* __restrict__ loss, float* __restrict__ dR, int64_t lddr) {
+  const float tw0 = tw ? tw[0] : 1.f, tw1 = tw ? tw[1] : 1.f;
+  auto row = [&](int64_t b, float* wr, float* g) {
+    const float y1 = Y[b * ldy], y2 = Y[b * ldy + 1];
+    const bool m1 = isfinite(y1), m2 = isfinite(y2);
+    *wr = (w ? w[b] : 1.f) * ((m1 ? tw0 : 0.f) + (m2 ? tw1 : 0.f));
+    return enrichment_term(R[b * ldr], nan_to_num0(y1), nan_to_num0(y2), d, method, zscale, zi, g);
+  };
+  float l = 0.f, cnt = 0.f;
+  for (int64_t b = threadIdx.x; b < B; b += blockDim.x) {
+    float wr, g;
+    const float L = row(b, &wr, &g);
+    l = fmaf(wr, L, l);
+    cnt += (float)(isfinite(Y[b * ldy]) + isfinite(Y[b * ldy + 1]));
+  }
+  const float2 tot = block_sum2(l, cnt);
+  if (threadIdx.x == 0) loss[0] = tot.y > 0.f ? tot.x / tot.y : tot.x;      // all masked: 0, or NaN from a NaN z
+  const float inv_n = tot.y > 0.f ? 1.f / tot.y : 0.f;
+  if (dR != nullptr)
+    for (int64_t b = threadIdx.x; b < B; b += blockDim.x) {
+      float wr, g;
+      row(b, &wr, &g);
+      dR[b * lddr] = wr * inv_n * g;
     }
 }
 
@@ -878,7 +954,7 @@ extern "C" int dmpnn_class_probs(const float* P, int64_t ldp, int64_t B, int64_t
 // outputs per task of each kind; 0 = any u >= 1 (the Dirichlet kinds: the number of classes)
 static int pred_kind_u(int kind) {
   switch (kind) {
-    case head::kRegression: return 1;
+    case head::kRegression: case head::kSoftplus: return 1;
     case head::kMve: case head::kQuantile: case head::kDirichletBinary: return 2;
     case head::kEvidential: return 4;
     default: return 0;
@@ -888,7 +964,7 @@ static int pred_kind_u(int kind) {
 extern "C" int dmpnn_pred_transform(const float* X, int64_t ldx, int64_t B, int64_t T, int kind, int64_t u,
                                     const float* mean, const float* scale, float* out, int64_t ldo, void* stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
-  DMPNN_CHECK_ARG(kind >= head::kRegression && kind <= head::kDirichletBinary, "pred_transform: unknown kind");
+  DMPNN_CHECK_ARG(kind >= head::kRegression && kind <= head::kSoftplus, "pred_transform: unknown kind");
   DMPNN_CHECK_ARG(B >= 0 && T > 0 && u > 0 && T * u <= INT32_MAX && (B == 0 || (X && out)), "pred_transform: bad args");
   DMPNN_CHECK_ARG(pred_kind_u(kind) == 0 || pred_kind_u(kind) == u, "pred_transform: u does not match the kind");
   DMPNN_CHECK_ARG((mean == nullptr && scale == nullptr) || (kind <= head::kQuantile && mean && scale),
@@ -904,7 +980,8 @@ extern "C" int dmpnn_pred_transform(const float* X, int64_t ldx, int64_t B, int6
 extern "C" int dmpnn_pred_transform_bwd(const float* X, int64_t ldx, const float* dOut, int64_t lddo, int64_t B, int64_t T,
                                         int kind, int64_t u, const float* scale, float* dX, int64_t lddx, void* stream_) {
   cudaStream_t st = (cudaStream_t)stream_;
-  DMPNN_CHECK_ARG(kind >= head::kRegression && kind <= head::kDirichlet, "pred_transform_bwd: unknown kind");
+  DMPNN_CHECK_ARG((kind >= head::kRegression && kind <= head::kDirichlet) || kind == head::kSoftplus,
+                  "pred_transform_bwd: unknown kind");
   DMPNN_CHECK_ARG(B >= 0 && T > 0 && u > 0 && T * u <= INT32_MAX && (B == 0 || (X && dOut && dX)),
                   "pred_transform_bwd: bad args");
   DMPNN_CHECK_ARG(pred_kind_u(kind) == 0 || pred_kind_u(kind) == u, "pred_transform_bwd: u does not match the kind");
@@ -1041,4 +1118,20 @@ extern "C" int dmpnn_wasserstein_loss(const float* P, int64_t ldp, const float* 
                                       float* dP, int64_t lddp, void* workspace, void* stream) {
   return spectral_loss<true>("wasserstein_loss", P, ldp, Y, ldy, weights, task_weights, B, T, threshold, loss, dP, lddp,
                              workspace, stream);
+}
+
+extern "C" int dmpnn_enrichment_loss(const float* R, int64_t ldr, const float* Y, int64_t ldy, const float* weights,
+                                     const float* task_weights, int64_t B, float d, int method, float zscale, float zinterval,
+                                     float* loss, float* dR, int64_t lddr, void* stream_) {
+  cudaStream_t st = (cudaStream_t)stream_;
+  DMPNN_CHECK_ARG(method >= head::kEnrichSqrt && method <= head::kEnrichWald, "enrichment_loss: unknown method");
+  DMPNN_CHECK_ARG(std::isfinite(d) && d > 0.f && std::isfinite(zscale) && zscale != 0.f && std::isfinite(zinterval) &&
+                      zinterval >= 0.f, "enrichment_loss: d must be finite and > 0, zscale finite and nonzero, zinterval "
+                  "finite and >= 0");
+  DMPNN_CHECK_ARG(B >= 0 && loss && (B == 0 || (R && Y)), "enrichment_loss: bad args");
+  DMPNN_CHECK_ARG(ldr >= 1 && ldy >= 2 && (dR == nullptr || lddr >= 1), "enrichment_loss: row strides too small");
+  head::k_enrichment_loss<<<1, 1024, 0, st>>>(R, ldr, Y, ldy, weights, task_weights, B, d, method, zscale, zinterval, loss,
+                                              dR, lddr);
+  DMPNN_CHECK_LAUNCH("enrichment_loss", 1);
+  return 0;
 }

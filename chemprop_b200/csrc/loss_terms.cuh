@@ -31,4 +31,16 @@ __device__ __forceinline__ float reg_residual(float p, float y, const uint8_t* l
   return p - y;
 }
 
+// PointQuantileLoss (metrics.py:282-285): alpha (y - p) where y - p > 0, (1 - alpha)(p - y) otherwise; *g = dL/dp, which at
+// y == p is torch.where's second branch, 1 - alpha
+__device__ __forceinline__ float pinball_term(float p, float y, float alpha, float* g) {
+  const float d = y - p;
+  if (d > 0.f) {
+    *g = -alpha;
+    return alpha * d;
+  }
+  *g = 1.f - alpha;
+  return (1.f - alpha) * -d;
+}
+
 }  // namespace dmpnn

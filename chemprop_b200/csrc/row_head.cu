@@ -6,6 +6,8 @@
 //   dmpnn_regression_loss_rows   dmpnn_regression_loss (MSE / MAE / RMSE, bounded or not) spread over the whole grid
 //   dmpnn_bce_loss_rows          dmpnn_bce_loss spread over the whole grid
 //   dmpnn_ce_loss_rows           dmpnn_ce_loss spread over the whole grid
+//   dmpnn_pinball_loss_rows      PointQuantileLoss (chemprop/nn/metrics.py:264-288) over the whole grid, at every level: it
+//                                has no single-block twin, molecules run it too
 //
 // The _rows criteria keep their single-block twins' arguments, conventions and outputs.  Their reduction is two-phase: each
 // CTA of the first launch sums a fixed contiguous chunk of the (row, task) terms into one partial in the workspace; each CTA
@@ -15,6 +17,7 @@
 #include <math_constants.h>
 
 #include <algorithm>
+#include <cmath>
 
 #include "common.cuh"
 #include "loss_terms.cuh"
@@ -26,7 +29,7 @@ constexpr int kThreads = 256;
 constexpr int kMaxBlocks = 1024;
 constexpr int64_t kMinChunk = 2048;      // elements per CTA at least: below that the second launch's partial sum dominates
 
-enum RowLoss { kMse = 0, kMae = 1, kRmse = 2, kBce = 3, kCe = 4 };
+enum RowLoss { kMse = 0, kMae = 1, kRmse = 2, kBce = 3, kCe = 4, kPinball = 5 };
 
 struct Args {
   const float* P;
@@ -44,6 +47,7 @@ struct Args {
   float* loss;
   float* dP;
   int64_t lddp;
+  float alpha;                           // kPinball's quantile
 };
 
 // fixed-order block sum of (l, n): lanes by a shuffle tree, then the warp partials in order; every thread gets the totals
@@ -85,6 +89,10 @@ __device__ __forceinline__ float term(const Args& a, int64_t b, int t, float y) 
   }
   const float p = a.P[b * a.ldp + t];
   if (L == kBce) return ww * bce_with_logits(p, y);
+  if (L == kPinball) {
+    float g;
+    return ww * pinball_term(p, y, a.alpha, &g);
+  }
   const float e = reg_residual(p, y, a.lt, a.gt, b * a.ldm + t);
   if (L == kMae) return ww * fabsf(e);
   return ww * e * e;
@@ -159,6 +167,9 @@ k_row_loss_finish(Args a, int64_t chunk, int G, const float* __restrict__ part_l
       const float p = a.P[b * a.ldp + t];
       if (L == kBce) {
         g = (sigmoid_stable(p) - y) * ww * inv_n;
+      } else if (L == kPinball) {
+        pinball_term(p, y, a.alpha, &g);
+        g *= ww * inv_n;
       } else {
         const float e = reg_residual(p, y, a.lt, a.gt, b * a.ldm + t);
         if (L == kMae) g = ww * (e > 0.f ? 1.f : (e < 0.f ? -1.f : 0.f)) * inv_n;
@@ -272,6 +283,12 @@ extern "C" int dmpnn_ce_loss_rows_workspace_bytes(int64_t B, int64_t T, size_t* 
   return 0;
 }
 
+extern "C" int dmpnn_pinball_loss_rows_workspace_bytes(int64_t B, int64_t T, size_t* bytes) {
+  DMPNN_CHECK_ARG(B >= 0 && T > 0 && bytes, "pinball_loss_rows_workspace_bytes: bad args");
+  *bytes = rowhead::workspace_bytes(B * T);
+  return 0;
+}
+
 extern "C" int dmpnn_regression_loss_rows(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
                                           const float* task_weights, const uint8_t* lt_mask, const uint8_t* gt_mask,
                                           int64_t ldm, int64_t B, int64_t T, int kind, float* loss, float* dP, int64_t lddp,
@@ -304,4 +321,15 @@ extern "C" int dmpnn_ce_loss_rows(const float* P, int64_t ldp, const float* Y, i
   DMPNN_CHECK_ARG(ldp >= T * C && ldy >= T && (dP == nullptr || lddp >= T * C), "ce_loss_rows: row strides too small");
   const rowhead::Args a{P, ldp, Y, ldy, weights, task_weights, nullptr, nullptr, 0, B, (int)T, (int)C, loss, dP, lddp};
   return rowhead::row_loss<rowhead::kCe>("ce_loss_rows", a, workspace, stream);
+}
+
+extern "C" int dmpnn_pinball_loss_rows(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                                       const float* task_weights, int64_t B, int64_t T, float alpha, float* loss, float* dP,
+                                       int64_t lddp, void* workspace, void* stream) {
+  DMPNN_CHECK_ARG(std::isfinite(alpha), "pinball_loss_rows: alpha must be finite");
+  DMPNN_CHECK_ARG(B >= 0 && T > 0 && T <= INT32_MAX && loss && workspace && (B == 0 || (P && Y)),
+                  "pinball_loss_rows: bad args");
+  DMPNN_CHECK_ARG(ldp >= T && ldy >= T && (dP == nullptr || lddp >= T), "pinball_loss_rows: row strides too small");
+  const rowhead::Args a{P, ldp, Y, ldy, weights, task_weights, nullptr, nullptr, 0, B, (int)T, 1, loss, dP, lddp, alpha};
+  return rowhead::row_loss<rowhead::kPinball>("pinball_loss_rows", a, workspace, stream);
 }

@@ -684,6 +684,18 @@ def regression_loss(P: Tensor, Y: Tensor, w, tw, lt_mask, gt_mask, kind: int, lo
     _lib.check(rc, "dmpnn_regression_loss")
 
 
+def enrichment_loss(P: Tensor, Y: Tensor, w, tw, d: float, method: int, zscale: float, zinterval: float, loss: Tensor,
+                    dP: Tensor):
+    """NLogProbEnrichment on P (B x 1, the predicted enrichment) and Y (B x 2 counts k1, k2; NaN = masked); tw has 2
+    entries, d = n2 / n1, method by _lib.ENRICH_METHODS."""
+    lib = _lib.load()
+    B = P.shape[0]
+    rc = lib.dmpnn_enrichment_loss(P.data_ptr(), P.stride(0) if B else 1, Y.data_ptr(), Y.stride(0) if B else 2, _ptr(w),
+                                   _ptr(tw), B, float(d), method, float(zscale), float(zinterval), loss.data_ptr(), _ptr(dP),
+                                   dP.stride(0) if B else 1, _stream())
+    _lib.check(rc, "dmpnn_enrichment_loss")
+
+
 def spectral_transform(X: Tensor, act: int, out: Tensor):
     """out (B x T) = a(a(X)) normalised per row, a = softplus or exp (_lib.SPEC_*)."""
     lib = _lib.load()
@@ -771,6 +783,17 @@ def bce_loss_rows(P: Tensor, Y: Tensor, w, tw, loss: Tensor, dP: Tensor):
     rc = lib.dmpnn_bce_loss_rows(P.data_ptr(), P.stride(0) if B else T, Y.data_ptr(), Y.stride(0) if B else T, _ptr(w),
                                  _ptr(tw), B, T, loss.data_ptr(), _ptr(dP), dP.stride(0) if B else T, ws.data_ptr(), _stream())
     _lib.check(rc, "dmpnn_bce_loss_rows")
+
+
+def pinball_loss_rows(P: Tensor, Y: Tensor, w, tw, alpha: float, loss: Tensor, dP: Tensor):
+    """PointQuantileLoss at `alpha` over the whole grid (dmpnn_pinball_loss_rows), for molecule, atom or bond rows."""
+    lib = _lib.load()
+    B, T = P.shape
+    ws = _rows_workspace("dmpnn_pinball_loss_rows", B, T, P.device)
+    rc = lib.dmpnn_pinball_loss_rows(P.data_ptr(), P.stride(0) if B else T, Y.data_ptr(), Y.stride(0) if B else T, _ptr(w),
+                                     _ptr(tw), B, T, float(alpha), loss.data_ptr(), _ptr(dP), dP.stride(0) if B else T,
+                                     ws.data_ptr(), _stream())
+    _lib.check(rc, "dmpnn_pinball_loss_rows")
 
 
 def ce_loss_rows(P: Tensor, Y: Tensor, w, tw, C_: int, loss: Tensor, dP: Tensor):

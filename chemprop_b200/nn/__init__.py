@@ -4,7 +4,7 @@ from .constrainer import ConstrainerFFN
 from .head import (EngineBatchNorm1d, EngineBinaryClassificationFFN, EngineBinaryDirichletFFN, EngineBoundedMAE,
                    EngineBoundedMSE, EngineBoundedRMSE, EngineDirichletLoss, EngineEvidentialFFN, EngineEvidentialLoss,
                    EngineLinear, EngineMAE, EngineMPNN, EngineMulticlassClassificationFFN, EngineMulticlassDirichletFFN,
-                   EngineMveFFN, EngineMVELoss, EngineQuantileFFN, EngineQuantileLoss, EngineRegressionFFN, EngineRMSE,
+                   EngineMveFFN, EngineMVELoss, EngineNLogProbEnrichment, EnginePointQuantileLoss, EngineQuantileFFN, EngineQuantileLoss, EngineRegressionFFN, EngineRMSE,
                    EngineSID, EngineSpectralFFN, EngineWasserstein)
 from .message_passing import AtomMessagePassing, BondMessagePassing
 from .metrics import EngineCriterionMetric, EngineMetric, EngineMetricRegistry
@@ -20,6 +20,6 @@ __all__ = ["Aggregation", "AggregationRegistry", "AttentiveAggregation", "MeanAg
            "EngineQuantileFFN", "EngineBinaryDirichletFFN", "EngineMulticlassDirichletFFN", "EngineMVELoss",
            "EngineEvidentialLoss", "EngineQuantileLoss", "EngineDirichletLoss", "EngineSpectralFFN", "EngineSID",
            "EngineWasserstein", "EngineMAE", "EngineRMSE", "EngineBoundedMSE", "EngineBoundedMAE", "EngineBoundedRMSE",
-           "EngineBatchNorm1d", "EngineLinear", "EngineMolAtomBondMPNN",
+           "EngineBatchNorm1d", "EngineLinear", "EngineNLogProbEnrichment", "EnginePointQuantileLoss", "EngineMolAtomBondMPNN",
            "EngineMulticomponentMessagePassing", "EngineMulticomponentMPNN", "EngineMetric", "EngineMetricRegistry",
            "EngineCriterionMetric"]

@@ -29,6 +29,7 @@ from .. import engine as K
 from .agg import Aggregation, MeanAggregation
 from .constrainer import build_mlp
 from .message_passing import DEFAULT_HIDDEN_DIM, engine_activation, is_fused_activation
+from .transforms import UnscaleTransform
 
 
 class BatchNormTrainFunction(torch.autograd.Function):
@@ -251,7 +252,7 @@ class PredTransformFunction(torch.autograd.Function):
         kind, u, dt = ctx.cfg
         b, n = Xc.shape
         g = g.float().reshape(b, n).contiguous()
-        if kind <= _lib.PRED_DIRICHLET:
+        if kind <= _lib.PRED_DIRICHLET or kind == _lib.PRED_SOFTPLUS:
             dX = torch.empty_like(Xc)
             K.pred_transform_bwd(Xc, g, kind, u, s, dX)
         else:
@@ -279,17 +280,15 @@ def _loss_weights(weights, task_weights, b: int, T: int):
 
 
 class CriterionLossFunction(torch.autograd.Function):
-    """A criterion's loss and dLoss/dPreds in one launch, at any level.  `preds` is b x T, or b x T x u when `grouped` (u
-    values per task: class logits, the uncertainty predictors' outputs), and `targets` b x T.  `launch(P, Y, w, tw, lt, gt,
-    loss, dP)` (_Criterion._loss) gets them as b x (T*u) and b x T f32, the weights as exactly b and T entries
-    (_loss_weights) and the bound masks as b x T uint8 (None where not given); it writes loss[0] and dP."""
+    """A criterion's loss and dLoss/dPreds in one launch, at any level.  `preds` is b x T, or b x T x u (u values per task:
+    class logits, the uncertainty predictors' outputs), and `targets` b x T' -- which shapes go together is the criterion's
+    rule, checked before this runs (_Criterion._check_shapes).  `launch(P, Y, w, tw, lt, gt, loss, dP)` (_Criterion._loss)
+    gets them as b x (T*u) and b x T' f32, the weights as exactly b and T' entries (_loss_weights) and the bound masks as
+    b x T' uint8 (None where not given); it writes loss[0] and dP."""
 
     @staticmethod
-    def forward(ctx, preds, targets, weights, task_weights, lt_mask, gt_mask, launch, grouped):
+    def forward(ctx, preds, targets, weights, task_weights, lt_mask, gt_mask, launch):
         K._require_cuda(preds, targets, lt_mask, gt_mask)
-        if preds.dim() != (3 if grouped else 2) or targets.shape != preds.shape[:2]:
-            raise ValueError(f"expected {'b x T x u' if grouped else 'b x T'} predictions and b x T targets, got "
-                             f"{tuple(preds.shape)} and {tuple(targets.shape)}")
         b, T = targets.shape
         P, Y = preds.float().flatten(1).contiguous(), targets.float().contiguous()
         w, tw = _loss_weights(weights, task_weights, b, T)
@@ -304,7 +303,7 @@ class CriterionLossFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         (dP,) = ctx.saved_tensors
-        return (dP * g).to(ctx.pdtype), None, None, None, None, None, None, None
+        return (dP * g).to(ctx.pdtype), None, None, None, None, None, None
 
 
 # the engine wrappers that take the b x T bound masks and a _lib.LOSS_* kind after `tw`
@@ -346,17 +345,29 @@ class _Criterion(nn.Module):
     def _args(self, preds) -> tuple:
         return ()
 
+    def nan_error(self) -> str | None:
+        """The reference's error message where it raises on a NaN loss instead of returning it; None for the criteria
+        whose reference returns the NaN."""
+        return None
+
+    def _check_shapes(self, preds, targets):
+        """b x T predictions (b x T x u when `_grouped`) and b x T targets."""
+        if preds.dim() != (3 if self._grouped else 2) or targets.shape != preds.shape[:2]:
+            raise ValueError(f"expected {'b x T x u' if self._grouped else 'b x T'} predictions and b x T targets, got "
+                             f"{tuple(preds.shape)} and {tuple(targets.shape)}")
+
     def _loss(self, kernel, preds, targets, weights, lt_mask, gt_mask):
         if not self._bounded and (lt_mask is not None or gt_mask is not None):
             raise NotImplementedError(f"{type(self).__name__} takes no lt_mask / gt_mask; the bounded criteria "
                                       "(EngineBoundedMSE, EngineBoundedMAE, EngineBoundedRMSE) do")
+        self._check_shapes(preds, targets)
         fn, regression = getattr(K, kernel), kernel in _REGRESSION_WRAPPERS
+        args = () if regression else self._args(preds)          # a criterion refuses its bad arguments before any launch
 
         def launch(P, Y, w, tw, lt, gt, loss, dP):
-            fn(P, Y, w, tw, *((lt, gt, self._kind) if regression else self._args(preds)), loss, dP)
+            fn(P, Y, w, tw, *((lt, gt, self._kind) if regression else args), loss, dP)
 
-        return CriterionLossFunction.apply(preds, targets, weights, self.task_weights, lt_mask, gt_mask, launch,
-                                           self._grouped)
+        return CriterionLossFunction.apply(preds, targets, weights, self.task_weights, lt_mask, gt_mask, launch)
 
 
 class _BCECriterion(_Criterion):
@@ -441,6 +452,66 @@ class EngineDirichletLoss(_Criterion):
 
     def extra_repr(self) -> str:
         return f"v_kl={self.v_kl}"
+
+
+class EnginePointQuantileLoss(_Criterion):
+    """chemprop's PointQuantileLoss (nn/metrics.py:264-288): the pinball loss of b x T point predictions at `alpha`, alpha
+    (y - p) above the target and (1 - alpha)(p - y) elsewhere.  One row-parallel kernel at every level
+    (dmpnn_pinball_loss_rows)."""
+    _kernel = "pinball_loss_rows"
+    _row_kernel = "pinball_loss_rows"
+
+    def __init__(self, task_weights=1.0, alpha: float = 0.1):
+        super().__init__(task_weights)
+        self.alpha = alpha
+
+    def _args(self, preds) -> tuple:
+        return (self.alpha,)
+
+    def extra_repr(self) -> str:
+        return f"alpha={self.alpha}"
+
+
+class EngineNLogProbEnrichment(_Criterion):
+    """chemprop's NLogProbEnrichment (nn/metrics.py:616-692), the loss of DNA-encoded-library screening counts, on b x 1
+    predicted enrichments R (EngineRegressionFFN with its Softplus output) and b x 2 count targets (k1 in the positive
+    sample, k2 in the counter sample; NaN = masked, counted as 0 in z as training_step's nan_to_num does): -log of the
+    two-sided Poisson-ratio p-value of z = get_zstats(R, k1, k2, n1, n2, method), clamped at +-zinterval after dividing by
+    zscale; the molecule's loss counts once per unmasked count, as the reference broadcasts its b x 1 loss against the
+    b x 2 mask.  Task weights have 1 or 2 entries.  One launch (dmpnn_enrichment_loss); no row kernel.
+
+    Where the reference raises ("Got nan loss": a NaN z anywhere in the batch, e.g. method "score" or "wald" with a row of
+    zero counts) the loss is NaN instead, so that a training step never synchronises with the host and captures into a
+    CUDA graph; `EngineMPNN.evaluate` raises the reference's ValueError at its one host sync."""
+    _kernel = "enrichment_loss"
+    _row_kernel = None
+
+    def __init__(self, task_weights=1.0, n1: int = 1, n2: int = 1, method: str = "sqrt", zscale: float = 1.0,
+                 zinterval: float = 5.0):
+        super().__init__(task_weights)
+        self.n1 = n1
+        self.n2 = n2
+        self.method = method
+        self.zscale = zscale
+        self.zinterval = zinterval
+
+    def nan_error(self) -> str:
+        """The reference's message where a z is NaN."""
+        return (f"Got nan loss with method '{self.method}', ensure row-wise sum of counts are nonzero or use "
+                "method='sqrt'")
+
+    def _check_shapes(self, preds, targets):
+        if preds.dim() != 2 or preds.shape[1] != 1 or targets.dim() != 2 or targets.shape != (preds.shape[0], 2):
+            raise ValueError(f"NLogProbEnrichment takes b x 1 predictions and b x 2 count targets (k1, k2), got "
+                             f"{tuple(preds.shape)} and {tuple(targets.shape)}")
+
+    def _args(self, preds) -> tuple:
+        if self.method not in _lib.ENRICH_METHODS:
+            raise ValueError(f"Unsupported method: {self.method}")
+        return self.n2 / self.n1, _lib.ENRICH_METHODS[self.method], self.zscale, self.zinterval
+
+    def extra_repr(self) -> str:
+        return f"n1={self.n1}, n2={self.n2}, method='{self.method}', zscale={self.zscale}, zinterval={self.zinterval}"
 
 
 class SpectralTransformFunction(torch.autograd.Function):
@@ -576,19 +647,32 @@ class _EngineFFNPredictor(nn.Module):
         return engine_mlp(self.ffn, Z)
 
 
+def _is_default_softplus(t: nn.Module) -> bool:
+    return isinstance(t, nn.Softplus) and t.beta == 1 and t.threshold == 20
+
+
 class EngineRegressionFFN(_EngineFFNPredictor):
     """`RegressionFFN` (chemprop/nn/predictors.py:160-169) with the reference's module tree; GEMMs on the engine.  With an
-    UnscaleTransform as `output_transform`, eval-mode predictions are `Y * scale + mean` (dmpnn_pred_transform)."""
+    UnscaleTransform as `output_transform`, eval-mode predictions are `Y * scale + mean` (dmpnn_pred_transform); with
+    `nn.Softplus()` (beta 1, threshold 20: the output of NLogProbEnrichment's enrichment ratios) they are softplus(Y) in
+    training and eval mode alike.  Any other output transform is refused: the engine would not apply it.  The uncertainty
+    predictors below take only an UnscaleTransform."""
     _kind = _lib.PRED_REGRESSION
 
     def _unscale(self):
         t = self.output_transform
+        if not isinstance(t, (nn.Identity, UnscaleTransform)):
+            allowed = "nn.Identity, UnscaleTransform" + (" or nn.Softplus()" if self._kind == _lib.PRED_REGRESSION else "")
+            raise ValueError(f"{type(self).__name__} runs the output transforms {allowed} (beta 1, threshold 20) on its "
+                             f"kernels; got {t!r}")
         if isinstance(t, nn.Identity) or t.training:      # UnscaleTransform is the identity in training mode
             return None, None
         return t.mean, t.scale
 
     def forward(self, Z: Tensor) -> Tensor:
         Y = self._mlp(Z)
+        if self._kind == _lib.PRED_REGRESSION and _is_default_softplus(self.output_transform):
+            return PredTransformFunction.apply(Y, _lib.PRED_SOFTPLUS, 1, None, None).view(Y.shape)
         mean, scale = self._unscale()
         if self._kind == _lib.PRED_REGRESSION:
             return Y if mean is None else PredTransformFunction.apply(Y, self._kind, 1, mean, scale).view(Y.shape)
@@ -827,7 +911,8 @@ class EngineMPNN(nn.Module):
         targets per task, and mask non-finite targets.  `metrics` (EngineMetric objects, reset here) default to the
         predictor's default metric (nn.metrics.default_metric).  Runs under no_grad, restores every module's training flag,
         and synchronises with the host once, at the end.  Returns {"val_loss": .., "val/<alias>": ..} or
-        {"test/<alias>": ..}; raises ValueError where an update met a target its metric cannot take."""
+        {"test/<alias>": ..}; raises ValueError where an update met a target its metric cannot take, or where the
+        NLogProbEnrichment criterion (as the loss or as a metric) met a NaN z, with the reference's message."""
         from .metrics import EngineCriterionMetric, default_metric
 
         if stage not in ("val", "test"):
@@ -856,16 +941,19 @@ class EngineMPNN(nn.Module):
                     if loss is not None:     # validation_step: the same fingerprint through train_step
                         loss.update(self.predictor.train_step(Z), targets, mask, weights, lt_mask, gt_mask)
                 values = [m.compute() for m in metrics] + ([] if loss is None else [loss.compute()])
-                checked = [m for m in metrics if m._status is not None]
+                checked = [m for m in metrics + ([] if loss is None else [loss]) if m._status is not None]
                 host = torch.stack([v.double().reshape(()) for v in values]
                                    + [m._status.double().reshape(()) for m in checked]).tolist()
         finally:
             for m, f in flags:
                 m.training = f
-        bad = [m.alias for m, s in zip(checked, host[len(values):]) if s]
+        bad = [m for m, s in zip(checked, host[len(values):]) if s]
+        for m in bad:                   # a criterion whose reference raises on a NaN loss (EngineNLogProbEnrichment)
+            if isinstance(m, EngineCriterionMetric):
+                raise ValueError(m.criterion.nan_error())
         if bad:
-            raise ValueError(f"metric(s) {bad}: a target is not a valid label (binary targets must be 0 or 1, class "
-                             "targets in [-C, C))")
+            raise ValueError(f"metric(s) {[m.alias for m in bad]}: a target is not a valid label (binary targets must be 0 "
+                             "or 1, class targets in [-C, C))")
         out = {f"{stage}/{m.alias}": v for m, v in zip(metrics, host)}
         if loss is not None:
             out = {"val_loss": host[len(metrics)], **out}

@@ -339,7 +339,9 @@ class EngineCriterionMetric(EngineMetric):
     """Any engine criterion as the reference's validation-loss accumulator (`MPNN.metrics[-1]`, models/model.py:99-103,
     181): each update adds the criterion's batch value times the batch's mask count in f64 -- every engine criterion
     reduces a batch to sum L w tw m / sum m, so the sum is the reference's `total_loss` -- and `compute` divides by the
-    total count.  For the RMSE criteria the value squared times the count is added, and `compute` takes the sqrt."""
+    total count.  For the RMSE criteria the value squared times the count is added, and `compute` takes the sqrt.  A criterion
+    whose reference raises where its loss is NaN (`nan_error()` not None: EngineNLogProbEnrichment) sets the status flag on a
+    NaN batch value, and `EngineMPNN.evaluate` raises the reference's error."""
     _n_f, _n_i = 1, 1
 
     def __init__(self, criterion):
@@ -359,9 +361,11 @@ class EngineCriterionMetric(EngineMetric):
         n = m.sum()
         self._f.add_((v * v if self._rmse else v) * n)
         self._i.add_(n)
+        if self.criterion.nan_error() is not None:
+            self._status.bitwise_or_(v.isnan().to(torch.int32))
 
     def _states(self) -> list[Tensor]:
-        return [self._f, self._i]
+        return [self._f, self._i, self._status]
 
     def compute(self) -> Tensor:
         v = self._f[0] / self._i[0]

@@ -518,12 +518,14 @@ int dmpnn_class_probs(const float* P, int64_t ldp, int64_t B, int64_t T, int64_t
  *                               4 Dirichlet (u = C >= 1)   alpha = softplus(x) + 1
  *                               5 Dirichlet probabilities  alpha / sum(alpha)
  *                               6 binary Dirichlet (u = 2) (alpha_1 / S, 2 / S), S = alpha_0 + alpha_1
+ *                               7 softplus (u = 1)         softplus(x): RegressionFFN's nn.Softplus() output transform
+ *                                                          (beta 1, threshold 20), in training and eval mode
  *                             Kinds 0-3 read target j of task t from column j*T + t (torch.chunk of the MLP output);
  *                             kinds 4-6 read class c of task t from column t*u + c (reshape(B, T, u)).  softplus is
  *                             F.softplus with threshold 20.  mean and scale (T entries each, both or neither, kinds 0-3
  *                             only) apply UnscaleTransform's eval mode: x*scale + mean to the mean / bounds, var*scale^2
  *                             to MVE's var and evidential's beta, each product and sum rounded as torch rounds it.
- *   dmpnn_pred_transform_bwd  the mirror for kinds 0-4: dX (B x (T*u)) from dOut (B x T x u) and the forward's X; scale
+ *   dmpnn_pred_transform_bwd  the mirror for kinds 0-4 and 7: dX (B x (T*u)) from dOut (B x T x u) and the forward's X; scale
  *                             (nullable) as in the forward.  Every column of dX in [0, T*u) is written.
  *   dmpnn_mve_loss            MVELoss on P (B x T x 2: mean, var): L = (mean - y)^2 / (2 var) + log(2 pi var) / 2
  *   dmpnn_evidential_loss     EvidentialLoss on P (B x T x 4: mean, v, alpha, beta) with v_kl and eps; d|r|/dr = 0 at r = 0
@@ -553,6 +555,31 @@ int dmpnn_quantile_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy
 int dmpnn_dirichlet_loss(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
                          const float* task_weights, int64_t B, int64_t T, int64_t C, float v_kl, float* loss, float* dP,
                          int64_t lddp, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Count-data regression (csrc/head.cu; chemprop/nn/metrics.py:616-692, the loss of DNA-encoded-library screens):
+ *   dmpnn_enrichment_loss     NLogProbEnrichment on R (B x 1, row stride ldr: the predicted enrichment, softplus output)
+ *                             and Y (B x 2, row stride ldy: counts k1 in the positive and k2 in the negative sample).
+ *                             Per molecule, with k = Y where finite and 0 where not (training_step's nan_to_num) and
+ *                             Rd = R / d (d = n2 / n1):
+ *                               method 0 sqrt   z = 2 (sqrt(k1 + 3/8) - sqrt((k2 + 3/8) Rd)) / sqrt(1 + Rd)
+ *                               method 1 score  z = (k1 - k2 Rd) / sqrt((k1 + k2) Rd)
+ *                               method 2 wald   z = (k1 - k2 Rd) / sqrt(k1 + k2 Rd^2)
+ *                             c = clamp(z / zscale, -zinterval, zinterval), L = -log(1 - erf(|c| / sqrt 2)), computed as
+ *                             x^2 - log(erfcx(x)) with x = |c| / sqrt 2 (no cancellation, no underflow).  loss[0] =
+ *                             sum_b L_b w[b] (tw[0] m_b0 + tw[1] m_b1) / sum m with m = isfinite(Y): the reference's b x 1
+ *                             loss broadcast against its b x 2 mask.  task_weights (nullable) has exactly 2 entries.
+ *                             dR (nullable, row stride lddr) = dloss/dR for every row, masked ones 0; the clamp passes
+ *                             the gradient at its bounds (inclusive) and not outside, d|c|/dc = 0 at c = 0, as torch's
+ *                             autograd.  Where the reference raises ("Got nan loss", any NaN z, masked rows included:
+ *                             score / wald with a row of zero counts, a NaN prediction) loss[0] is NaN, and so is that
+ *                             row's dR.  Every target masked: loss[0] = 0 and dR = 0.  One block; fixed reduction order;
+ *                             no atomics; no host synchronisation.  Refused: an unknown method, d not finite and > 0,
+ *                             zscale not finite and nonzero, zinterval not finite and >= 0.
+ * ------------------------------------------------------------------------------------- */
+int dmpnn_enrichment_loss(const float* R, int64_t ldr, const float* Y, int64_t ldy, const float* weights,
+                          const float* task_weights, int64_t B, float d, int method, float zscale, float zinterval,
+                          float* loss, float* dR, int64_t lddr, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Regression-loss family and the spectral predictor (csrc/head.cu; chemprop/nn/metrics.py:128-183, 547-585,
@@ -610,6 +637,10 @@ int dmpnn_wasserstein_loss(const float* P, int64_t ldp, const float* Y, int64_t 
  *                             without synchronising with the host).  E must be even (refused otherwise); E = 0 launches
  *                             nothing.
  *   dmpnn_edge_pair_mean_bwd  its mirror: dP[2i] = dP[2i+1] = G[i] / 2.
+ *   dmpnn_pinball_loss_rows   PointQuantileLoss (chemprop/nn/metrics.py:264-288) at `alpha`, under the _rows reduction
+ *                             below and at every level (molecules included: it has no single-block twin): L =
+ *                             alpha (y - p) where y - p > 0, (1 - alpha)(p - y) otherwise; dL/dp at y == p is 1 - alpha
+ *                             (torch.where's second branch).
  *   dmpnn_regression_loss_rows, dmpnn_bce_loss_rows, dmpnn_ce_loss_rows
  *                             dmpnn_regression_loss, dmpnn_bce_loss and dmpnn_ce_loss with the same arguments, conventions
  *                             and outputs (NaN targets masked, w and tw nullable, division by the mask count, loss 0 and
@@ -635,6 +666,10 @@ int dmpnn_bce_loss_rows_workspace_bytes(int64_t B, int64_t T, size_t* bytes);
 int dmpnn_bce_loss_rows(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
                         const float* task_weights, int64_t B, int64_t T, float* loss, float* dP, int64_t lddp,
                         void* workspace, void* stream);
+int dmpnn_pinball_loss_rows_workspace_bytes(int64_t B, int64_t T, size_t* bytes);
+int dmpnn_pinball_loss_rows(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
+                            const float* task_weights, int64_t B, int64_t T, float alpha, float* loss, float* dP, int64_t lddp,
+                            void* workspace, void* stream);
 int dmpnn_ce_loss_rows_workspace_bytes(int64_t B, int64_t T, size_t* bytes);
 int dmpnn_ce_loss_rows(const float* P, int64_t ldp, const float* Y, int64_t ldy, const float* weights,
                        const float* task_weights, int64_t B, int64_t T, int64_t C, float* loss, float* dP, int64_t lddp,
